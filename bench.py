@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W          (N>1: launched under torchrun)
     python bench.py --impl reference ...                   CPU arm: the oracle port, all host threads
+    python bench.py ... --dump-outputs DIR                 also write the last timed step's outputs as DIR/*.npy
 
 A "step" is ONE synchronous MaxSum cycle over the whole factor graph: every factor->variable
 min-marginal and every variable->factor message recomputed (2*E edge-message updates), damping,
@@ -36,7 +37,7 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": 3350.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -167,7 +168,7 @@ def reference_threadmode(seconds=10):
         lines += ["agents:"] + [f"  a{i:03d}: {{capacity: 1000}}" for i in range(300)]
         c2f = os.path.join(td, "c2_family_v100.yaml")
         open(c2f, "w").write("\n".join(lines) + "\n")
-        c1 = os.path.join(ref_shim.REFERENCE_ROOT, "tests", "instances", "graph_coloring_10_4_15_0.1.yml")
+        c1 = os.path.join(ref_shim.INSTANCES, "graph_coloring_10_4_15_0.1.yml")
         for name, path, n_edges, dist in (("C1 graph_coloring_10_4_15_0.1.yml", c1, 24, "adhoc"),
                                           ("C2-family V=100 d=10 F=200", c2f, 400, "oneagent")):
             code = ("import sys; sys.path[:0] = [%r]\nimport ref_shim; ref_shim.install()\n"
@@ -188,6 +189,42 @@ def reference_threadmode(seconds=10):
             except Exception as ex:  # noqa: BLE001 — a baseline must not cost the measured line
                 out.append({"kind": "reference-threadmode", "unavailable": f"{name}: {ex!r}"[:300]})
     return out
+
+
+DUMP_BYTES = 64 << 20      # --dump-outputs: at most this many bytes in all
+DUMP_SAMPLE = 1 << 20      # elements kept of each large array when the whole set would not fit
+
+
+def engine_outputs(eng, precision):
+    """What a caller of the timed engine receives after a step: the assignment (value indices) and, where the
+    engine reports them, the per-variable costs and MaxSum's messages (q, r), all in canonical order.  Values in
+    the engine's precision; indices as float64 (exact)."""
+    ft = np.float32 if precision == "f32" else np.float64
+    v = eng.values()
+    out = {}
+    if isinstance(v, tuple):
+        out["value"], out["value_cost"] = np.asarray(v[0], np.float64), np.asarray(v[1], ft)
+    else:
+        out["value"] = np.asarray(v, np.float64)
+    if hasattr(eng, "messages"):
+        q, r = eng.messages()
+        out["q"], out["r"] = q.astype(ft), r.astype(ft)
+    return out
+
+
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy for every array.  When the whole set exceeds DUMP_BYTES, every array longer than DUMP_SAMPLE
+    is replaced by a fixed sample of DUMP_SAMPLE elements (numpy default_rng(0), sorted positions), and the positions
+    go to DIR/<name>_index.npy (float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    sample = sum(a.nbytes for a in arrays.values()) > DUMP_BYTES
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a).reshape(-1)
+        if sample and a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def _partition_cache_path(inst, world, part):
@@ -283,6 +320,10 @@ def side_workload(args, dev):
         evs.append((a, b))
     torch.cuda.synchronize(dev)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        outs = engine_outputs(eng, args.precision)    # collective for a sharded engine: every rank calls it
+        if rank == 0:
+            dump_outputs(args.dump_outputs, outs)
     ms = sum(a.elapsed_time(b) for a, b in evs) / args.steps
     parity = None
     breakdown = None
@@ -360,7 +401,10 @@ def main():
                     help="c2 (default, the driver's line) | c3 Ising 1024^2 | c5 arity-3 | target 1M vars "
                          "| c4 DSA 1M vars d=20 (variable updates/s) | mgm: MGM on the c4 instance")
     ap.add_argument("--profile", action="store_true",
-                    help="lean run for ncu: init + warmup + steps back to back, no flush/e2e/JSON")
+                    help="lean run for a profiler: init + warmup + steps back to back, no flush/e2e/JSON")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy "
+                         "(float32 / float64, at most 64 MiB in all; a fixed sample of larger outputs)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -482,6 +526,10 @@ def main():
         dist.barrier()
     launches = runner.launch_count - l0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        outs = engine_outputs(runner, args.precision)    # collective for a sharded engine: every rank calls it
+        if rank == 0:
+            dump_outputs(args.dump_outputs, outs)
     ms = sum(a.elapsed_time(b) for a, b in evs)
     if world > 1:
         t = torch.tensor([ms], device=dev, dtype=torch.float64)
@@ -561,10 +609,6 @@ def main():
         return
     peaks, peak_kind = load_peaks()
     peak = float(peaks["hbm_gbs"])
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r02_traffic_c2_f32.json")   # the final round-2 kernels (k_f2v_warp + k_v2f_warp)
-    if world == 1 and args.precision == "f32" and args.vars_per_gpu == 100_000 and os.path.exists(tpath):
-        traffic = json.load(open(tpath))["per_step_bytes"]   # from the committed ncu --set full capture
     per_gpu_bytes = alg_bytes / max(1, world)
     achieved = per_gpu_bytes / (ms_per_step * 1e-3) / 1e9
     line = {
@@ -573,16 +617,11 @@ def main():
         "scaling": "weak", "vs_baseline": None, "dtype": args.precision, "data": "synthetic",
         "config": config, "clocks": clocks, "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic,
-                     "traffic_source": ("constant from the committed ncu --set full capture profiles/r02_traffic_c2_f32.json "
-                                        "(dram__bytes_read + dram__bytes_write of one launch of each kernel of this build), "
-                                        "not a measurement of this run"
-                                        if traffic is not None else None),
-                     "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({peak_kind})",
+                     "frac": achieved / peak,
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peak_kind == "measured" else peak_kind,
                      "algorithmic_bytes_per_step": int(per_gpu_bytes),
                      "bytes_per_update": alg_bytes / updates_per_step,
-                     "kernel": "f2v + v2f kernels of one cycle (whole step; per-kernel split in "
-                               "profiles/)"},
+                     "kernel": "f2v + v2f kernels of one cycle (whole step)"},
         "e2e": e2e,
     }
     if run_info:

@@ -1,4 +1,4 @@
-/* pydcop_b200 — C-ABI of the B200-native factor-graph message-passing engine.
+/* pydcop_b200 — C-ABI of the factor-graph message-passing engine (H100, sm_90a).
  *
  * The reference (Orange-OpenSource/pyDcop) is pure Python and has NO FFI: its boundary for this
  * path is the algorithm-module surface `pydcop.algorithms.<name>` (GRAPH_TYPE / algo_params /

@@ -42,7 +42,7 @@ import pydcop.algorithms.dsa as ref_dsa  # noqa: E402
 import pydcop.infrastructure.computations as ref_computations  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(HERE), "tests", "golden")
-INSTANCES = os.path.join(ref_shim.REFERENCE_ROOT, "tests", "instances")
+INSTANCES = ref_shim.INSTANCES
 
 
 # --------------------------------------------------------------------------------------

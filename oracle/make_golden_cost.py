@@ -64,7 +64,7 @@ def main():
             constraints.append(NAryMatrixRelation(scope, m, name=f"c{j:02d}"))
         problems.append({"name": f"random_inf_{inf:g}", "infinity": inf, **arrays(variables, constraints),
                          "cases": cases_for(variables, constraints, inf, rng, 12)})
-    dcop = load_dcop_from_file([os.path.join(G.ref_shim.REFERENCE_ROOT, "tests", "instances",
+    dcop = load_dcop_from_file([os.path.join(G.ref_shim.INSTANCES,
                                              "graph_coloring_10_4_15_0.1.yml")])
     variables = list(dcop.variables.values())
     constraints = list(dcop.constraints.values())

@@ -1,4 +1,4 @@
-"""pydcop_b200 — B200-native batched factor-graph message passing for pyDcop's MaxSum / DSA hot path.
+"""pydcop_b200 — batched factor-graph message passing on the H100 for pyDcop's MaxSum / DSA hot path.
 
 Public API:
     build_layout / layout_from_instance   host packing of a factor graph (pydcop_b200.layout)

@@ -1,4 +1,4 @@
-"""pyDcop algorithm modules backed by the B200 engine.
+"""pyDcop algorithm modules backed by the GPU engine.
 
 This directory is appended to `pydcop.algorithms.__path__` (see pydcop_b200.launcher.install),
 after which the unmodified reference lists and loads `maxsum_gpu` / `dsa_gpu` like its own

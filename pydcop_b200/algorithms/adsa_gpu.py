@@ -1,4 +1,4 @@
-"""adsa_gpu — drop-in pyDcop algorithm module: A-DSA on the B200 engine.
+"""adsa_gpu — drop-in pyDcop algorithm module: A-DSA on the GPU engine.
 
 Same module surface as the reference's `pydcop/algorithms/adsa.py` (GRAPH_TYPE :100, algo_params :121-125:
 period 0.5, probability 0.7, variant B; memory / load models as DSA's).  The reference's computation is

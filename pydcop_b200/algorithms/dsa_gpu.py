@@ -1,4 +1,4 @@
-"""dsa_gpu — drop-in pyDcop algorithm module: DSA-A/B/C on the B200 engine.
+"""dsa_gpu — drop-in pyDcop algorithm module: DSA-A/B/C on the GPU engine.
 
 Same module surface as the reference's `pydcop/algorithms/dsa.py` (GRAPH_TYPE :114, algo_params
 :130-135, computation_memory :138-160, communication_load :163-184; build_computation is what

@@ -1,4 +1,4 @@
-"""maxsum_gpu — drop-in pyDcop algorithm module: synchronous MaxSum on the B200 engine.
+"""maxsum_gpu — drop-in pyDcop algorithm module: synchronous MaxSum on the GPU engine.
 
 Same module surface as the reference's `pydcop/algorithms/maxsum.py` (GRAPH_TYPE :103,
 algo_params :212-220, build_computation :118-124, computation_memory :127-171,

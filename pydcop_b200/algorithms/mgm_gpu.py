@@ -1,4 +1,4 @@
-"""mgm_gpu — drop-in pyDcop algorithm module: MGM on the B200 engine.
+"""mgm_gpu — drop-in pyDcop algorithm module: MGM on the GPU engine.
 
 Same module surface as the reference's `pydcop/algorithms/mgm.py` (GRAPH_TYPE :68, algo_params
 :78-81, computation_memory :84-110, communication_load :113-133; build_computation is what

@@ -1,7 +1,7 @@
-"""Builds the C-ABI shared library in-tree: pydcop_b200/lib/libpydcop_b200.so (sm_100a only).
+"""Builds the C-ABI shared library in-tree: pydcop_b200/lib/libpydcop_b200.so (sm_90a, H100, only).
 
-nvcc cross-compiles without a GPU, so this runs in the CPU build container; the built .so travels
-to the GPU box with the repo snapshot (it is git-ignored, not gpurun-ignored).
+nvcc cross-compiles without a GPU, so the library can be built on a machine without one; it is a
+build product and stays out of git.
 """
 import os
 import shutil
@@ -14,7 +14,7 @@ LIB_DIR = os.path.join(PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libpydcop_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-fmad=false",           # keep the reference's operand order: no FMA contraction (bit parity)
     "--extended-lambda", "-shared", "-Xcompiler", "-fPIC", "-diag-suppress", "177",
 ]

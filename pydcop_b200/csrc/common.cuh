@@ -1,4 +1,4 @@
-// Shared device helpers for the factor-graph kernels (sm_100a).
+// Shared device helpers for the factor-graph kernels (sm_90a).
 // Arithmetic note: every floating-point expression below keeps the operand ORDER of the
 // reference (pydcop/algorithms/maxsum.py) and the file is compiled with -fmad=false, so the
 // f64 instantiation is bit-identical to the reference's Python floats and the f32 instantiation

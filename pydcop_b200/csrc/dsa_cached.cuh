@@ -2,9 +2,8 @@
 //
 // evaluate_cycle (dsa.py:320-357) needs, per incident constraint, ONE row of D costs of the table oriented
 // towards the variable: the row of the neighbour's current value.  Read from the oriented tables
-// (dsa_fast.cuh) that is one random 128-byte line per incidence — ncu on C4: DRAM at 33 % of peak with 6 %
-// issue utilisation; tools/gather_peak.py shows that this is what random lines reach on HBM3e with nothing
-// else going on.  But a neighbour's value changes rarely once DSA has taken its first steps, and the row is
+// (dsa_fast.cuh) that is one random 128-byte line per incidence, and random lines are all HBM delivers to
+// that pattern (tools/gather_peak.py measures it alone).  But a neighbour's value changes rarely once DSA has taken its first steps, and the row is
 // a function of that value alone.  So the engine keeps, per slot, the row it read last in a slot-major array
 // (`row_cache`, the rows of one variable contiguous, variables in kernel order) next to the neighbour value
 // it belongs to (`slot_last`); a cycle
@@ -13,8 +12,7 @@
 //      from the oriented table and replaces it in shared memory and in the array,
 //   3. sums the rows per variable in slot order, one thread per variable with its D costs in registers —
 //      the same adds in the same order as k_dsa_step_bin, so the result is bit-identical — and runs the
-//      decision rule.  (A first version summed per (variable, value) item: 130 M instructions per cycle on
-//      C4, 398 us; profiles/r02_call11_*.)
+//      decision rule.
 // The bytes that cross HBM per cycle are the algorithmic ones (one row per incidence, SURVEY §8d), now
 // sequential; a cycle in which EVERY neighbour changed costs what the uncached kernel costs plus the
 // write-back.  slot_last = 0xFF (fg_dsa_init) marks a row as not yet read.

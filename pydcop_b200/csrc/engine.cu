@@ -47,9 +47,8 @@ struct fg_maxsum {
   bool chained_now = false; // the cycle being enqueued was closed inside phase 0
   cudaEvent_t ev_r = nullptr;
   // early q push (EXPERIMENT, PYDCOP_B200_PUSH_EARLY=1|2): the variable classes with a remote factor (FG_CLASS_BOUNDARY) are
-  // launched first and their rows leave while the interior classes are still being computed.  The device-timed cycle
-  // improves (88 -> 87 us at N = 2, more as the cut grows) but 300 back-to-back enqueued cycles collapse to 330-445 us per
-  // cycle (profiles/r02_call18_*, r02_call21_*): not understood yet, so off by default
+  // launched first and their rows leave while the interior classes are still being computed.  Many back-to-back
+  // enqueued cycles run slower with it, for a reason not understood yet, so it is off by default
   bool early_q = false;
   int early_mode = 1;   // 1: the q push follows the r push on the main stream; 2: on a third stream (PYDCOP_B200_PUSH_EARLY=2)
   cudaStream_t push_stream = nullptr;
@@ -212,8 +211,8 @@ static int maxsum_compute_t(fg_maxsum *h, cudaStream_t st, bool push_split = fal
   const int cur = h->cur, nxt = cur ^ 1;
   // The generic kernels of cycle 1 consult the validity arrays.  The buffers are zero-filled at init and
   // a never-sent message counts as zeros in every sum (maxsum.py:430-436, 656-661), so the tiled
-  // kernels, which read every row, compute the same values in cycle 1 too (default; validated on the
-  // B200 against the generic kernels and the oracle, tests/test_gpu_zz_fast_first.py).
+  // kernels, which read every row, compute the same values in cycle 1 too (default; checked against the
+  // generic kernels and the oracle by tests/test_gpu_zz_fast_first.py).
   const bool first = (h->cycle == 0) && !h->fast_first;
   const bool first_cycle = (h->cycle == 0);
   MaxSumParams p{d.mode_max, d.damp_vars, d.damp_factors, d.damping, 1.0 - d.damping, d.stability, nullptr, nullptr};
@@ -416,12 +415,12 @@ extern "C" int fg_maxsum_shard_attach(fg_maxsum_t h, const fg_halo_plan_t *plan)
   h->halo = *plan;
   h->has_halo = true;
   h->epoch = 0;
-  { const char *e = getenv("PYDCOP_B200_PUSH_SPLIT"); h->split_push = !(e && e[0] == '0'); }   // default on: 102 vs 177 us at N=2
+  { const char *e = getenv("PYDCOP_B200_PUSH_SPLIT"); h->split_push = !(e && e[0] == '0'); }   // default on
   // fused halo: every class that produces rows must run on a warp kernel (they carry the peer stores)
   bool all_warp = plan->dev_edge_dst_r[0] && plan->dev_edge_dst_r[1] && plan->dev_slot_dst_q[0] && plan->dev_slot_dst_q[1] &&
                   h->warp.v2f_on && h->fast.slow_varclasses.empty() && fg_env_is("PYDCOP_B200_PUSH_FUSED", '1') &&
-                  fg_env_int("PYDCOP_B200_F2VW_NS", 2) == 2 && fg_env_int("PYDCOP_B200_V2FW_NS", 2) == 2;   // opt-in: faster at N = 2
-                  // (82 vs 89 us) but the stores stall the compute kernels once the cut grows (N = 8: 157 vs 123 us)
+                  fg_env_int("PYDCOP_B200_F2VW_NS", 2) == 2 && fg_env_int("PYDCOP_B200_V2FW_NS", 2) == 2;   // opt-in: the stores stall the
+                  // compute kernels more as the cut grows
   for (size_t i = 0; all_warp && i < h->classes.size(); ++i)
     if (h->classes[i].n_factors && !(h->classes[i].flags & FG_CLASS_GHOST) && !h->warp.f2v[i]) all_warp = false;
   h->fused_push = all_warp;

@@ -3,8 +3,7 @@
 // the factor's on_new_cycle (maxsum.py:339-379) with RUNTIME dimensions and compile-time arity.
 //
 // The one-thread-per-edge kernel (maxsum_generic.cuh) reads each table `arity` times with a stride of one
-// table between neighbouring threads — 3.5 % of the HBM roofline on C2 (profiles/r01_bench_v0_generic_kernels.json),
-// and a class of few large tables (arity 4 over 12 values: 83 KB each) keeps a handful of threads busy for
+// table between neighbouring threads, and a class of few large tables (arity 4 over 12 values: 83 KB each) keeps a handful of threads busy for
 // tens of milliseconds.  Here a CTA owns a run of consecutive factors of one class: their tables, their
 // previous messages and their output rows are CONTIGUOUS in the class-major layout, so every byte crosses
 // HBM once, in coalesced requests; only the incoming q rows are gathered (one row per edge, via edge_qoff).
@@ -46,9 +45,19 @@ struct TiledRtCfg {
 
 inline int tiled_rt_pow2_ge(int d) { int g = 1; while (g < d && g < 32) g *= 2; return g; }
 // tables up to this many entries: one lane per output value walks its whole slice (the lane-group / parts split
-// costs more in index arithmetic and shuffles than the bank conflicts of a small table; B200, mixed-shape side
-// workload: arity 2 197 -> 344 us, arity 3 279 -> 425 us with the split, arity 4 1019 -> 437 us)
+// costs more in index arithmetic and shuffles than the bank conflicts of a small table)
 constexpr int64_t FG_TILED_RT_WIDE = 2048;
+
+// SMs of the current device (queried once): the tile size spreads a class over about 6 tiles per SM
+inline int tiled_rt_n_sm() {
+  static int n_sm = 0;
+  if (!n_sm) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n_sm <= 0) n_sm = 1;
+  }
+  return n_sm;
+}
 
 inline TiledRtCfg tiled_rt_cfg(const fg_class_t &c, size_t elem) {
   TiledRtCfg r;
@@ -63,7 +72,7 @@ inline TiledRtCfg tiled_rt_cfg(const fg_class_t &c, size_t elem) {
   int64_t threads = ((wide && a >= 3) ? (int64_t)c.dom[0] : 1) * d_last;     // lanes a factor keeps busy
   for (int j = 0; j + 1 < a; ++j) threads += (int64_t)c.dom[j] * (wide ? tiled_rt_pow2_ge(d_last) : 1);
   const int64_t want = std::max<int64_t>(1, (2 * FG_TILED_RT_THREADS + threads - 1) / threads);
-  const int64_t spread = std::max<int64_t>(1, c.n_factors / (148 * 6));
+  const int64_t spread = std::max<int64_t>(1, c.n_factors / ((int64_t)tiled_rt_n_sm() * 6));
   const int64_t target = std::max(want, std::min<int64_t>(spread, 4 * want));
   const int64_t per = sp * (int64_t)elem + rows;
   if (per <= (int64_t)FG_TILED_RT_SMEM) {

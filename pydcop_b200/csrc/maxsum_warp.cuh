@@ -1,11 +1,9 @@
-// Warp-autonomous MaxSum kernels (round 2): every warp runs its OWN software pipeline over its own
+// Warp-autonomous MaxSum kernels: every warp runs its OWN software pipeline over its own
 // tiles — its own shared-memory stages, its own mbarriers and cp.async groups — so there is no
-// block-wide barrier anywhere (round 1's k_v2f_pipe spent 45 % of its issue slots parked at
-// __syncthreads, profiles/r01_final_ncu_v2f_pipe_c2.txt), and the arithmetic is written for the issue
-// slots it costs: ncu showed both sides of the cycle bounded by instruction issue (30-40 % issue
-// utilisation at 1-2 warps per scheduler, DRAM at 12-40 %, profiles/r02_ncu_*_warp_v1.txt), so
-//   * add chains run as packed fp32x2 instructions (FADD2 / FMUL2) and optima as 3-input FMNMX3
-//     (packed.cuh) — every element still gets the correctly rounded IEEE operation of the scalar code;
+// block-wide barrier anywhere (the CTA-pipelined k_v2f_pipe spends much of its issue slots parked at
+// __syncthreads), and the arithmetic is written for the issue slots it costs, so
+//   * rows are handled as value pairs (packed.cuh) — every element gets the correctly rounded IEEE
+//     operation of the scalar code;
 //   * min / max is a template parameter, tile descriptors are arithmetic from a per-class table staged in
 //     shared memory (no dependent global load on the critical path), lane -> (variable, slot) uses a
 //     reciprocal from that table.
@@ -468,8 +466,7 @@ inline bool launch_v2f_warp_ns(const WClassEntry *dev_classes, const WTileRange 
   }
 }
 
-// pipeline depth: PYDCOP_B200_V2FW_NS = 2 | 3 | 4 stages per warp (default 2: 12 warps x 2 stages per SM measured
-// faster on C2 than 8 x 3, profiles/r02_call5_sweep.txt)
+// pipeline depth: PYDCOP_B200_V2FW_NS = 2 | 3 | 4 stages per warp (default 2)
 template <typename T, int D>
 inline void launch_v2f_warp(const WClassEntry *dev_tiles, const WTileRange &rg, const fg_maxsum_desc_t &d, const T *r_cur,
                             const T *q_cur, T *q_next, const MaxSumParams &p, cudaStream_t st) {

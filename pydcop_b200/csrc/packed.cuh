@@ -1,12 +1,9 @@
-// Packed arithmetic helpers for the warp-autonomous kernels (sm_100a).
+// Pair arithmetic helpers for the warp-autonomous kernels (sm_90a).
 //
-// Blackwell issues two IEEE fp32 operations per lane with ONE instruction (SASS FADD2 / FMUL2, PTX
-// add / sub / mul .rn.f32x2) and takes three inputs in one min / max (FMNMX3).  The kernels of this
-// engine are bounded by instruction issue, not by arithmetic (ncu: 30-40 % issue utilisation at 1-2
-// warps per scheduler, DRAM 12-40 %), so halving the instruction count of the add / min chains is worth
-// more than any reordering.  Every operation here is the correctly rounded IEEE operation on each
-// element: results are bit-identical to the scalar code (and to the CPU oracle); no FMA contraction.
-// double has no packed form: the same helpers fall back to two scalar operations.
+// The kernels keep message rows as pairs of values (float2 / double2) so that loads and stores move 8 or
+// 16 bytes per lane.  Hopper has no packed fp32 add / mul and no three-input min / max, so every helper is
+// one correctly rounded IEEE operation per element (__fadd_rn / __fsub_rn / __fmul_rn are never contracted
+// into an FMA): results are bit-identical to the scalar code and to the CPU oracle.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -17,31 +14,12 @@ template <typename T> struct Pair;
 template <> struct Pair<float> { using type = float2; };
 template <> struct Pair<double> { using type = double2; };
 
-__device__ __forceinline__ float2 padd(float2 a, float2 b) {
-  float2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<uint64_t &>(r)) : "l"(reinterpret_cast<uint64_t &>(a)), "l"(reinterpret_cast<uint64_t &>(b)));
-  return r;
-}
-__device__ __forceinline__ float2 psub(float2 a, float2 b) {
-  float2 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<uint64_t &>(r)) : "l"(reinterpret_cast<uint64_t &>(a)), "l"(reinterpret_cast<uint64_t &>(b)));
-  return r;
-}
-__device__ __forceinline__ float2 pmul(float2 a, float2 b) {
-  float2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<uint64_t &>(r)) : "l"(reinterpret_cast<uint64_t &>(a)), "l"(reinterpret_cast<uint64_t &>(b)));
-  return r;
-}
-__device__ __forceinline__ double2 padd(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ double2 psub(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }
-__device__ __forceinline__ double2 pmul(double2 a, double2 b) { return make_double2(a.x * b.x, a.y * b.y); }
-
-// a + b with the two sums as SCALAR correctly-rounded adds (__fadd_rn is never contracted): ptxas fuses a
-// packed mul.rn.f32x2 feeding a packed add.rn.f32x2 into FFMA2 — one rounding instead of two, which broke bit
-// parity of the damping step for damping != 0.5 (seen on the B200, r02 call 5) — so wherever the inputs of
-// an add are products, the add must not be the packed form.
-__device__ __forceinline__ float2 padd_noncontract(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-__device__ __forceinline__ double2 padd_noncontract(double2 a, double2 b) { return make_double2(__dadd_rn(a.x, b.x), __dadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 padd(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 psub(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 pmul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ double2 padd(double2 a, double2 b) { return make_double2(__dadd_rn(a.x, b.x), __dadd_rn(a.y, b.y)); }
+__device__ __forceinline__ double2 psub(double2 a, double2 b) { return make_double2(__dsub_rn(a.x, b.x), __dsub_rn(a.y, b.y)); }
+__device__ __forceinline__ double2 pmul(double2 a, double2 b) { return make_double2(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)); }
 
 template <typename T> __device__ __forceinline__ typename Pair<T>::type pmake(T x, T y);
 template <> __device__ __forceinline__ float2 pmake<float>(float x, float y) { return make_float2(x, y); }
@@ -50,15 +28,10 @@ template <> __device__ __forceinline__ double2 pmake<double>(double x, double y)
 // optimum of two / three values; MX: max instead of min.  NaN operands are ignored like fminf / fmaxf.
 template <bool MX> __device__ __forceinline__ float opt2(float a, float b) { return MX ? fmaxf(a, b) : fminf(a, b); }
 template <bool MX> __device__ __forceinline__ double opt2(double a, double b) { return MX ? fmax(a, b) : fmin(a, b); }
-template <bool MX> __device__ __forceinline__ float opt3(float a, float b, float c) {
-  float r;
-  if (MX) asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  else asm("min.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
+template <bool MX> __device__ __forceinline__ float opt3(float a, float b, float c) { return opt2<MX>(opt2<MX>(a, b), c); }
 template <bool MX> __device__ __forceinline__ double opt3(double a, double b, double c) { return opt2<MX>(opt2<MX>(a, b), c); }
 
-// optimum of N values held in registers (static indices): 3-input tree
+// optimum of N values held in registers (static indices): tree of three-way optima
 template <bool MX, typename T, int N>
 __device__ __forceinline__ T opt_tree3(const T (&v)[N]) {
   if constexpr (N == 1) {
@@ -97,7 +70,7 @@ __device__ __forceinline__ bool damp_match_pairs(T (&cand)[N], const T (&prev)[N
   for (int i = 0; i < N / 2; ++i) {
     const P p = pmake<T>(prev[2 * i], prev[2 * i + 1]);
     P c = pmake<T>(cand[2 * i], cand[2 * i + 1]);
-    if (damp_side) c = padd_noncontract(pmul(lam2, p), pmul(oml2, c));   // lam * prev + (1 - lam) * c: three roundings
+    if (damp_side) c = padd(pmul(lam2, p), pmul(oml2, c));   // lam * prev + (1 - lam) * c: three roundings
     cand[2 * i] = c.x;
     cand[2 * i + 1] = c.y;
     const P s = padd(p, c);
@@ -140,7 +113,7 @@ __device__ __forceinline__ void damp_match_pairs2(T (&cand)[N], const T (&prev)[
   for (int i = 0; i < N / 2; ++i) {
     const P p = pmake<T>(prev[2 * i], prev[2 * i + 1]);
     P c = pmake<T>(cand[2 * i], cand[2 * i + 1]);
-    if (damp_side) c = padd_noncontract(pmul(lam2, p), pmul(oml2, c));
+    if (damp_side) c = padd(pmul(lam2, p), pmul(oml2, c));
     cand[2 * i] = c.x;
     cand[2 * i + 1] = c.y;
     const P s = padd(p, c);

@@ -31,8 +31,7 @@ __host__ __device__ __forceinline__ void fg_load_row(const T *__restrict__ p, T 
 // Oriented DSA / MGM tables keep every row on its own cache-line slot: a row of D elements is stored with
 // stride fg_row_stride<T, D>() = the next power of two >= D (rounded to whole 128-byte lines above 128 bytes),
 // so the ONE row a slot reads per cycle costs one or two whole DRAM lines instead of the 1.5 lines an
-// unaligned 80-byte row averaged (ncu on C4: 1.31 GB of DRAM reads for 584 MB of algorithmic bytes,
-// profiles/r02_ncu_dsa_step_c4_baseline.txt).  pydcop_b200/engine.py::dsa_row_stride is the same rule.
+// unaligned 80-byte row averaged.  pydcop_b200/engine.py::dsa_row_stride is the same rule.
 template <typename T, int D>
 __host__ __device__ constexpr int fg_row_stride() {
   int p2 = 1;

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers (sm_100a): 1-D bulk async copies (TMA, SASS UBLKCP) with mbarrier
+// Thin inline-PTX wrappers (sm_90a): 1-D bulk async copies (TMA, SASS UBLKCP) with mbarrier
 // completion, bulk stores, and 16-byte cp.async (LDGSTS).
 #pragma once
 #include <cuda_runtime.h>

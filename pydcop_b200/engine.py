@@ -1,7 +1,7 @@
-"""Python host of the B200 engine: device memory (torch), streams, and the C-ABI calls.
+"""Python host of the GPU engine: device memory (torch), streams, and the C-ABI calls.
 
 `MaxSumEngine` / `DsaEngine` are what the pyDcop plugin modules (pydcop_b200/algorithms/) and
-bench.py drive.  All arithmetic on messages happens in libpydcop_b200.so (hand-written sm_100a
+bench.py drive.  All arithmetic on messages happens in libpydcop_b200.so (hand-written sm_90a
 kernels); torch only owns the buffers.  There is no CPU path: constructing an engine without a
 CUDA device raises EngineError.
 """
@@ -620,8 +620,7 @@ class MgmEngine(_EngineBase):
         d.dev_gain, d.dev_new_value = _ptr(self.gain), _ptr(self.new_value)
         d.mode_max, d.stop_cycle, d.seed = int(mode == "max"), int(stop_cycle), int(seed) & (2 ** 64 - 1)
         # the fast value-phase kernel on the DSA fast-path arrays (binary constraints over one domain size
-        # in {4, 8, 10, 16, 20}); 2 incidences per trip measured fastest on the B200 (C4 instance: 605 us
-        # per cycle vs 1869 us generic, profiles/r02_call1_pending_summary.txt).  PYDCOP_B200_MGM_FAST=0|2|4
+        # in {4, 8, 10, 16, 20}), 2 incidences per trip by default.  PYDCOP_B200_MGM_FAST=0|2|4
         self.fast_chunk = 0
         chunk = int(os.environ.get("PYDCOP_B200_MGM_FAST", "2") or 0)
         if chunk in (2, 4):

@@ -1,6 +1,6 @@
 """bench.py's contract on CPU: the reference arm prints ONE JSON line with the required keys; the
 GPU arm refuses to run without a device (no CPU fallback); under a multi-rank launch only rank 0
-of the reference arm prints.  (The GPU arm's own line is checked where it runs, on the B200.)"""
+of the reference arm prints.  (The GPU arm's own line is checked where it runs, on the H100.)"""
 import json
 import os
 import subprocess

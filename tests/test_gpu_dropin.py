@@ -22,7 +22,7 @@ pytestmark = [pytest.mark.gpu,
                                  reason="no reference: neither /root/reference nor baseline/_ref")]
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INSTANCES = os.path.join(ref_shim.REFERENCE_ROOT, "tests", "instances")
+INSTANCES = ref_shim.INSTANCES
 
 
 def _cli(args, tmp_path, timeout=240):

@@ -1,4 +1,4 @@
-"""GPU parity (run on the B200 box): CUDA engine through the C-ABI vs the CPU oracle and vs the
+"""GPU parity (run on an H100): CUDA engine through the C-ABI vs the CPU oracle and vs the
 reference's own lock-step trajectories (tests/golden, made from the unmodified reference).
 
 Bar (north_star): integer assignments bit-exact; float messages within 1e-5 relative.  What is

@@ -1,7 +1,7 @@
 """YAML / object / binary ingestion (pydcop_b200/ingest.py, SURVEY.md §8(f).2) against what the
 UNMODIFIED reference loader produces (tests/golden/ingest_expected.json, written by
-oracle/make_golden_ingest.py) and, when /root/reference is importable, against the reference's own
-test instances."""
+oracle/make_golden_ingest.py) and against what it makes of its own test instances
+(tests/golden/reference_expected.json + reference_tables.npz, written by oracle/make_golden_reference.py)."""
 import glob
 import itertools
 import json
@@ -274,7 +274,7 @@ def test_from_dcop_objects():
         ingest.from_dcop(None, variables=[x])
 
 
-# ---- the reference's own instances (only where /root/reference exists) --------------------------
+# ---- the reference's own instances (tests/golden/instances) -------------------------------------
 def _reference():
     import ref_shim
     if not ref_shim.reference_available():
@@ -284,9 +284,37 @@ def _reference():
 
 
 def test_reference_test_instances_load_identically():
+    """Names in the reference's order and every table (axes in sorted name order) as the reference's loader
+    makes them of its own test instances (stored: tests/golden/instances, reference_expected.json,
+    reference_tables.npz)."""
+    ref_exp = json.load(open(os.path.join(HERE, "golden", "reference_expected.json")))["instances"]
+    ref_tab = np.load(os.path.join(HERE, "golden", "reference_tables.npz"))
+    files = sorted(glob.glob(os.path.join(HERE, "golden", "instances", "*.y*ml")))
+    assert len(files) >= 10 and sorted(os.path.basename(f) for f in files) == sorted(ref_exp)
+    n = 0
+    for fn in files:
+        want = ref_exp[os.path.basename(fn)]
+        if want["external_variables"]:
+            with pytest.raises(NotImplementedError):
+                ingest.load_yaml(fn)
+            continue
+        d = ingest.load_yaml(fn)
+        assert d.var_names == want["var_names"] and d.con_names == want["con_names"]
+        for ci, cn in enumerate(d.con_names):
+            scope, table = sorted_axis_table(d, ci)
+            key = os.path.basename(fn) + "/" + cn
+            assert scope == want["scopes"][cn] and table.tolist() == ref_tab[key].tolist(), (fn, cn)
+        n += 1
+    assert n >= 10
+
+
+def test_reference_test_instances_load_like_the_live_reference():
+    """Where the reference is importable: every one of its own test instances (the ones with external python
+    sources included) through its loader and through the ingestion, and the object route (from_dcop) gives the
+    same arrays as the text route."""
     shim = _reference()
     from pydcop.dcop.yamldcop import load_dcop_from_file
-    files = sorted(glob.glob(os.path.join(shim.REFERENCE_ROOT, "tests", "instances", "*.y*ml")))
+    files = sorted(glob.glob(os.path.join(shim.REFERENCE_INSTANCES, "*.y*ml")))
     assert len(files) >= 10
     n = 0
     for fn in files:

@@ -15,7 +15,7 @@ import ref_shim
 pytestmark = pytest.mark.skipif(not ref_shim.reference_available(),
                                 reason="reference tree not present (GPU box)")
 
-INSTANCES = os.path.join(ref_shim.REFERENCE_ROOT, "tests", "instances")
+INSTANCES = ref_shim.REFERENCE_INSTANCES
 
 
 def retry_once(fn):
