@@ -33,6 +33,14 @@ def maxsum_case(rng):
               "stability": float(rng.choice([0.001, 0.1, 0.5])),
               "start_messages": str(rng.choice(["leafs", "leafs_vars", "all"])), "noise": 0.0}
     mode = str(rng.choice(["min", "max"]))
+    hard = bool(rng.random() < 0.4)
+    if hard:   # hard constraints: forbidden cells, and variables with every value forbidden
+        inf = np.inf if mode == "min" else -np.inf
+        for c in cs:
+            if len(c.dimensions) > 1 and rng.random() < 0.5:
+                c._m[rng.random(c._m.shape) < 0.3] = inf
+        for j, i in enumerate(rng.choice(n_vars, size=int(rng.integers(1, 3)), replace=False)):
+            cs.append(G.NAryMatrixRelation([vs[int(i)]], np.full(len(vs[int(i)].domain), inf), name=f"h{j:03d}"))
     arr, meta = G.run_maxsum(vs, cs, params, mode, 10, seed=int(rng.integers(1, 1000)))
     p = {k: v for k, v in params.items() if k != "noise"}
     o = orc.MaxSumOracle(arr, np.float64, mode=mode, **p).init()
@@ -41,10 +49,10 @@ def maxsum_case(rng):
             o.step()
         if not (np.array_equal(o.q, arr["q_state"][k], equal_nan=True) and np.array_equal(o.r, arr["r_state"][k], equal_nan=True)
                 and np.array_equal(o.q_sent, arr["q_sent"][k]) and np.array_equal(o.r_sent, arr["r_sent"][k])):
-            return f"maxsum messages differ at cycle {k}: {params} {mode} scale={scale}"
+            return f"maxsum messages differ at cycle {k}: {params} {mode} scale={scale} hard={hard}"
         if not np.array_equal(o.value, arr["value"][k]):
             # reported selection: ties at the ulp level are arrival-order dependent in the reference
-            return None if scale != 1.0 else f"maxsum values differ at cycle {k}: {params} {mode}"
+            return None if scale != 1.0 else f"maxsum values differ at cycle {k}: {params} {mode} hard={hard}"
     return None
 
 

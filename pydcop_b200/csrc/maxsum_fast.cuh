@@ -242,7 +242,7 @@ __device__ __forceinline__ void f2v_compute_tile(const T *__restrict__ tab, cons
             ld_row<T, D, C::VT>(tf + (x_lo + i) * D, row);
 #pragma unroll
             for (int x1 = 0; x1 < D; ++x1) row[x1] = row[x1] + qo[x1];
-            cand[i] = opt_tree<T, D>(row, mx);
+            cand[i] = fg_opt<T>(init, opt_tree<T, D>(row, mx), mx);   // all candidates NaN: +/-inf, as the reference
           }
         } else {
 #pragma unroll
@@ -273,7 +273,7 @@ __device__ __forceinline__ void f2v_compute_tile(const T *__restrict__ tab, cons
               for (int x2 = 0; x2 < D; ++x2) row[x2] = row[x2] + (q1[x1] + q2[x2]);
               part[x1] = opt_tree<T, D>(row, mx);
             }
-            of[i] = opt_tree<T, D>(part, mx);
+            of[i] = fg_opt<T>(init, opt_tree<T, D>(part, mx), mx);
           }
           ld_row<T, HD, C::VH>(of, cand);
         } else if (j == 1) {

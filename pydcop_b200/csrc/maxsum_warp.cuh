@@ -738,8 +738,9 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
           part[x] = opt3<MX>(part[x], ua.x, ub.x);
           part[x + 1] = opt3<MX>(part[x + 1], ua.y, ub.y);
         }
-        cc[2 * pi] = opt_tree3<MX, T, D>(a0);
-        cc[2 * pi + 1] = opt_tree3<MX, T, D>(a1);
+        // from the +/-inf start like the reference: an output whose candidates are all NaN stays +/-inf
+        cc[2 * pi] = opt2<MX>(init, opt_tree3<MX, T, D>(a0));
+        cc[2 * pi + 1] = opt2<MX>(init, opt_tree3<MX, T, D>(a1));
       }
       if constexpr (C::SINGLE) {
         const int ra = h == 0 ? f2vw_row<D>(0, HD - 1) : f2vw_row<D>(1, HD - 1);
@@ -756,7 +757,7 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
           part[x] = opt2<MX>(part[x], ua.x);
           part[x + 1] = opt2<MX>(part[x + 1], ua.y);
         }
-        cc[HD - 1] = opt_tree3<MX, T, D>(a0);
+        cc[HD - 1] = opt2<MX>(init, opt_tree3<MX, T, D>(a0));
       }
     }
     // complete position 1: I keep x1 in [h*HD, (h+1)*HD), the partner lane sends its partial optima for it

@@ -12,9 +12,22 @@ import numpy as np
 import pytest
 
 import oracle as orc
+from _hard_constraints import factor_family
 from conftest import GOLDEN_DIR, golden_names
 
 pytestmark = pytest.mark.gpu
+
+# factor / variable kernel selections the environment offers; the hard-constraint fixtures (msx_*, +/-inf
+# costs, inf and NaN messages) run under every one of them
+KERNEL_CONFIGS = {
+    "default": {},
+    "pipe": {"PYDCOP_B200_F2V": "pipe", "PYDCOP_B200_V2F": "pipe"},
+    "no_tiled_rt": {"PYDCOP_B200_TILED_RT": "0"},
+    "no_fast": {"PYDCOP_B200_NO_FAST": "1"},
+    "generic_first": {"PYDCOP_B200_FAST_FIRST": "0"},
+}
+CASES = [pytest.param(n, "default", id=n) for n in golden_names("ms_")] + \
+        [pytest.param(n, c, id=f"{n}-{c}") for n in golden_names("msx_") for c in KERNEL_CONFIGS]
 
 
 def _engine_state(eng):
@@ -25,9 +38,13 @@ def _engine_state(eng):
 
 
 @pytest.mark.parametrize("precision", ["f64", "f32"])
-@pytest.mark.parametrize("name", golden_names("ms_"))
-def test_maxsum_engine_bit_exact_vs_oracle(name, precision):
+@pytest.mark.parametrize("name,config", CASES)
+def test_maxsum_engine_bit_exact_vs_oracle(name, config, precision, monkeypatch):
+    """Messages (NaN where the oracle has NaN), send flags, gate counters, values and reported costs at
+    every cycle; f64 also against the reference's own trajectory."""
     from pydcop_b200 import MaxSumEngine, layout_from_instance
+    for k, v in KERNEL_CONFIGS[config].items():
+        monkeypatch.setenv(k, v)
     inst, meta = orc.load_golden(os.path.join(GOLDEN_DIR, name + ".npz"))
     npdt = np.float64 if precision == "f64" else np.float32
     o = orc.MaxSumOracle(inst, npdt, mode=meta["mode"], **meta["params"]).init()
@@ -38,17 +55,36 @@ def test_maxsum_engine_bit_exact_vs_oracle(name, precision):
             o.step()
             eng.step()
         q, r, fl, val, cost = _engine_state(eng)
-        assert np.array_equal(q, o.q.astype(np.float64)), (name, k, "q")
-        assert np.array_equal(r, o.r.astype(np.float64)), (name, k, "r")
-        assert np.array_equal(fl["q_sent"], o.q_sent), (name, k, "q_sent")
-        assert np.array_equal(fl["r_sent"], o.r_sent), (name, k, "r_sent")
-        assert np.array_equal(val, o.value), (name, k, "value")
-        assert np.array_equal(cost, o.value_cost.astype(np.float64)), (name, k, "value_cost")
+        where = (name, config, k)
+        assert np.array_equal(q, o.q.astype(np.float64), equal_nan=True), (where, "q")
+        assert np.array_equal(r, o.r.astype(np.float64), equal_nan=True), (where, "r")
+        assert np.array_equal(fl["q_sent"], o.q_sent), (where, "q_sent")
+        assert np.array_equal(fl["r_sent"], o.r_sent), (where, "r_sent")
+        assert np.array_equal(fl["r_cnt"] >> 1, o.r_flags >> 2), (where, "r count")
+        assert np.array_equal(fl["q_cnt"] >> 1, o.q_flags >> 2), (where, "q count")
+        assert np.array_equal(val, o.value), (where, "value")
+        assert np.array_equal(cost, o.value_cost.astype(np.float64), equal_nan=True), (where, "value_cost")
         if precision == "f64":  # directly against the reference's trajectory
-            assert np.array_equal(q, inst["q_state"][k]), (name, k, "q vs reference")
-            assert np.array_equal(r, inst["r_state"][k]), (name, k, "r vs reference")
-            assert np.array_equal(fl["q_sent"].astype(bool), inst["q_sent"][k]), (name, k)
-            assert np.array_equal(fl["r_sent"].astype(bool), inst["r_sent"][k]), (name, k)
+            assert np.array_equal(q, inst["q_state"][k], equal_nan=True), (where, "q vs reference")
+            assert np.array_equal(r, inst["r_state"][k], equal_nan=True), (where, "r vs reference")
+            assert np.array_equal(fl["q_sent"].astype(bool), inst["q_sent"][k]), (where, "q_sent vs reference")
+            assert np.array_equal(fl["r_sent"].astype(bool), inst["r_sent"][k]), (where, "r_sent vs reference")
+
+
+@pytest.mark.parametrize("precision", ["f64", "f32"])
+def test_hard_constraint_fixtures_reach_every_factor_kernel(precision):
+    """In the default configuration the msx_* fixtures put factor classes on the warp, the pipelined and
+    the runtime-shape kernels, each class on the family tests/_hard_constraints.py expects (the CPU test
+    of the fixtures' all-NaN sites relies on that mapping)."""
+    from pydcop_b200 import MaxSumEngine, layout_from_instance
+    seen = set()
+    for name in golden_names("msx_"):
+        inst, meta = orc.load_golden(os.path.join(GOLDEN_DIR, name + ".npz"))
+        L = layout_from_instance(inst)
+        plan = MaxSumEngine(L, precision=precision, mode=meta["mode"]).kernel_plan()
+        assert plan == [factor_family(tuple(c.dom[:c.arity])) for c in L.classes], (name, plan)
+        seen.update(plan)
+    assert {"warp", "pipe", "tiled_rt"} <= seen, seen
 
 
 @pytest.mark.parametrize("precision", ["f64", "f32"])

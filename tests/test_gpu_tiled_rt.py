@@ -23,12 +23,35 @@ def test_mixed_domains_and_arities_bit_exact_vs_oracle(precision):
     assert "generic" not in fam
 
 
-@pytest.mark.parametrize("arity,d", [(2, 7), (2, 12), (2, 31), (3, 6), (3, 11), (4, 4), (5, 3), (6, 2)])
+UNIFORM_RT = [(2, 7), (2, 12), (2, 31), (3, 6), (3, 11), (4, 4), (5, 3), (6, 2)]
+
+
+@pytest.mark.parametrize("arity,d", UNIFORM_RT)
 def test_uniform_shapes_outside_the_compiled_set(arity, d):
     n_f = 400
     inst = random_factor_graph(max(120, n_f * arity // 4), d, n_f, arity, seed=40 + arity * d, int_tables=False)
     eng = _run_pair(inst, "f32", 6)
     assert set(eng.kernel_plan()) == {"tiled_rt"}
+
+
+@pytest.mark.parametrize("precision", ["f32", "f64"])
+@pytest.mark.parametrize("mode", ["min", "max"])
+def test_mixed_domains_with_hard_constraints(mode, precision):
+    """+/-inf cells and variables with every value forbidden, on the mixed-shape classes"""
+    inst = mixed_shape_graph(seed=3, **MIXED)
+    eng = _run_pair(inst, precision, 12, hard_sites={"tiled_rt"}, mode=mode)
+    assert "tiled_rt" in eng.kernel_plan() and "generic" not in eng.kernel_plan()
+
+
+@pytest.mark.parametrize("precision", ["f32", "f64"])
+@pytest.mark.parametrize("arity,d", UNIFORM_RT + [(7, 2), (8, 2)])
+def test_uniform_shapes_outside_the_compiled_set_with_hard_constraints(arity, d, precision):
+    n_f = 400
+    inst = random_factor_graph(max(120, n_f * arity // 4), d, n_f, arity, seed=40 + arity * d, int_tables=False)
+    mode = "max" if (arity + d) % 2 else "min"
+    eng = _run_pair(inst, precision, 12, hard_sites={"tiled_rt"}, mode=mode)
+    fam = eng.kernel_plan()
+    assert [f for c, f in zip(eng.layout.classes, fam) if c.arity >= 2] == ["tiled_rt"], fam
 
 
 @pytest.mark.parametrize("params", [

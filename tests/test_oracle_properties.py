@@ -10,7 +10,7 @@ from hypothesis import given, settings, strategies as st
 
 import oracle as orc
 import ref_shim
-from conftest import GOLDEN_DIR, ROOT
+from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200.generators import random_factor_graph
 from pydcop_b200.layout import default_var_csr
 
@@ -140,7 +140,9 @@ def test_infinite_cost_fixtures_regenerate_bit_for_bit(tmp_path):
         "import sys, os; sys.path.insert(0, %r); sys.argv = ['make_golden_extra.py']\n"
         "import make_golden_extra as m; m.G.GOLDEN = %r; m.main()\n") % (os.path.join(ROOT, "oracle"), str(tmp_path))
     subprocess.run([sys.executable, "-W", "ignore", "-c", code], check=True, capture_output=True, timeout=300)
-    for name in ("msx_hard_inf_min", "msx_hard_inf_max"):
+    written = sorted(f[:-4] for f in os.listdir(str(tmp_path)) if f.endswith(".npz"))
+    assert written == golden_names("msx_"), written
+    for name in written:
         new = np.load(os.path.join(str(tmp_path), name + ".npz"))
         old = np.load(os.path.join(GOLDEN_DIR, name + ".npz"))
         for k in ("r_state", "q_state", "r_sent", "q_sent", "value", "tables"):
