@@ -406,6 +406,76 @@ int fg_mgm_step(fg_mgm_t h, int32_t n_cycles, void *stream);
 int fg_mgm_current(fg_mgm_t h, int64_t *cycle, int32_t *finished);
 int64_t fg_mgm_launch_count(fg_mgm_t h);
 
+/* ------------------------------------------------------------------------------------------
+ * MGM-2  (pydcop/algorithms/mgm2.py: coordinated moves of neighbour pairs, for ALL variables at
+ * once).  Same constraint-hypergraph arrays as MGM; variable costs are never counted (mgm2.py uses
+ * assignment_cost without them).  One cycle = five launches, in the order of the data they need:
+ *   1. value phase (:742-785): current cost, best unilateral move, offerer coin and partner pick,
+ *      the offerer's table of improving joint moves (own value x partner value, all its constraints)
+ *   2. answers (:787-856): every non-offerer scores the offers it got over its constraints that do
+ *      not contain the offerer and commits to the best one (favor rule) or to none
+ *   3. commit (:858-890): an accepted offerer takes the receiver's value and global gain
+ *   4. gain phase (:892-972): GO flags of committed variables, unilateral moves of the others
+ *   5. go (:974-1001): a committed pair moves when both sent GO.
+ * Draws: Philox4x32-10, counter (canonical variable id, cycle, purpose, 0) — cycle 0xffffffff for
+ * the start values (purpose 0), else the 1-based round; purposes 1 offerer coin + partner pick,
+ * 2 unilateral value pick, 3 favor "no" coin, 4 offer pick (philox_draw, csrc/philox.cuh).
+ * ------------------------------------------------------------------------------------------ */
+enum { FG_MGM2_FAVOR_UNILATERAL = 0, FG_MGM2_FAVOR_NO = 1, FG_MGM2_FAVOR_COORDINATED = 2 };
+
+typedef struct {
+  int32_t abi_version, precision;
+  int32_t n_vars, n_factors, n_edges, n_classes;
+  const fg_class_t *classes;      /* HOST [n_classes] */
+  const void *dev_tables;         /* T[...] */
+  const int32_t *dev_dom_size;    /* [n_vars] */
+  const int32_t *dev_var_id;      /* [n_vars] canonical id = Philox counter */
+  const int32_t *dev_var_rank;    /* [n_vars] position of the variable's NAME in sorted order */
+  const int32_t *dev_edge_var;    /* [n_edges] */
+  const int32_t *dev_edge_class;  /* [n_edges] */
+  const int32_t *dev_var_ptr;     /* [n_vars+1] */
+  const int32_t *dev_slot_edge;   /* [n_edges] incident edges of v in node.constraints order */
+  const int32_t *dev_nbr_ptr;     /* [n_vars+1] distinct neighbours, first-appearance order */
+  const int32_t *dev_nbr_idx;     /* [nbr_ptr[n_vars]] */
+  const int32_t *dev_init_value;  /* [n_vars] value index or -1 (random), may be NULL */
+  int32_t *dev_value;             /* [n_vars] in/out */
+  void *dev_cost;                 /* T[n_vars] current_cost */
+  uint8_t *dev_has_cost;          /* [n_vars] current_cost is not None */
+  void *dev_gain;                 /* T[n_vars] potential_gain */
+  int32_t *dev_potential_value;   /* [n_vars] */
+  void *dev_local_cost;           /* T[n_vars] cost computed in the value phase */
+  uint8_t *dev_offerer;           /* [n_vars] the variable made an offer this cycle */
+  int32_t *dev_partner;           /* [n_vars] offerer: its partner; committed receiver: its offerer; else -1 */
+  uint8_t *dev_committed;         /* [n_vars] */
+  uint8_t *dev_go;                /* [n_vars] a committed variable sent GO */
+  uint8_t *dev_answer;            /* [n_vars] by offerer: accepted by its partner */
+  int32_t *dev_answer_value;      /* [n_vars] by offerer: its value in the accepted joint move */
+  void *dev_answer_gain;          /* T[n_vars] by offerer: the receiver's global gain */
+  const int64_t *dev_offer_off;   /* [n_vars] start of v's offer table in dev_offer */
+  void *dev_offer;                /* T[...] v's table: dom(v) x max dom of its neighbours entries, row
+                                     stride dom(partner); an entry not offered holds 0 (an offered gain
+                                     is > 0 in min mode, < 0 in max mode) */
+  int32_t mode_max;
+  int32_t favor;                  /* FG_MGM2_FAVOR_* */
+  double threshold;               /* offerer when u < threshold */
+  int32_t stop_cycle;             /* 0 = never; a run ends when round + 1 >= stop_cycle (mgm2.py:613) */
+  int32_t reserved0;
+  uint64_t seed;
+} fg_mgm2_desc_t;
+
+typedef struct fg_mgm2 *fg_mgm2_t;
+
+int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out);
+int fg_mgm2_destroy(fg_mgm2_t h);
+const char *fg_mgm2_last_error(fg_mgm2_t h);
+/* on_start: start values of the variables with neighbours (initial_value or a draw); a variable
+ * without neighbours takes a drawn value among its best over its (unary) constraints and is done. */
+int fg_mgm2_init(fg_mgm2_t h, void *stream);
+/* up to n_cycles cycles (stops as the reference does at stop_cycle). */
+int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream);
+int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished);
+int64_t fg_mgm2_launch_count(fg_mgm2_t h);
+
 /* Solution cost (next-tier row §8f.1; pydcop/dcop/dcop.py:319-367 `solution_cost`, called by the
  * orchestrator at the end of a run and at every metric tick, orchestrator.py:1229-1231): over the factors
  * of every non-ghost class the table entry at the assignment, over the first n_vars variables

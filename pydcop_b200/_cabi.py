@@ -84,6 +84,23 @@ class FgMgmDesc(C.Structure):
                 ("dev_row_cache", P), ("dev_slot_last", P)]
 
 
+class FgMgm2Desc(C.Structure):
+    _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
+                ("n_vars", C.c_int32), ("n_factors", C.c_int32), ("n_edges", C.c_int32),
+                ("n_classes", C.c_int32), ("classes", C.POINTER(FgClass)),
+                ("dev_tables", P), ("dev_dom_size", P), ("dev_var_id", P), ("dev_var_rank", P),
+                ("dev_edge_var", P), ("dev_edge_class", P), ("dev_var_ptr", P), ("dev_slot_edge", P),
+                ("dev_nbr_ptr", P), ("dev_nbr_idx", P), ("dev_init_value", P),
+                ("dev_value", P), ("dev_cost", P), ("dev_has_cost", P), ("dev_gain", P),
+                ("dev_potential_value", P), ("dev_local_cost", P), ("dev_offerer", P), ("dev_partner", P),
+                ("dev_committed", P), ("dev_go", P), ("dev_answer", P), ("dev_answer_value", P),
+                ("dev_answer_gain", P), ("dev_offer_off", P), ("dev_offer", P),
+                ("mode_max", C.c_int32), ("favor", C.c_int32), ("threshold", C.c_double),
+                ("stop_cycle", C.c_int32), ("reserved0", C.c_int32), ("seed", C.c_uint64)]
+
+
+MGM2_FAVORS = {"unilateral": 0, "no": 1, "coordinated": 2}
+
 FG_MAX_PEERS = 16
 
 
@@ -152,6 +169,13 @@ SYMBOLS = {
     "fg_mgm_step": (C.c_int, [P, C.c_int32, P]),
     "fg_mgm_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "fg_mgm_launch_count": (C.c_int64, [P]),
+    "fg_mgm2_create": (C.c_int, [C.POINTER(FgMgm2Desc), C.POINTER(P)]),
+    "fg_mgm2_destroy": (C.c_int, [P]),
+    "fg_mgm2_last_error": (C.c_char_p, [P]),
+    "fg_mgm2_init": (C.c_int, [P, P]),
+    "fg_mgm2_step": (C.c_int, [P, C.c_int32, P]),
+    "fg_mgm2_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "fg_mgm2_launch_count": (C.c_int64, [P]),
     "fg_solution_cost": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
                                    C.c_int32, P, P, C.c_double, P, P]),
 }

@@ -1,0 +1,184 @@
+// MGM-2 for all variables at once: C-ABI entry points fg_mgm2_* and their kernels
+// (csrc/mgm2_kernels.cuh).  Its own translation unit, so the MaxSum / DSA / MGM code in engine.cu
+// and mgm.cu is compiled exactly as before.
+//
+// Floating-point operand order follows pydcop/algorithms/mgm2.py so that the f64 build equals the
+// reference's Python floats and the f32 build the f32 oracle (tests/_mgm2_oracle.py):
+//   cost of an assignment = ((0 + c1) + c2) + ...    in node.constraints order (assignment_cost)
+//   offer gain            = current_cost - cost                                   (:553)
+//   global gain           = (current_cost - cost over the other constraints) + offer gain (:593)
+//   cost after a move     = current_cost - potential_gain                         (:941, :986)
+#include <cstdio>
+#include <new>
+#include <vector>
+
+#include "common.cuh"
+#include "mgm2_kernels.cuh"
+
+struct fg_mgm2 {
+  fg_mgm2_desc_t d;
+  std::vector<fg_class_t> classes;
+  fg_class_t *dev_classes = nullptr;
+  int64_t cycle = 0;
+  int64_t launches = 0;
+  char err[512] = {0};
+};
+
+static char g_mgm2_static_err[64] = "invalid handle";
+
+static inline unsigned mgm2_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
+
+static MgmSide mgm2_side(const fg_mgm2 *h) {
+  const fg_mgm2_desc_t &d = h->d;
+  return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr};
+}
+
+extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
+  if (!desc || !out) return FG_ERR_ARG;
+  *out = nullptr;
+  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
+  if (desc->precision != FG_F32 && desc->precision != FG_F64) return FG_ERR_ARG;
+  fg_mgm2 *h = new (std::nothrow) fg_mgm2();
+  if (!h) return FG_ERR_ARG;
+  h->d = *desc;
+  h->classes.assign(desc->classes, desc->classes + desc->n_classes);
+  h->d.classes = h->classes.data();
+  *out = h;
+  for (auto &c : h->classes) {
+    if (c.arity < 1 || c.arity > FG_MAX_ARITY) {
+      snprintf(h->err, sizeof(h->err), "class arity %d out of range", c.arity);
+      return FG_ERR_ARG;
+    }
+    int64_t ts = 1;
+    for (int i = 0; i < c.arity; ++i) {
+      if (c.dom[i] < 1 || c.dom[i] > FG_MAX_DOM) {
+        snprintf(h->err, sizeof(h->err), "domain size %d out of range", c.dom[i]);
+        return FG_ERR_ARG;
+      }
+      ts *= c.dom[i];
+    }
+    if (ts != c.table_size) {
+      snprintf(h->err, sizeof(h->err), "class size mismatch");
+      return FG_ERR_ARG;
+    }
+  }
+  if (desc->favor < FG_MGM2_FAVOR_UNILATERAL || desc->favor > FG_MGM2_FAVOR_COORDINATED) {
+    snprintf(h->err, sizeof(h->err), "favor %d is not one of unilateral (0), no (1), coordinated (2)", desc->favor);
+    return FG_ERR_ARG;
+  }
+  if (!(desc->threshold >= 0.0 && desc->threshold <= 1.0)) {
+    snprintf(h->err, sizeof(h->err), "threshold %g is not in [0, 1]", desc->threshold);
+    return FG_ERR_ARG;
+  }
+  if (desc->stop_cycle < 0) {
+    snprintf(h->err, sizeof(h->err), "negative stop_cycle %d", desc->stop_cycle);
+    return FG_ERR_ARG;
+  }
+  if (desc->n_vars > 0 &&
+      (!desc->dev_tables || !desc->dev_dom_size || !desc->dev_var_id || !desc->dev_var_rank || !desc->dev_var_ptr ||
+       !desc->dev_nbr_ptr || !desc->dev_nbr_idx || !desc->dev_value || !desc->dev_cost || !desc->dev_has_cost ||
+       !desc->dev_gain || !desc->dev_potential_value || !desc->dev_local_cost || !desc->dev_offerer ||
+       !desc->dev_partner || !desc->dev_committed || !desc->dev_go || !desc->dev_answer || !desc->dev_answer_value ||
+       !desc->dev_answer_gain || !desc->dev_offer_off || !desc->dev_offer)) {
+    snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
+    return FG_ERR_ARG;
+  }
+  if (desc->n_edges > 0 && (!desc->dev_edge_var || !desc->dev_edge_class || !desc->dev_slot_edge)) {
+    snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
+    return FG_ERR_ARG;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
+    cudaGetLastError();
+    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
+    return FG_ERR_CUDA;
+  }
+  size_t bytes = sizeof(fg_class_t) * (h->classes.empty() ? 1 : h->classes.size());
+  CUDA_TRY(h, cudaMalloc(&h->dev_classes, bytes));
+  if (!h->classes.empty())
+    CUDA_TRY(h, cudaMemcpy(h->dev_classes, h->classes.data(), sizeof(fg_class_t) * h->classes.size(), cudaMemcpyHostToDevice));
+  return FG_OK;
+}
+
+extern "C" int fg_mgm2_destroy(fg_mgm2_t h) {
+  if (h && h->dev_classes) cudaFree(h->dev_classes);
+  delete h;
+  return FG_OK;
+}
+
+extern "C" const char *fg_mgm2_last_error(fg_mgm2_t h) { return h ? h->err : g_mgm2_static_err; }
+
+template <typename T>
+static void mgm2_init_t(fg_mgm2 *h, cudaStream_t st) {
+  const fg_mgm2_desc_t &d = h->d;
+  k_mgm2_init<T><<<mgm2_blocks(d.n_vars, 128), 128, 0, st>>>(mgm2_side(h), d.n_vars, (const T *)d.dev_tables,
+                                                             d.dev_init_value, d.mode_max, d.seed, d.dev_value,
+                                                             (T *)d.dev_cost, d.dev_has_cost);
+}
+
+extern "C" int fg_mgm2_init(fg_mgm2_t h, void *stream) {
+  if (!h) return FG_ERR_ARG;
+  const fg_mgm2_desc_t &d = h->d;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d.n_vars) {
+    if (d.precision == FG_F64) mgm2_init_t<double>(h, st);
+    else mgm2_init_t<float>(h, st);
+    ++h->launches;
+  }
+  CUDA_TRY(h, cudaGetLastError());
+  h->cycle = 0;
+  return FG_OK;
+}
+
+static bool mgm2_finished(const fg_mgm2 *h) { return h->d.stop_cycle && h->cycle + 1 >= h->d.stop_cycle; }
+
+template <typename T>
+static int mgm2_cycle_t(fg_mgm2 *h, cudaStream_t st) {
+  const fg_mgm2_desc_t &d = h->d;
+  if (d.n_vars) {
+    const MgmSide g = mgm2_side(h);
+    const uint32_t cyc = (uint32_t)(h->cycle + 1);
+    const int n = d.n_vars;
+    T *cost = (T *)d.dev_cost, *local = (T *)d.dev_local_cost, *gain = (T *)d.dev_gain;
+    k_mgm2_value<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
+        g, n, (const T *)d.dev_tables, d.dev_value, cost, d.dev_has_cost, local, gain, d.dev_potential_value,
+        d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_offer_off, (T *)d.dev_offer, d.mode_max,
+        d.threshold, d.seed, cyc);
+    k_mgm2_answer<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
+        g, n, (const T *)d.dev_tables, d.dev_value, local, gain, d.dev_potential_value, d.dev_offerer, d.dev_partner,
+        d.dev_committed, d.dev_answer, d.dev_answer_value, (T *)d.dev_answer_gain, d.dev_offer_off,
+        (const T *)d.dev_offer, d.mode_max, d.favor, d.seed, cyc);
+    k_mgm2_commit<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, d.dev_offerer, d.dev_answer, d.dev_answer_value,
+                                                          (const T *)d.dev_answer_gain, gain, d.dev_potential_value,
+                                                          d.dev_committed);
+    k_mgm2_gain<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(g, n, gain, d.dev_potential_value, d.dev_committed,
+                                                        d.dev_partner, d.dev_go, d.dev_value, cost);
+    k_mgm2_go<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, d.dev_committed, d.dev_partner, d.dev_go, gain,
+                                                      d.dev_potential_value, d.dev_value, cost);
+    h->launches += 5;
+  }
+  CUDA_TRY(h, cudaGetLastError());
+  ++h->cycle;
+  return FG_OK;
+}
+
+extern "C" int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream) {
+  if (!h) return FG_ERR_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  for (int i = 0; i < n_cycles; ++i) {
+    if (mgm2_finished(h)) break;
+    int rc = h->d.precision == FG_F64 ? mgm2_cycle_t<double>(h, st) : mgm2_cycle_t<float>(h, st);
+    if (rc != FG_OK) return rc;
+  }
+  return FG_OK;
+}
+
+extern "C" int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished) {
+  if (!h) return FG_ERR_ARG;
+  if (cycle) *cycle = h->cycle;
+  if (finished) *finished = mgm2_finished(h) ? 1 : 0;
+  return FG_OK;
+}
+
+extern "C" int64_t fg_mgm2_launch_count(fg_mgm2_t h) { return h ? h->launches : -1; }

@@ -25,3 +25,10 @@ __host__ __device__ __forceinline__ double philox_u53(const uint32_t b[4]) {
 __host__ __device__ __forceinline__ int philox_choice(const uint32_t b[4], int n) {
   return (int)(((uint64_t)b[2] * (uint64_t)n) >> 32);
 }
+
+// block of counter (var, cycle, purpose, 0): one stream per kind of decision (MGM-2); purpose 0 is
+// the block every existing draw uses
+__host__ __device__ __forceinline__ void philox_draw(uint32_t var, uint32_t cycle, uint32_t purpose, uint64_t seed,
+                                                     uint32_t out[4]) {
+  philox4x32_10(var, cycle, purpose, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), out);
+}

@@ -703,3 +703,169 @@ class MgmEngine(_EngineBase):
         n = L.n_vars
         return (L.vars_to_canonical(self.gain[:n].double().cpu().numpy()),
                 L.vars_to_canonical(self.new_value[:n].cpu().numpy()))
+
+
+def mgm2_offer_offsets(layout: FactorGraphLayout, nbr_ptr, nbr_idx):
+    """Start of every variable's MGM-2 offer table (internal order) and the total size: an offerer
+    writes dom(v) x dom(partner) gains, so v gets dom(v) x max dom of its neighbours entries (none
+    without neighbours)."""
+    L = layout
+    dom = L.dom_size.astype(np.int64)
+    deg = np.diff(nbr_ptr).astype(np.int64)
+    widest = np.zeros(L.n_vars, dtype=np.int64)
+    if len(nbr_idx) and int(nbr_ptr[-1]):
+        owner = np.repeat(np.arange(L.n_vars), deg)
+        np.maximum.at(widest, owner, dom[nbr_idx[:int(nbr_ptr[-1])]])
+    size = dom * widest
+    off = np.zeros(L.n_vars + 1, dtype=np.int64)
+    np.cumsum(size, out=off[1:])
+    return off[:-1].copy(), int(off[-1])
+
+
+class Mgm2Engine(_EngineBase):
+    """All-variables-at-once MGM-2 (pydcop/algorithms/mgm2.py; parameters :139-143).
+
+    threshold  a variable offers a coordinated move when its draw u < threshold
+    favor      unilateral | no | coordinated: what a receiver does when its best offer's global gain
+               EQUALS its best unilateral gain (mgm2.py:818-822)
+    var_rank   canonical order: position of each variable's NAME in sorted order, the lexicographic
+               tie break of mgm2.py:944-949 (default: the canonical index)
+    Variable costs are not part of MGM-2's costs (assignment_cost without them); a variable without
+    neighbours takes a drawn value among its best over its unary constraints on the device.
+    """
+
+    def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
+                 threshold=0.5, favor="unilateral", stop_cycle=0, seed=0, var_rank=None):
+        self.lib = _cabi.load()
+        self.device = _require_cuda(device)
+        self.layout = L = layout
+        self.precision = precision
+        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        if mode not in ("min", "max"):
+            raise ValueError(f"invalid mode {mode!r}")
+        if favor not in _cabi.MGM2_FAVORS:
+            raise ValueError(f"invalid favor {favor!r}: expected one of {sorted(_cabi.MGM2_FAVORS)}")
+        h = mgm_host_arrays(L, mode, var_rank)
+        self.nbr_ptr_host, self.nbr_idx_host = h["nbr_ptr"], h["nbr_idx"]
+        self.has_nbr_host = h["has_nbr"]
+        offer_off, offer_size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
+        self.offer_bytes = offer_size * np.dtype(self.np_dtype).itemsize
+        n = max(L.n_vars, 1)
+        with torch.cuda.device(self.device):
+            self.tables = self._dev(L.tables, tdt)
+            self.dom_size = self._dev(L.dom_size, torch.int32)
+            self.var_id = self._dev(L.var_order, torch.int32)
+            self.var_rank = self._dev(h["var_rank"], torch.int32)
+            self.edge_var = self._dev(L.edge_var, torch.int32)
+            self.edge_class = self._dev(L.edge_class, torch.int32)
+            self.var_ptr = self._dev(L.var_ptr, torch.int32)
+            self.slot_edge = self._dev(L.slot_edge, torch.int32)
+            self.nbr_ptr = self._dev(h["nbr_ptr"], torch.int32)
+            self.nbr_idx = self._dev(h["nbr_idx"], torch.int32)
+            self.init_value = self._dev(L.init_value, torch.int32)
+            self.offer_off = self._dev(np.resize(offer_off, n) if L.n_vars else np.zeros(1, np.int64), torch.int64)
+            z = lambda dt: torch.zeros(n, dtype=dt, device=self.device)  # noqa: E731
+            self.value, self.potential_value, self.answer_value = z(torch.int32), z(torch.int32), z(torch.int32)
+            self.partner = torch.full((n,), -1, dtype=torch.int32, device=self.device)
+            self.cost, self.gain, self.local_cost, self.answer_gain = z(tdt), z(tdt), z(tdt), z(tdt)
+            self.has_cost, self.offerer, self.committed = z(torch.uint8), z(torch.uint8), z(torch.uint8)
+            self.go, self.answer = z(torch.uint8), z(torch.uint8)
+            self.offer = torch.zeros(max(offer_size, 1), dtype=tdt, device=self.device)
+        self._classes = _class_array(L)
+        d = _cabi.FgMgm2Desc()
+        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
+        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
+        d.classes = C.cast(self._classes, C.POINTER(FgClass))
+        d.dev_tables, d.dev_dom_size = _ptr(self.tables), _ptr(self.dom_size)
+        d.dev_var_id, d.dev_var_rank = _ptr(self.var_id), _ptr(self.var_rank)
+        d.dev_edge_var, d.dev_edge_class = _ptr(self.edge_var), _ptr(self.edge_class)
+        d.dev_var_ptr, d.dev_slot_edge = _ptr(self.var_ptr), _ptr(self.slot_edge)
+        d.dev_nbr_ptr, d.dev_nbr_idx = _ptr(self.nbr_ptr), _ptr(self.nbr_idx)
+        d.dev_init_value = _ptr(self.init_value)
+        d.dev_value, d.dev_cost, d.dev_has_cost = _ptr(self.value), _ptr(self.cost), _ptr(self.has_cost)
+        d.dev_gain, d.dev_potential_value = _ptr(self.gain), _ptr(self.potential_value)
+        d.dev_local_cost, d.dev_offerer, d.dev_partner = _ptr(self.local_cost), _ptr(self.offerer), _ptr(self.partner)
+        d.dev_committed, d.dev_go = _ptr(self.committed), _ptr(self.go)
+        d.dev_answer, d.dev_answer_value = _ptr(self.answer), _ptr(self.answer_value)
+        d.dev_answer_gain = _ptr(self.answer_gain)
+        d.dev_offer_off, d.dev_offer = _ptr(self.offer_off), _ptr(self.offer)
+        d.mode_max, d.favor, d.threshold = int(mode == "max"), _cabi.MGM2_FAVORS[favor], float(threshold)
+        d.stop_cycle, d.seed = int(stop_cycle or 0), int(seed) & (2 ** 64 - 1)
+        self._desc = d
+        self._h = C.c_void_p()
+        self._check(self.lib.fg_mgm2_create(C.byref(d), C.byref(self._h)), "fg_mgm2_create")
+
+    def _last_error(self):
+        return (self.lib.fg_mgm2_last_error(self._h) or b"").decode()
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self.lib.fg_mgm2_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def init(self):
+        with torch.cuda.device(self.device):
+            self._check(self.lib.fg_mgm2_init(self._h, self._stream()), "fg_mgm2_init")
+        return self
+
+    def step(self, n_cycles=1):
+        with torch.cuda.device(self.device):
+            self._check(self.lib.fg_mgm2_step(self._h, int(n_cycles), self._stream()), "fg_mgm2_step")
+        return self
+
+    def _current(self):
+        c, f = C.c_int64(), C.c_int32()
+        self.lib.fg_mgm2_current(self._h, C.byref(c), C.byref(f))
+        return c.value, bool(f.value)
+
+    @property
+    def cycle(self):
+        return self._current()[0]
+
+    @property
+    def finished(self):
+        return self._current()[1]
+
+    @property
+    def launch_count(self):
+        return int(self.lib.fg_mgm2_launch_count(self._h))
+
+    def values(self):
+        """(value index, current cost or NaN while the reference's is None) per variable,
+        canonical variable order."""
+        L = self.layout
+        n = L.n_vars
+        cost = self.cost[:n].double().cpu().numpy()
+        cost[self.has_cost[:n].cpu().numpy() == 0] = np.nan
+        return L.vars_to_canonical(self.value[:n].cpu().numpy()), L.vars_to_canonical(cost)
+
+    def record(self):
+        """State of the last cycle per variable, canonical order: local_cost and gain (NaN without
+        neighbours), offerer, partner (position in the variable's neighbour list, or -1), committed,
+        potential_value (-1 without neighbours), go."""
+        L = self.layout
+        n = L.n_vars
+        conn = self.has_nbr_host[:n]
+        host = lambda t: t[:n].cpu().numpy()  # noqa: E731
+        partner = host(self.partner)
+        pos = np.full(n, -1, dtype=np.int32)
+        for v in np.nonzero(partner >= 0)[0]:
+            row = self.nbr_idx_host[self.nbr_ptr_host[v]:self.nbr_ptr_host[v + 1]]
+            pos[v] = int(np.nonzero(row == partner[v])[0][0])
+        out = dict(local_cost=np.where(conn, host(self.local_cost).astype(np.float64), np.nan),
+                   gain=np.where(conn, host(self.gain).astype(np.float64), np.nan),
+                   offerer=host(self.offerer), partner=pos, committed=host(self.committed),
+                   potential_value=np.where(conn, host(self.potential_value), -1).astype(np.int32),
+                   go=host(self.go))
+        return {k: L.vars_to_canonical(v) for k, v in out.items()}
+
+    def solution_cost(self, infinity=float("inf"), unary=None):
+        """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
+        out = self._solution_cost(self.value, infinity, unary).cpu().numpy()
+        return float(out[0]), int(out[1])

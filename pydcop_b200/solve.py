@@ -1,5 +1,5 @@
 """Direct solve: a DCOP file (or arrays, or a pyDcop DCOP object) -> GPU engine -> result dict
-(algorithms: maxsum, dsa, adsa, mgm).
+(algorithms: maxsum, dsa, adsa, mgm, mgm2).
 
 The plugin modules (pydcop_b200/algorithms/) keep pyDcop's orchestrator, agents and one Python
 computation object per graph node around the engine — that is the drop-in path, and it is what
@@ -10,7 +10,7 @@ pydcop/commands/solve.py:611-624): status, assignment, cost, violation, time, cy
 msg_size.
 
 Parameters and defaults are the reference algorithms' own (maxsum.py:212-220, dsa.py:130-135,
-mgm.py:78-81).
+mgm.py:78-81, mgm2.py:139-143).
 MaxSum has no termination test of its own (maxsum.py: it runs until `stop_cycle` or the
 orchestrator's timeout), so one of `stop_cycle` / `timeout` is required here as well; status is
 FINISHED when `stop_cycle` was reached and TIMEOUT otherwise, as in the reference
@@ -34,13 +34,15 @@ MAXSUM_DEFAULTS = {"damping": 0.5, "damping_nodes": "both", "stability": 0.1, "n
 DSA_DEFAULTS = {"probability": 0.7, "p_mode": "fixed", "variant": "B", "stop_cycle": 0}
 ADSA_DEFAULTS = {"period": 0.5, "probability": 0.7, "variant": "B", "stop_cycle": 0}   # adsa.py:121-125 + stop_cycle
 MGM_DEFAULTS = {"break_mode": "lexic", "stop_cycle": 0}
-DEFAULTS = {"maxsum": MAXSUM_DEFAULTS, "dsa": DSA_DEFAULTS, "mgm": MGM_DEFAULTS, "adsa": ADSA_DEFAULTS}
+MGM2_DEFAULTS = {"threshold": 0.5, "favor": "unilateral", "stop_cycle": 0}
+DEFAULTS = {"maxsum": MAXSUM_DEFAULTS, "dsa": DSA_DEFAULTS, "mgm": MGM_DEFAULTS, "adsa": ADSA_DEFAULTS,
+            "mgm2": MGM2_DEFAULTS}
 _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "start_messages": ("leafs", "leafs_vars", "all"),
             "p_mode": ("fixed", "arity"), "variant": ("A", "B", "C"),
-            "break_mode": ("lexic", "random")}
+            "break_mode": ("lexic", "random"), "favor": ("unilateral", "no", "coordinated")}
 ALGOS = {"maxsum": "maxsum", "maxsum_gpu": "maxsum", "dsa": "dsa", "dsa_gpu": "dsa",
-         "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa"}
+         "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa", "mgm2": "mgm2", "mgm2_gpu": "mgm2"}
 
 
 def check_params(kind: str, params: Optional[Dict[str, Any]]) -> Dict[str, Any]:
@@ -134,7 +136,11 @@ def name_rank(dcop: ingest.DcopArrays) -> np.ndarray:
 
 
 def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
-    from .engine import DsaEngine, MaxSumEngine, MgmEngine
+    from .engine import DsaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+    if kind == "mgm2":
+        return Mgm2Engine(layout, device=device, precision=precision, mode=mode,
+                          threshold=params["threshold"], favor=params["favor"],
+                          stop_cycle=params["stop_cycle"], seed=seed or 0, var_rank=name_rank(dcop))
     if kind == "mgm":
         return MgmEngine(layout, device=device, precision=precision, mode=mode,
                          stop_cycle=params["stop_cycle"], seed=seed or 0,
@@ -160,8 +166,8 @@ def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, par
     from .multigpu import ShardedMaxSum, broadcast_owner
     from .multigpu_dsa import ShardedDsa
     rank, world = dist.get_rank(), dist.get_world_size()
-    if kind == "mgm":
-        raise ValueError("mgm is not sharded: run it on one GPU")
+    if kind in ("mgm", "mgm2"):
+        raise ValueError(f"{kind} is not sharded: run it on one GPU")
     kw = dict(sharded_kwargs or {})
     dev = device if device is not None else (torch.device("cuda", torch.cuda.current_device())
                                              if torch.cuda.is_available() and "engine_factory" not in kw
@@ -200,7 +206,7 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     noise).
 
     problem      see `load`
-    algo         maxsum | dsa | mgm (the *_gpu spellings of the plugin modules are accepted)
+    algo         maxsum | dsa | adsa | mgm | mgm2 (the *_gpu spellings of the plugin modules are accepted)
     algo_params  the reference's parameter names; `stop_cycle` bounds the run in cycles
     timeout      wall-clock bound in seconds (checked every `chunk` cycles)
     precision    f32 | f64 (f64 reproduces the reference's double arithmetic bit for bit)
