@@ -166,6 +166,12 @@ int64_t fg_maxsum_launch_count(fg_maxsum_t h);
 enum { FG_KERNEL_GENERIC = 0, FG_KERNEL_PIPE = 1, FG_KERNEL_WARP = 2, FG_KERNEL_TILED_RT = 3 };
 int fg_maxsum_kernel_plan(fg_maxsum_t h, int32_t *family, int32_t n_classes);
 
+/* Bytes per stored table entry that the factor side reads for each class (diagnostic): 1 where the warp kernel reads
+ * an 8-bit copy made at creation — every entry of the class an integer in [-128, 127], none -0.0, NaN or inf, so the
+ * messages are the same bit for bit — else the value width (4 or 8).  The copy is taken once by fg_maxsum_create:
+ * writes to dev_tables after creation are not seen by those classes. */
+int fg_maxsum_table_width(fg_maxsum_t h, int32_t *bytes, int32_t n_classes);
+
 /* Gather / scatter of boundary message rows for the halo exchange (replaces
  * Messaging.post_msg for cut edges, pydcop/infrastructure/communication.py:588-698).
  * rows: `n_rows` (offset,len) pairs in dev_row_off/dev_row_len; packed back to back. */

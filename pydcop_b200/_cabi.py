@@ -133,6 +133,7 @@ SYMBOLS = {
     "fg_maxsum_current": (C.c_int, [P, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "fg_maxsum_launch_count": (C.c_int64, [P]),
     "fg_maxsum_kernel_plan": (C.c_int, [P, P, C.c_int32]),
+    "fg_maxsum_table_width": (C.c_int, [P, P, C.c_int32]),
     "fg_maxsum_shard_fused": (C.c_int, [P]),
     "fg_halo_pack": (C.c_int, [C.c_int32, P, P, P, P, P, C.c_int64, P]),
     "fg_halo_unpack": (C.c_int, [C.c_int32, P, P, P, P, P, C.c_int64, P]),

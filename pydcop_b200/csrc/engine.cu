@@ -131,6 +131,10 @@ extern "C" int fg_maxsum_create(const fg_maxsum_desc_t *desc, fg_maxsum_t *out) 
     return FG_ERR_CUDA;
   }
   maxsum_warp_plan_f2v(h->d, h->classes, h->fast, h->warp);
+  if (maxsum_warp_plan_tab8(h->d, h->classes, h->warp) != FG_OK) {
+    snprintf(h->err, sizeof(h->err), "8-bit table copy of the factor side: %s", cudaGetErrorString(cudaGetLastError()));
+    return FG_ERR_CUDA;
+  }
   {
     std::vector<uint8_t> skip(h->classes.size(), 0);
     for (size_t i = 0; i < h->classes.size(); ++i) skip[i] = h->fast.f2v[i] || h->warp.f2v[i];
@@ -158,6 +162,7 @@ extern "C" int fg_maxsum_destroy(fg_maxsum_t h) {
     if (h->push_stream) cudaStreamDestroy(h->push_stream);
     if (h->side_stream) cudaStreamDestroy(h->side_stream);
     if (h->warp.dev_classes) cudaFree(h->warp.dev_classes);
+    if (h->warp.tab8) cudaFree(h->warp.tab8);
     tiled_rt_free(h->tiled_rt);
   }
   delete h;
@@ -231,7 +236,13 @@ static int maxsum_compute_t(fg_maxsum *h, cudaStream_t st, bool push_split = fal
   for (size_t ci = 0; ci < h->classes.size(); ++ci) {
     const fg_class_t &c = h->classes[ci];
     if (c.n_factors == 0 || (c.flags & FG_CLASS_GHOST)) continue;
-    if (!first && h->warp.f2v[ci] && dispatch_f2v_warp<T>(false, c, d, q_cur, r_cur, r_next, p, st)) { ++h->launches; continue; }
+    if (!first && h->warp.f2v[ci]) {
+      if (launch_f2v_warp_class<T>(h->warp, ci, c, d, q_cur, r_cur, r_next, p, st)) { ++h->launches; continue; }
+      if (fused) {   // no other kernel stores boundary rows to the peers: never drop them silently
+        snprintf(h->err, sizeof(h->err), "fused halo: no peer-store factor kernel for class %zu", ci);
+        return FG_ERR_ARG;
+      }
+    }
     if (!first && maxsum_fast_f2v<T>(h->fast, (int)ci, c, d, q_cur, r_cur, r_next, p, st, h->launches)) continue;
     if (!first && h->tiled_rt.on[ci]) continue;   // below, one launch per arity
     const int64_t n = (int64_t)c.n_factors * c.arity;
@@ -381,6 +392,14 @@ extern "C" int fg_maxsum_kernel_plan(fg_maxsum_t h, int32_t *family, int32_t n_c
     family[i] = (c.flags & FG_CLASS_GHOST) ? -1 : h->warp.f2v[i] ? FG_KERNEL_WARP : h->fast.f2v[i] ? FG_KERNEL_PIPE
               : h->tiled_rt.on[i] ? FG_KERNEL_TILED_RT : FG_KERNEL_GENERIC;
   }
+  return FG_OK;
+}
+
+extern "C" int fg_maxsum_table_width(fg_maxsum_t h, int32_t *bytes, int32_t n_classes) {
+  if (!h || !bytes || n_classes != (int32_t)h->classes.size()) return FG_ERR_ARG;
+  const int32_t full = (int32_t)prec_size(h->d.precision);
+  for (int32_t i = 0; i < n_classes; ++i)
+    bytes[i] = (!h->warp.tab8_base.empty() && h->warp.tab8_base[i] >= 0) ? 1 : full;
   return FG_OK;
 }
 

@@ -32,6 +32,7 @@
 #pragma once
 #include "maxsum_fast.cuh"
 #include "packed.cuh"
+#include "table_i8.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // variable -> factor
@@ -425,6 +426,11 @@ struct MaxSumWarpPlan {
   bool v2f_on = false;               // PYDCOP_B200_V2F != pipe
   std::vector<WTileRange> v2f;       // launches of the variable side
   WClassEntry *dev_classes = nullptr;   // library-owned: class table of every launch (48 bytes per class)
+  // factor side: 8-bit copy of the integer tables (maxsum_warp_plan_tab8), library-owned; per class its byte offset
+  // in it, -1 = the kernel reads dev_tables at full width
+  int8_t *tab8 = nullptr;
+  int64_t tab8_bytes = 0;
+  std::vector<int64_t> tab8_base;
 };
 
 template <typename T, int D, int NS_, bool MX>
@@ -548,21 +554,31 @@ inline int maxsum_warp_plan(const fg_maxsum_desc_t &d, const std::vector<fg_varc
 //      async copies on a per-warp mbarrier), the 32 q rows are gathered through edge_qoff with
 //      cp.async (lanes <-> (row, piece)), the produced r rows are written in place over the staged
 //      previous rows and leave with one bulk store.  NS stages: tile k computes while k+1 .. k+NS-1 load.
+//      TT = the table storage type: T, or int8_t for the classes whose every entry passes fg_table_entry_fits_i8
+//      (table_i8.cuh; a copy the engine makes at creation, MaxSumWarpPlan::tab8): the same body, only the table
+//      loads decode bytes to T exactly (tab_decode), so every message keeps its bits.
 // ------------------------------------------------------------------------------------------------
-template <typename T, int D, int NS_>
+template <typename T, typename TT, int D, int NS_>
 struct F2VWarpCfg {
   static constexpr int S = D * D, HD = D / 2, NF = 16;
   static constexpr int NPAIR = (HD % 2 == 0) ? HD / 2 : (HD - 1) / 2;   // row pairs per lane
   static constexpr bool SINGLE = (HD % 2) != 0;                          // plus one single row
+  static constexpr bool NARROW = sizeof(TT) < sizeof(T);                 // 8-bit table codes
   static constexpr int VR = V2FCfg<T, D>::VR;          // elements per row vector (row = D elements)
   static constexpr int VR_BYTES = V2FCfg<T, D>::VR_BYTES;
   static constexpr int PIECES = D / VR;
   static constexpr int V2_BYTES = fg_gcd(16, 2 * D * (int)sizeof(T));   // a pair of rows / a factor's 2 message rows
   static constexpr int V2 = V2_BYTES / (int)sizeof(T);
-  static constexpr int STAGE = NF * S + 2 * NF * 2 * D;              // tab | rt (previous r rows) | qt   (elements)
+  // table loads, in bytes: a row pair starts at fl*S + ra*D entries (ra even), the single row at fl*S + (D-2+h)*D.
+  // Full width: as the message rows.  8-bit: the alignment those offsets guarantee (D = 10: 4-byte pairs — the
+  // factor stride of 25 words is odd, so a half-warp's 16 factors hit 16 banks — and 2-byte single rows)
+  static constexpr int TV2_BYTES = NARROW ? fg_gcd(fg_gcd(16, 2 * D), S) : V2_BYTES;
+  static constexpr int TV1_BYTES = NARROW ? fg_gcd(16, D) : VR_BYTES;
+  static constexpr int TAB_BYTES = NF * S * (int)sizeof(TT);           // a multiple of 16: rt stays 16-byte aligned
+  static constexpr int STAGE_BYTES = TAB_BYTES + 2 * NF * 2 * D * (int)sizeof(T);   // tab | rt (previous r rows) | qt
   static constexpr int OUT = NF * 2 * D;                             // produced r rows, double-buffered per warp
   static constexpr int NS = NS_;
-  static constexpr size_t WARP_SMEM = (size_t)(NS * STAGE + 2 * OUT) * sizeof(T);
+  static constexpr size_t WARP_SMEM = (size_t)NS * STAGE_BYTES + (size_t)2 * OUT * sizeof(T);
   static constexpr size_t smem_for(int w) { return (size_t)w * WARP_SMEM + (size_t)w * NS * sizeof(uint64_t) + 16; }
   // warps per CTA: the CTA is only a container of independent warps
   static constexpr int WARPS = smem_for(2) <= FG_SMEM_LIMIT ? 2 : (smem_for(1) <= FG_SMEM_LIMIT ? 1 : 0);
@@ -570,26 +586,81 @@ struct F2VWarpCfg {
   static constexpr bool OK = (D % 2 == 0) && D >= 4 && WARPS > 0;
 };
 
+// Byte k of w (a signed 8-bit table code, already XOR-ed with 0x80, i.e. biased by +128) as T, exactly: the biased
+// byte becomes the low mantissa bits of 2^23 (2^52), and one correctly rounded subtract of 2^23 + 128 leaves the
+// integer in [-128, 127] (every intermediate is an integer below 2^24).  A PRMT and an add per entry.
+template <typename T> __device__ __forceinline__ T tab_decode(uint32_t wb, int k);
+template <> __device__ __forceinline__ float tab_decode<float>(uint32_t wb, int k) {
+  return __fsub_rn(__uint_as_float(__byte_perm(wb, 0x4B000000u, 0x7440u | (uint32_t)k)), 8388736.0f);
+}
+template <> __device__ __forceinline__ double tab_decode<double>(uint32_t wb, int k) {
+  return __dsub_rn(__hiloint2double(0x43300000, (int)__byte_perm(wb, 0u, 0x4440u | (uint32_t)k)), 4503599627370624.0);
+}
+
+// N consecutive table entries at p, VB-byte aligned, as T: full-width tables load as message rows do, 8-bit codes
+// load as 16-bit (VB = 2) or 32/64/128-bit words and are decoded
+template <typename T, int N, int VB>
+__device__ __forceinline__ void ld_tab(const T *__restrict__ p, T (&out)[N]) {
+  ld_row<T, N, VB / (int)sizeof(T)>(p, out);
+}
+template <typename T, int N, int VB>
+__device__ __forceinline__ void ld_tab(const int8_t *__restrict__ p, T (&out)[N]) {
+  static_assert(N % VB == 0 && (VB == 2 || VB == 4 || VB == 8 || VB == 16), "table load width");
+  if constexpr (VB == 2) {
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      const uint32_t wb = (uint32_t)*reinterpret_cast<const uint16_t *>(p + 2 * i) ^ 0x8080u;
+      out[2 * i] = tab_decode<T>(wb, 0);
+      out[2 * i + 1] = tab_decode<T>(wb, 1);
+    }
+  } else {
+    constexpr int W = VB / 4;   // 32-bit words per load
+#pragma unroll
+    for (int i = 0; i < N / VB; ++i) {
+      uint32_t w[W];
+      if constexpr (W == 1) {
+        w[0] = *reinterpret_cast<const uint32_t *>(p + VB * i);
+      } else if constexpr (W == 2) {
+        const uint2 v = *reinterpret_cast<const uint2 *>(p + VB * i);
+        w[0] = v.x; w[1] = v.y;
+      } else {
+        const uint4 v = *reinterpret_cast<const uint4 *>(p + VB * i);
+        w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
+      }
+#pragma unroll
+      for (int j = 0; j < W; ++j) {
+        const uint32_t wb = w[j] ^ 0x80808080u;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) out[VB * i + 4 * j + k] = tab_decode<T>(wb, k);
+      }
+    }
+  }
+}
+
 // table row index of the i-th row lane h owns (i < D/2); see the kernel comment
 template <int D>
 __host__ __device__ constexpr int f2vw_row(int h, int i) {
   return ((D / 2) % 2 == 0) ? h * (D / 2) + i : (i < D / 2 - 1 ? h * (D / 2 - 1) + i : 2 * (D / 2 - 1) + h);
 }
 
-template <typename T, int D, int NS_, bool MX, typename OffT, bool PEER = false>
-__global__ void __launch_bounds__(F2VWarpCfg<T, D, NS_>::WARPS > 0 ? F2VWarpCfg<T, D, NS_>::WARPS * 32 : 32)
-k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict__ q_cur,
+template <typename T, typename TT, int D, int NS_, bool MX, typename OffT, bool PEER = false>
+__global__ void __launch_bounds__(F2VWarpCfg<T, TT, D, NS_>::WARPS > 0 ? F2VWarpCfg<T, TT, D, NS_>::WARPS * 32 : 32)
+k_f2v_warp(const fg_class_t c, const TT *__restrict__ tables, const T *__restrict__ q_cur,
            const T *__restrict__ r_cur, T *__restrict__ r_next, const OffT *__restrict__ edge_qoff,
            uint8_t *__restrict__ r_cnt, uint8_t *__restrict__ r_sent, MaxSumParams p) {
-  using C = F2VWarpCfg<T, D, NS_>;
+  using C = F2VWarpCfg<T, TT, D, NS_>;
   // PEER (opt-in fused halo): per edge the peer address of its r row this cycle, 0 = interior
   const int64_t *__restrict__ edge_dst = PEER ? p.edge_dst : nullptr;
   using P = typename Pair<T>::type;
-  constexpr int S = C::S, HD = C::HD, NF = C::NF, NS = C::NS, VR = C::VR, PIECES = C::PIECES, R = 2 * D;
+  constexpr int S = C::S, HD = C::HD, NF = C::NF, NS = C::NS, PIECES = C::PIECES, R = 2 * D;
+  constexpr int VR = C::VR;
   constexpr int WARPS = C::WARPS > 0 ? C::WARPS : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  T *stage0 = reinterpret_cast<T *>(smem_raw + (size_t)wib * C::WARP_SMEM);
+  unsigned char *stage0 = smem_raw + (size_t)wib * C::WARP_SMEM;
+  // stage s: table (TT) | previous r rows (T) | gathered q rows (T)
+  auto stage_tab = [&](int s) { return reinterpret_cast<TT *>(stage0 + (size_t)s * C::STAGE_BYTES); };
+  auto stage_rt = [&](int s) { return reinterpret_cast<T *>(stage0 + (size_t)s * C::STAGE_BYTES + C::TAB_BYTES); };
   uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)WARPS * C::WARP_SMEM) + NS * wib;
   if (lane == 0) {
 #pragma unroll
@@ -631,19 +702,23 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
       const int s = k % NS;
       const int f0 = (gw + k * nw) * NF;
       const int nf = min(NF, c.n_factors - f0);
-      T *tab = stage0 + s * C::STAGE;
-      T *rt = tab + NF * S;
+      TT *tab = stage_tab(s);
+      T *rt = stage_rt(s);
       T *qt = rt + NF * R;
-      const T *gtab = tables + c.table_base + (int64_t)f0 * S;
+      const TT *gtab = tables + c.table_base + (int64_t)f0 * S;
       const T *grow = r_cur + c.msg_base + (int64_t)f0 * R;
-      const uint32_t tb = (uint32_t)(nf * S) * (uint32_t)sizeof(T), rb = (uint32_t)(nf * R) * (uint32_t)sizeof(T);
+      // 8-bit codes: every class is padded to whole tiles (maxsum_warp_plan_tab8), so the tail tile loads all NF
+      // tables too and its size stays a multiple of 16 (there is no 1-byte cp.async to fall back on)
+      const uint32_t tb = (uint32_t)((C::NARROW ? NF : nf) * S) * (uint32_t)sizeof(TT);
+      const uint32_t rb = (uint32_t)(nf * R) * (uint32_t)sizeof(T);
       const bool tma_t = (tb % 16 == 0), tma_r = (rb % 16 == 0);   // bases are 128-byte aligned, tiles 16 factors
       if (lane == 0) {
         mbar_expect_tx(&bars[s], (tma_t ? tb : 0u) + (tma_r ? rb : 0u));
         if (tma_t) tma_load_1d(tab, gtab, tb, &bars[s]);
         if (tma_r) tma_load_1d(rt, grow, rb, &bars[s]);
       }
-      if (!tma_t) for (int i = lane; i < nf * S; i += 32) cp_async_b<(int)sizeof(T)>(tab + i, gtab + i);
+      if constexpr (!C::NARROW)
+        if (!tma_t) for (int i = lane; i < nf * S; i += 32) cp_async_b<(int)sizeof(T)>(tab + i, gtab + i);
       if (!tma_r) for (int i = lane; i < nf * R; i += 32) cp_async_b<(int)sizeof(T)>(rt + i, grow + i);
 #pragma unroll
       for (int it = 0; it < PIECES; ++it) {
@@ -662,7 +737,7 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
   // odd number of 16-byte units for D = 6, 10) spreads a quarter-warp's 128-bit reads over all 32 banks; the first
   // mapping (half in the low lane bit) had 43 % conflict wavefronts.  The partner of a lane is lane ^ 16.
   const int fl = lane & 15, h = lane >> 4;
-  T *out0 = stage0 + NS * C::STAGE;
+  T *out0 = reinterpret_cast<T *>(stage0 + (size_t)NS * C::STAGE_BYTES);
 
   // prologue: tiles 0 .. NS-2 in flight, gather offsets of tile NS-1 and counters of tile 0 on their way
 #pragma unroll 1
@@ -690,8 +765,8 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
 
     const int f0 = (gw + k * nw) * NF;
     const int nf = min(NF, c.n_factors - f0);
-    T *tab = stage0 + s * C::STAGE;
-    T *rt = tab + NF * S;
+    const TT *tab = stage_tab(s);
+    T *rt = stage_rt(s);
     const T *qt = rt + NF * R;
     const bool act = fl < nf;
     // counters were loaded lane = edge index (2 f + j): fetch both edges of my factor
@@ -706,7 +781,7 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
 #pragma unroll
     for (int i = 0; i < 2 * HD; ++i) { cc[i] = init; pp[i] = (T)0; }
     if (act) {
-      const T *tf = tab + fl * S;
+      const TT *tf = tab + fl * S;
       T q0[D], q1[D];
       {
         T qq[2 * D];
@@ -721,7 +796,7 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
         (void)dummy;
         const int ra = h == 0 ? f2vw_row<D>(0, 2 * pi) : f2vw_row<D>(1, 2 * pi);   // rows ra, ra + 1
         T rows[2 * D];
-        ld_row<T, 2 * D, C::V2>(tf + ra * D, rows);
+        ld_tab<T, 2 * D, C::TV2_BYTES>(tf + ra * D, rows);
         // q0[ra], q0[ra + 1] with static register indices: h selects between two compile-time candidates
         const T qa = h == 0 ? q0[f2vw_row<D>(0, 2 * pi)] : q0[f2vw_row<D>(1, 2 * pi)];
         const T qb = h == 0 ? q0[f2vw_row<D>(0, 2 * pi) + 1] : q0[f2vw_row<D>(1, 2 * pi) + 1];
@@ -745,7 +820,7 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
       if constexpr (C::SINGLE) {
         const int ra = h == 0 ? f2vw_row<D>(0, HD - 1) : f2vw_row<D>(1, HD - 1);
         T row[D], a0[D];
-        ld_row<T, D, VR>(tf + ra * D, row);
+        ld_tab<T, D, C::TV1_BYTES>(tf + ra * D, row);
         const T qa = h == 0 ? q0[f2vw_row<D>(0, HD - 1)] : q0[f2vw_row<D>(1, HD - 1)];
         const P qa2 = pmake<T>(qa, qa);
 #pragma unroll
@@ -828,15 +903,23 @@ k_f2v_warp(const fg_class_t c, const T *__restrict__ tables, const T *__restrict
   if (lane == 0) tma_store_wait_read();
 }
 
-template <typename T, int D, int NS_, bool MX>
-inline bool launch_f2v_warp_ns(bool probe, const fg_class_t &c, const fg_maxsum_desc_t &d, const T *q_cur, const T *r_cur,
-                               T *r_next, const MaxSumParams &p, cudaStream_t st) {
-  using C = F2VWarpCfg<T, D, NS_>;
+// Launch shape of the 8-bit table instantiations (PYDCOP_B200_F2VW_CPS / _NS override both widths): a stage is half
+// the size of a full-width one, so more CTAs and stages keep the same bytes in flight (sweep on C2: DESIGN.md §5)
+#define FG_F2VW8_CPS 4
+#define FG_F2VW8_NS 3
+// the fused halo's peer-store kernel (PEER = true) is compiled at the default depth of each table width only
+#define FG_F2VW_PEER_NS(T, TT) (sizeof(TT) < sizeof(T) ? FG_F2VW8_NS : 2)
+
+// tables: dev_tables (TT = T) or the 8-bit copy (TT = int8_t; c.table_base is then the class's byte offset in it)
+template <typename T, typename TT, int D, int NS_, bool MX>
+inline bool launch_f2v_warp_ns(bool probe, const fg_class_t &c, const TT *tables, const fg_maxsum_desc_t &d, const T *q_cur,
+                               const T *r_cur, T *r_next, const MaxSumParams &p, cudaStream_t st) {
+  using C = F2VWarpCfg<T, TT, D, NS_>;
   if constexpr (!C::OK) {
     return false;
   } else {
     if (probe) return true;
-    auto kern = k_f2v_warp<T, D, NS_, MX, uint32_t>;
+    auto kern = k_f2v_warp<T, TT, D, NS_, MX, uint32_t>;
     static int per_sm = 0, n_sm = 0;  // one per instantiation
     if (!per_sm) {
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
@@ -845,36 +928,47 @@ inline bool launch_f2v_warp_ns(bool probe, const fg_class_t &c, const fg_maxsum_
       cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, C::WARPS * 32, C::SMEM);
       if (per_sm < 1) per_sm = 1;
-      const int cap = fg_env_int("PYDCOP_B200_F2VW_CPS", 3);  // CTAs of 2 warps; the variable side shares the SMs
+      // CTAs of 2 warps; the variable side shares the SMs
+      const int cap = fg_env_int("PYDCOP_B200_F2VW_CPS", C::NARROW ? FG_F2VW8_CPS : 3);
       if (per_sm > cap) per_sm = cap;
     }
     const int n_tiles = (c.n_factors + C::NF - 1) / C::NF;
     const int need = (n_tiles + C::WARPS - 1) / C::WARPS;
     const unsigned blocks = (unsigned)std::min(need, n_sm * per_sm);
-    if constexpr (NS_ == 2) {   // fused halo: same kernel with the peer stores compiled in (default depth only)
-      if (p.edge_dst != nullptr) {
-        auto kp = k_f2v_warp<T, D, NS_, MX, uint32_t, true>;
+    if (p.edge_dst != nullptr) {   // fused halo: only the PEER instantiation stores the boundary rows
+      if constexpr (NS_ == FG_F2VW_PEER_NS(T, TT)) {
+        auto kp = k_f2v_warp<T, TT, D, NS_, MX, uint32_t, true>;
         static bool attr = false;
         if (!attr) { cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM); attr = true; }
-        kp<<<blocks, C::WARPS * 32, C::SMEM, st>>>(c, (const T *)d.dev_tables, q_cur, r_cur, r_next, d.dev_edge_qoff32,
+        kp<<<blocks, C::WARPS * 32, C::SMEM, st>>>(c, tables, q_cur, r_cur, r_next, d.dev_edge_qoff32,
                                                   d.dev_r_cnt, d.dev_r_sent, p);
         return true;
+      } else {
+        return false;   // not compiled at this depth (launch_f2v_warp never asks): the caller reports an error
       }
     }
-    kern<<<blocks, C::WARPS * 32, C::SMEM, st>>>(c, (const T *)d.dev_tables, q_cur, r_cur, r_next, d.dev_edge_qoff32,
+    kern<<<blocks, C::WARPS * 32, C::SMEM, st>>>(c, tables, q_cur, r_cur, r_next, d.dev_edge_qoff32,
                                                 d.dev_r_cnt, d.dev_r_sent, p);
     return true;
   }
 }
 
-// pipeline depth: PYDCOP_B200_F2VW_NS = 2 | 3 | 4 stages per warp (default 2), shallower when it does not fit
-template <typename T, int D>
-inline bool launch_f2v_warp(bool probe, const fg_class_t &c, const fg_maxsum_desc_t &d, const T *q_cur, const T *r_cur,
-                            T *r_next, const MaxSumParams &p, cudaStream_t st) {
-  static const int ns = fg_env_int("PYDCOP_B200_F2VW_NS", 2);
-#define FG_TRY(NS_)                                                                                      \
-  if (p.mode_max ? launch_f2v_warp_ns<T, D, NS_, true>(probe, c, d, q_cur, r_cur, r_next, p, st)        \
-                 : launch_f2v_warp_ns<T, D, NS_, false>(probe, c, d, q_cur, r_cur, r_next, p, st))      \
+// pipeline depth: PYDCOP_B200_F2VW_NS = 2 | 3 | 4 stages per warp (default 2, FG_F2VW8_NS for 8-bit tables),
+// shallower when it does not fit.  A fused-halo launch (p.edge_dst set) always runs at the depth its peer-store kernel
+// is compiled at.
+template <typename T, typename TT, int D>
+inline bool launch_f2v_warp(bool probe, const fg_class_t &c, const TT *tables, const fg_maxsum_desc_t &d, const T *q_cur,
+                            const T *r_cur, T *r_next, const MaxSumParams &p, cudaStream_t st) {
+  constexpr int NSP = FG_F2VW_PEER_NS(T, TT);
+  static_assert(!F2VWarpCfg<T, TT, D, 2>::OK || F2VWarpCfg<T, TT, D, NSP>::OK,
+                "every shape of the warp kernel has its peer-store instantiation");
+  if (!probe && p.edge_dst != nullptr)
+    return p.mode_max ? launch_f2v_warp_ns<T, TT, D, NSP, true>(false, c, tables, d, q_cur, r_cur, r_next, p, st)
+                      : launch_f2v_warp_ns<T, TT, D, NSP, false>(false, c, tables, d, q_cur, r_cur, r_next, p, st);
+  static const int ns = fg_env_int("PYDCOP_B200_F2VW_NS", sizeof(TT) < sizeof(T) ? FG_F2VW8_NS : 2);
+#define FG_TRY(NS_)                                                                                              \
+  if (p.mode_max ? launch_f2v_warp_ns<T, TT, D, NS_, true>(probe, c, tables, d, q_cur, r_cur, r_next, p, st)    \
+                 : launch_f2v_warp_ns<T, TT, D, NS_, false>(probe, c, tables, d, q_cur, r_cur, r_next, p, st))  \
     return true;
   if (ns >= 4) { FG_TRY(4) }
   if (ns >= 3) { FG_TRY(3) }
@@ -883,17 +977,99 @@ inline bool launch_f2v_warp(bool probe, const fg_class_t &c, const fg_maxsum_des
   return false;
 }
 
-// binary classes over one even domain size; probe == true: only report whether the kernel exists
+// binary classes over one even domain size; probe == true: only report whether the kernel exists.
+// tab8 != nullptr: the class's tables are read from the 8-bit copy at byte offset tab8_base
 template <typename T>
-inline bool dispatch_f2v_warp(bool probe, const fg_class_t &c, const fg_maxsum_desc_t &d, const T *q_cur, const T *r_cur,
-                              T *r_next, const MaxSumParams &p, cudaStream_t st) {
+inline bool dispatch_f2v_warp(bool probe, const fg_class_t &c, const fg_maxsum_desc_t &d, const int8_t *tab8, int64_t tab8_base,
+                              const T *q_cur, const T *r_cur, T *r_next, const MaxSumParams &p, cudaStream_t st) {
   if (c.arity != 2 || c.dom[0] != c.dom[1]) return false;
+  fg_class_t c8 = c;
+  c8.table_base = tab8_base;
   switch (c.dom[0]) {
-#define X(n) case n: return launch_f2v_warp<T, n>(probe, c, d, q_cur, r_cur, r_next, p, st);
+#define X(n)                                                                                               \
+  case n:                                                                                                  \
+    return tab8 ? launch_f2v_warp<T, int8_t, n>(probe, c8, tab8, d, q_cur, r_cur, r_next, p, st)           \
+                : launch_f2v_warp<T, T, n>(probe, c, (const T *)d.dev_tables, d, q_cur, r_cur, r_next, p, st);
     X(4) X(6) X(8) X(10) X(16) X(20)
 #undef X
   }
   return false;
+}
+
+// the factor side of class ci on the warp kernel, from the 8-bit copy when the class has one
+template <typename T>
+inline bool launch_f2v_warp_class(const MaxSumWarpPlan &plan, size_t ci, const fg_class_t &c, const fg_maxsum_desc_t &d,
+                                  const T *q_cur, const T *r_cur, T *r_next, const MaxSumParams &p, cudaStream_t st) {
+  const bool narrow = plan.tab8 != nullptr && plan.tab8_base[ci] >= 0;
+  return dispatch_f2v_warp<T>(false, c, d, narrow ? plan.tab8 : nullptr, narrow ? plan.tab8_base[ci] : 0, q_cur, r_cur,
+                              r_next, p, st);
+}
+
+// Every entry of a class's tables fits int8 (fg_table_entry_fits_i8): *ok stays 1, else it is cleared
+template <typename T>
+__global__ void k_tab8_check(const T *__restrict__ t, int64_t n, int32_t *__restrict__ ok) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    if (!fg_table_entry_fits_i8<T>(t[i])) { *ok = 0; return; }
+}
+
+template <typename T>
+__global__ void k_tab8_encode(const T *__restrict__ t, int64_t n, int8_t *__restrict__ out) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = (int8_t)(int)t[i];
+}
+
+// 8-bit copy of the tables of every warp-kernel class whose entries all fit (engine creation; the device must be
+// there).  Each class starts on a 128-byte boundary and is padded with zeros to whole 16-factor tiles.  dev_tables
+// is left as it is for every other reader.  Synchronises the device: the tables may have been uploaded on any stream.
+template <typename T>
+inline int maxsum_warp_plan_tab8_t(const fg_maxsum_desc_t &d, const std::vector<fg_class_t> &classes, MaxSumWarpPlan &plan) {
+  const size_t n = classes.size();
+  plan.tab8_base.assign(n, -1);
+  std::vector<size_t> cand;
+  for (size_t i = 0; i < n; ++i)
+    if (plan.f2v[i] && classes[i].n_factors > 0) cand.push_back(i);
+  if (cand.empty()) return FG_OK;
+  if (cudaDeviceSynchronize() != cudaSuccess) return FG_ERR_CUDA;
+  int32_t *dev_ok = nullptr;
+  if (cudaMalloc(reinterpret_cast<void **>(&dev_ok), cand.size() * sizeof(int32_t)) != cudaSuccess) return FG_ERR_CUDA;
+  std::vector<int32_t> ok(cand.size(), 1);
+  int rc = FG_OK;
+  const T *tables = (const T *)d.dev_tables;
+  auto grid = [](int64_t m) { return (unsigned)std::min<int64_t>((m + 255) / 256, 4096); };
+  if (cudaMemcpy(dev_ok, ok.data(), ok.size() * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) rc = FG_ERR_CUDA;
+  for (size_t k = 0; rc == FG_OK && k < cand.size(); ++k) {
+    const fg_class_t &c = classes[cand[k]];
+    const int64_t m = (int64_t)c.n_factors * c.table_size;
+    k_tab8_check<T><<<grid(m), 256>>>(tables + c.table_base, m, dev_ok + k);
+  }
+  if (rc == FG_OK && cudaMemcpy(ok.data(), dev_ok, ok.size() * sizeof(int32_t), cudaMemcpyDeviceToHost) != cudaSuccess)
+    rc = FG_ERR_CUDA;
+  cudaFree(dev_ok);
+  if (rc != FG_OK) return rc;
+  int64_t total = 0;
+  for (size_t k = 0; k < cand.size(); ++k) {
+    if (!ok[k]) continue;
+    const fg_class_t &c = classes[cand[k]];
+    plan.tab8_base[cand[k]] = total;
+    total += ((int64_t)(c.n_factors + 15) / 16 * 16 * c.table_size + 127) / 128 * 128;
+  }
+  if (total == 0) return FG_OK;
+  if (cudaMalloc(reinterpret_cast<void **>(&plan.tab8), (size_t)total) != cudaSuccess) return FG_ERR_CUDA;
+  plan.tab8_bytes = total;
+  if (cudaMemset(plan.tab8, 0, (size_t)total) != cudaSuccess) return FG_ERR_CUDA;
+  for (size_t k = 0; k < cand.size(); ++k) {
+    if (!ok[k]) continue;
+    const fg_class_t &c = classes[cand[k]];
+    const int64_t m = (int64_t)c.n_factors * c.table_size;
+    k_tab8_encode<T><<<grid(m), 256>>>(tables + c.table_base, m, plan.tab8 + plan.tab8_base[cand[k]]);
+  }
+  if (cudaDeviceSynchronize() != cudaSuccess) return FG_ERR_CUDA;
+  return FG_OK;
+}
+
+inline int maxsum_warp_plan_tab8(const fg_maxsum_desc_t &d, const std::vector<fg_class_t> &classes, MaxSumWarpPlan &plan) {
+  return d.precision == FG_F64 ? maxsum_warp_plan_tab8_t<double>(d, classes, plan)
+                               : maxsum_warp_plan_tab8_t<float>(d, classes, plan);
 }
 
 // factor classes the warp kernel takes over from the round-1 pipelined kernel
@@ -906,8 +1082,8 @@ inline void maxsum_warp_plan_f2v(const fg_maxsum_desc_t &d, const std::vector<fg
   for (size_t i = 0; i < classes.size(); ++i) {
     if (classes[i].flags & FG_CLASS_GHOST) continue;
     const bool ok = d.precision == FG_F64
-                        ? dispatch_f2v_warp<double>(true, classes[i], d, nullptr, nullptr, nullptr, dummy, nullptr)
-                        : dispatch_f2v_warp<float>(true, classes[i], d, nullptr, nullptr, nullptr, dummy, nullptr);
+                        ? dispatch_f2v_warp<double>(true, classes[i], d, nullptr, 0, nullptr, nullptr, nullptr, dummy, nullptr)
+                        : dispatch_f2v_warp<float>(true, classes[i], d, nullptr, 0, nullptr, nullptr, nullptr, dummy, nullptr);
     if (ok) plan.f2v[i] = 1;
   }
 }

@@ -256,6 +256,16 @@ class MaxSumEngine(_EngineBase):
             raise EngineError(f"fg_maxsum_kernel_plan rc={rc}")
         return [self.KERNEL_FAMILIES[int(out[i])] for i in range(n)]
 
+    def table_widths(self):
+        """Bytes per stored table entry the factor side reads for every factor class (fg_maxsum_table_width):
+        1 where the warp kernel reads the engine's 8-bit copy of integer tables, else 4 (f32) or 8 (f64)."""
+        n = len(self.layout.classes)
+        out = (C.c_int32 * max(n, 1))()
+        rc = self.lib.fg_maxsum_table_width(self._h, out, n)
+        if rc != 0:
+            raise EngineError(f"fg_maxsum_table_width rc={rc}")
+        return [int(out[i]) for i in range(n)]
+
     # -- readback (canonical edge order) -----------------------------------------------------
     def messages(self):
         """(q, r) receiver-side message state as float64 numpy arrays in canonical edge order."""
