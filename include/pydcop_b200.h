@@ -482,6 +482,81 @@ int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream);
 int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished);
 int64_t fg_mgm2_launch_count(fg_mgm2_t h);
 
+/* ------------------------------------------------------------------------------------------
+ * GDBA  (pydcop/algorithms/gdba.py: distributed breakout with constraint modifiers, for ALL
+ * variables at once).  Same constraint-hypergraph arrays as MGM.  One round = two launches:
+ *   1. ok phase (:352-387): effective evaluation of every value (base cost combined with the
+ *      variable's modifier, plus the variable-cost terms), violated constraints at the current
+ *      value, improve and the value an improving variable would take
+ *   2. improve phase (:493-541): an improving variable that wins its neighbourhood moves; a variable
+ *      that cannot improve, when no neighbour's improve exceeds 0, raises its own modifiers on its
+ *      violated constraints.  Values are double-buffered: round k reads dev_value[(k-1) % 2] and
+ *      writes dev_value[k % 2], so a breakout reads the values the round was evaluated on.
+ * Modifier counts (int32, converted to T at use; reset by fg_gdba_init): increase mode T keeps one
+ * count per slot; E / R / C keep a table of the constraint's entries only for a slot whose constraint
+ * spans {variable} + all its neighbours — the only constraints where the reference ever reads what those
+ * modes write (:585-588 vs :634-654).
+ * Draws: Philox4x32-10 keyed as MGM's: counter (canonical variable id, cycle, 0, 0), cycle 0xffffffff
+ * for the start value, else the 1-based round.
+ * ------------------------------------------------------------------------------------------ */
+enum { FG_GDBA_MODIFIER_A = 0, FG_GDBA_MODIFIER_M = 1 };
+enum { FG_GDBA_VIOLATION_NZ = 0, FG_GDBA_VIOLATION_NM = 1, FG_GDBA_VIOLATION_MX = 2 };
+enum { FG_GDBA_INCREASE_E = 0, FG_GDBA_INCREASE_R = 1, FG_GDBA_INCREASE_C = 2, FG_GDBA_INCREASE_T = 3 };
+
+typedef struct {
+  int32_t abi_version, precision;
+  int32_t n_vars, n_factors, n_edges, n_classes;
+  const fg_class_t *classes;      /* HOST [n_classes] */
+  const void *dev_tables;         /* T[...] */
+  const void *dev_unary;          /* T[...] variable costs (cost_for_val) */
+  const int64_t *dev_unary_off;   /* [n_vars+1] */
+  const void *dev_viol_ref;       /* T[n_factors] internal factor order: min (NM) / max (MX) of the base
+                                     table (:252-274); may be NULL with NZ */
+  const int32_t *dev_dom_size;    /* [n_vars] */
+  const int32_t *dev_var_id;      /* [n_vars] canonical id = Philox counter */
+  const int32_t *dev_var_rank;    /* [n_vars] position of the variable's NAME in sorted order */
+  const int32_t *dev_edge_var;    /* [n_edges] */
+  const int32_t *dev_edge_class;  /* [n_edges] */
+  const int32_t *dev_var_ptr;     /* [n_vars+1] */
+  const int32_t *dev_slot_edge;   /* [n_edges] incident edges of v in node.constraints order */
+  const int32_t *dev_nbr_ptr;     /* [n_vars+1] distinct neighbours, first-appearance order */
+  const int32_t *dev_nbr_idx;     /* [nbr_ptr[n_vars]] */
+  const int32_t *dev_init_value;  /* [n_vars] value index or -1 (random), may be NULL */
+  int32_t *dev_value[2];          /* [n_vars] each; dev_value[0] holds the preset values of the variables
+                                     without neighbours (optimal_cost_value), the others are set by init */
+  void *dev_cost;                 /* T[n_vars] current_cost (preset for isolated variables) */
+  uint8_t *dev_has_cost;          /* [n_vars] current_cost is not None */
+  void *dev_improve;              /* T[n_vars] */
+  int32_t *dev_new_value;         /* [n_vars] */
+  uint8_t *dev_violated;          /* [n_edges] per slot: violated at the current value (last round) */
+  uint8_t *dev_breakout;          /* [n_vars] the last round raised a modifier */
+  int32_t *dev_mod;               /* modifier counts: [n_edges] (T) or the spanning tables (E / R / C) */
+  const int64_t *dev_mod_off;     /* [n_edges] E / R / C: start of the slot's table in dev_mod, -1 = none;
+                                     NULL with T */
+  int32_t mode_max;
+  int32_t modifier;               /* FG_GDBA_MODIFIER_* */
+  int32_t violation;              /* FG_GDBA_VIOLATION_* */
+  int32_t increase_mode;          /* FG_GDBA_INCREASE_* */
+  int32_t stop_cycle;             /* 0 = never; a run ends when round + 1 >= stop_cycle (as fg_mgm_desc_t) */
+  int32_t reserved0;
+  int64_t mod_size;               /* elements of dev_mod */
+  uint64_t seed;
+} fg_gdba_desc_t;
+
+typedef struct fg_gdba *fg_gdba_t;
+
+int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out);
+int fg_gdba_destroy(fg_gdba_t h);
+const char *fg_gdba_last_error(fg_gdba_t h);
+/* on_start: start values of the variables with neighbours (initial_value or a draw), every modifier
+ * back to its base. */
+int fg_gdba_init(fg_gdba_t h, void *stream);
+/* up to n_cycles rounds (stops at stop_cycle). */
+int fg_gdba_step(fg_gdba_t h, int32_t n_cycles, void *stream);
+/* rounds run; the current values are in dev_value[cycle % 2]. */
+int fg_gdba_current(fg_gdba_t h, int64_t *cycle, int32_t *finished);
+int64_t fg_gdba_launch_count(fg_gdba_t h);
+
 /* Solution cost (next-tier row §8f.1; pydcop/dcop/dcop.py:319-367 `solution_cost`, called by the
  * orchestrator at the end of a run and at every metric tick, orchestrator.py:1229-1231): over the factors
  * of every non-ghost class the table entry at the assignment, over the first n_vars variables

@@ -101,6 +101,26 @@ class FgMgm2Desc(C.Structure):
 
 MGM2_FAVORS = {"unilateral": 0, "no": 1, "coordinated": 2}
 
+
+class FgGdbaDesc(C.Structure):
+    _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
+                ("n_vars", C.c_int32), ("n_factors", C.c_int32), ("n_edges", C.c_int32),
+                ("n_classes", C.c_int32), ("classes", C.POINTER(FgClass)),
+                ("dev_tables", P), ("dev_unary", P), ("dev_unary_off", P), ("dev_viol_ref", P),
+                ("dev_dom_size", P), ("dev_var_id", P), ("dev_var_rank", P),
+                ("dev_edge_var", P), ("dev_edge_class", P), ("dev_var_ptr", P), ("dev_slot_edge", P),
+                ("dev_nbr_ptr", P), ("dev_nbr_idx", P), ("dev_init_value", P),
+                ("dev_value", P * 2), ("dev_cost", P), ("dev_has_cost", P), ("dev_improve", P),
+                ("dev_new_value", P), ("dev_violated", P), ("dev_breakout", P), ("dev_mod", P), ("dev_mod_off", P),
+                ("mode_max", C.c_int32), ("modifier", C.c_int32), ("violation", C.c_int32),
+                ("increase_mode", C.c_int32), ("stop_cycle", C.c_int32), ("reserved0", C.c_int32),
+                ("mod_size", C.c_int64), ("seed", C.c_uint64)]
+
+
+GDBA_MODIFIERS = {"A": 0, "M": 1}
+GDBA_VIOLATIONS = {"NZ": 0, "NM": 1, "MX": 2}
+GDBA_INCREASE_MODES = {"E": 0, "R": 1, "C": 2, "T": 3}
+
 FG_MAX_PEERS = 16
 
 
@@ -177,6 +197,13 @@ SYMBOLS = {
     "fg_mgm2_step": (C.c_int, [P, C.c_int32, P]),
     "fg_mgm2_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "fg_mgm2_launch_count": (C.c_int64, [P]),
+    "fg_gdba_create": (C.c_int, [C.POINTER(FgGdbaDesc), C.POINTER(P)]),
+    "fg_gdba_destroy": (C.c_int, [P]),
+    "fg_gdba_last_error": (C.c_char_p, [P]),
+    "fg_gdba_init": (C.c_int, [P, P]),
+    "fg_gdba_step": (C.c_int, [P, C.c_int32, P]),
+    "fg_gdba_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "fg_gdba_launch_count": (C.c_int64, [P]),
     "fg_solution_cost": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
                                    C.c_int32, P, P, C.c_double, P, P]),
 }

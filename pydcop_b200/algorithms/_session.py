@@ -232,8 +232,13 @@ class GpuSession:
         p = dict(self.params)
         if factory is not None:
             return factory(self.kind, layout, inst, dict(p, mode=self.mode))
-        from ..engine import DsaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+        from ..engine import DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
         precision = p.get("precision", "f64")
+        if self.kind == "gdba":  # variables are packed in name order: rank == index
+            return GdbaEngine(layout, precision=precision, mode=self.mode, modifier=p.get("modifier", "A"),
+                              violation=p.get("violation", "NZ"), increase_mode=p.get("increase_mode", "E"),
+                              stop_cycle=p.get("stop_cycle", 0), seed=p.get("seed", 0),
+                              isolated_value=inst.get("isolated_value"))
         if self.kind == "mgm2":  # variables are packed in name order: rank == index
             return Mgm2Engine(layout, precision=precision, mode=self.mode,
                               threshold=p.get("threshold", 0.5), favor=p.get("favor", "unilateral"),

@@ -1,0 +1,175 @@
+// GDBA for all variables at once: C-ABI entry points fg_gdba_* and their kernels
+// (csrc/gdba_kernels.cuh, which states the floating-point operand order).  Its own translation unit,
+// so the MaxSum / DSA / MGM / MGM-2 code is compiled exactly as before.
+#include <cstdio>
+#include <new>
+#include <vector>
+
+#include "common.cuh"
+#include "gdba_kernels.cuh"
+
+struct fg_gdba {
+  fg_gdba_desc_t d;
+  std::vector<fg_class_t> classes;
+  fg_class_t *dev_classes = nullptr;
+  int64_t cycle = 0;
+  int64_t launches = 0;
+  char err[512] = {0};
+};
+
+static char g_gdba_static_err[64] = "invalid handle";
+
+static inline unsigned gdba_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
+
+static MgmSide gdba_side(const fg_gdba *h) {
+  const fg_gdba_desc_t &d = h->d;
+  return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr};
+}
+
+extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
+  if (!desc || !out) return FG_ERR_ARG;
+  *out = nullptr;
+  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
+  if (desc->precision != FG_F32 && desc->precision != FG_F64) return FG_ERR_ARG;
+  fg_gdba *h = new (std::nothrow) fg_gdba();
+  if (!h) return FG_ERR_ARG;
+  h->d = *desc;
+  h->classes.assign(desc->classes, desc->classes + desc->n_classes);
+  h->d.classes = h->classes.data();
+  *out = h;
+  for (auto &c : h->classes) {
+    if (c.arity < 1 || c.arity > FG_MAX_ARITY) {
+      snprintf(h->err, sizeof(h->err), "class arity %d out of range", c.arity);
+      return FG_ERR_ARG;
+    }
+    int64_t ts = 1;
+    for (int i = 0; i < c.arity; ++i) {
+      if (c.dom[i] < 1 || c.dom[i] > FG_MAX_DOM) {
+        snprintf(h->err, sizeof(h->err), "domain size %d out of range", c.dom[i]);
+        return FG_ERR_ARG;
+      }
+      ts *= c.dom[i];
+    }
+    if (ts != c.table_size) {
+      snprintf(h->err, sizeof(h->err), "class size mismatch");
+      return FG_ERR_ARG;
+    }
+  }
+  if (desc->modifier != FG_GDBA_MODIFIER_A && desc->modifier != FG_GDBA_MODIFIER_M) {
+    snprintf(h->err, sizeof(h->err), "modifier %d is not one of A (0), M (1)", desc->modifier);
+    return FG_ERR_ARG;
+  }
+  if (desc->violation < FG_GDBA_VIOLATION_NZ || desc->violation > FG_GDBA_VIOLATION_MX) {
+    snprintf(h->err, sizeof(h->err), "violation %d is not one of NZ (0), NM (1), MX (2)", desc->violation);
+    return FG_ERR_ARG;
+  }
+  if (desc->increase_mode < FG_GDBA_INCREASE_E || desc->increase_mode > FG_GDBA_INCREASE_T) {
+    snprintf(h->err, sizeof(h->err), "increase_mode %d is not one of E (0), R (1), C (2), T (3)",
+             desc->increase_mode);
+    return FG_ERR_ARG;
+  }
+  if (desc->stop_cycle < 0) {
+    snprintf(h->err, sizeof(h->err), "negative stop_cycle %d", desc->stop_cycle);
+    return FG_ERR_ARG;
+  }
+  if (desc->mod_size < 0 || (desc->increase_mode == FG_GDBA_INCREASE_T && desc->mod_size < desc->n_edges)) {
+    snprintf(h->err, sizeof(h->err), "mod_size %lld too small", (long long)desc->mod_size);
+    return FG_ERR_ARG;
+  }
+  if (desc->n_vars > 0 &&
+      (!desc->dev_tables || !desc->dev_unary || !desc->dev_unary_off || !desc->dev_dom_size || !desc->dev_var_id ||
+       !desc->dev_var_rank || !desc->dev_var_ptr || !desc->dev_nbr_ptr || !desc->dev_nbr_idx || !desc->dev_value[0] ||
+       !desc->dev_value[1] || !desc->dev_cost || !desc->dev_has_cost || !desc->dev_improve ||
+       !desc->dev_new_value || !desc->dev_breakout)) {
+    snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
+    return FG_ERR_ARG;
+  }
+  if (desc->n_edges > 0 &&
+      (!desc->dev_edge_var || !desc->dev_edge_class || !desc->dev_slot_edge || !desc->dev_violated ||
+       !desc->dev_mod || (desc->increase_mode != FG_GDBA_INCREASE_T && !desc->dev_mod_off) ||
+       (desc->violation != FG_GDBA_VIOLATION_NZ && !desc->dev_viol_ref))) {
+    snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
+    return FG_ERR_ARG;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
+    cudaGetLastError();
+    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
+    return FG_ERR_CUDA;
+  }
+  size_t bytes = sizeof(fg_class_t) * (h->classes.empty() ? 1 : h->classes.size());
+  CUDA_TRY(h, cudaMalloc(&h->dev_classes, bytes));
+  if (!h->classes.empty())
+    CUDA_TRY(h, cudaMemcpy(h->dev_classes, h->classes.data(), sizeof(fg_class_t) * h->classes.size(), cudaMemcpyHostToDevice));
+  return FG_OK;
+}
+
+extern "C" int fg_gdba_destroy(fg_gdba_t h) {
+  if (h && h->dev_classes) cudaFree(h->dev_classes);
+  delete h;
+  return FG_OK;
+}
+
+extern "C" const char *fg_gdba_last_error(fg_gdba_t h) { return h ? h->err : g_gdba_static_err; }
+
+extern "C" int fg_gdba_init(fg_gdba_t h, void *stream) {
+  if (!h) return FG_ERR_ARG;
+  const fg_gdba_desc_t &d = h->d;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d.mod_size > 0) CUDA_TRY(h, cudaMemsetAsync(d.dev_mod, 0, sizeof(int32_t) * (size_t)d.mod_size, st));
+  if (d.n_vars) {
+    k_mgm_init<<<gdba_blocks(d.n_vars, 128), 128, 0, st>>>(gdba_side(h), d.n_vars, d.dev_init_value, d.seed,
+                                                          d.dev_value[0], d.dev_has_cost);
+    ++h->launches;
+  }
+  CUDA_TRY(h, cudaGetLastError());
+  h->cycle = 0;
+  return FG_OK;
+}
+
+static bool gdba_finished(const fg_gdba *h) { return h->d.stop_cycle && h->cycle + 1 >= h->d.stop_cycle; }
+
+template <typename T>
+static int gdba_cycle_t(fg_gdba *h, cudaStream_t st) {
+  const fg_gdba_desc_t &d = h->d;
+  if (d.n_vars) {
+    const MgmSide g = gdba_side(h);
+    const uint32_t cyc = (uint32_t)(h->cycle + 1);
+    const int n = d.n_vars;
+    int32_t *vin = d.dev_value[h->cycle & 1], *vout = d.dev_value[(h->cycle + 1) & 1];
+    const int64_t *mod_off = d.increase_mode == FG_GDBA_INCREASE_T ? nullptr : d.dev_mod_off;
+    k_gdba_eval<T><<<gdba_blocks(n, 128), 128, 0, st>>>(
+        g, n, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_unary_off, (const T *)d.dev_viol_ref,
+        d.dev_mod, mod_off, d.modifier, d.violation, vin, (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_improve,
+        d.dev_new_value, d.dev_violated, d.mode_max, d.seed, cyc);
+    k_gdba_decide<T><<<gdba_blocks(n, 256), 256, 0, st>>>(g, n, (const T *)d.dev_improve, d.dev_new_value,
+                                                          d.dev_violated, d.dev_mod, mod_off, d.increase_mode,
+                                                          d.mode_max, vin, vout, (T *)d.dev_cost,
+                                                          d.dev_breakout);
+    h->launches += 2;
+  }
+  CUDA_TRY(h, cudaGetLastError());
+  ++h->cycle;
+  return FG_OK;
+}
+
+extern "C" int fg_gdba_step(fg_gdba_t h, int32_t n_cycles, void *stream) {
+  if (!h) return FG_ERR_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  for (int i = 0; i < n_cycles; ++i) {
+    if (gdba_finished(h)) break;
+    int rc = h->d.precision == FG_F64 ? gdba_cycle_t<double>(h, st) : gdba_cycle_t<float>(h, st);
+    if (rc != FG_OK) return rc;
+  }
+  return FG_OK;
+}
+
+extern "C" int fg_gdba_current(fg_gdba_t h, int64_t *cycle, int32_t *finished) {
+  if (!h) return FG_ERR_ARG;
+  if (cycle) *cycle = h->cycle;
+  if (finished) *finished = gdba_finished(h) ? 1 : 0;
+  return FG_OK;
+}
+
+extern "C" int64_t fg_gdba_launch_count(fg_gdba_t h) { return h ? h->launches : -1; }

@@ -879,3 +879,221 @@ class Mgm2Engine(_EngineBase):
         """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
         out = self._solution_cost(self.value, infinity, unary).cpu().numpy()
         return float(out[0]), int(out[1])
+
+
+def gdba_host_arrays(layout: FactorGraphLayout, nbr_ptr, increase_mode="E", violation="NZ"):
+    """GDBA's host-side arrays, internal order:
+    mod_off   per slot, start of its modifier table (increase modes E / R / C; -1 where the slot's constraint
+              does not span {variable} + all its neighbours, so the reference never reads what those modes
+              write there), None with T (one count per slot)
+    mod_size  int32 elements of the modifier array
+    viol_ref  per internal factor, the min (NM) or max (MX) of its base table, None with NZ
+    canon_slot  canonical slot (var_ptr / var_con order) of every internal slot, and canon_mod_off the
+              start of every canonical slot's entries in the flattened `modifiers()` view."""
+    L = layout
+    E = L.n_edges
+    arity = np.array([c.arity for c in L.classes], dtype=np.int64)
+    tsize = np.array([c.table_size for c in L.classes], dtype=np.int64)
+    cls = L.edge_class[L.slot_edge].astype(np.int64) if E else np.zeros(0, np.int64)
+    deg = np.diff(nbr_ptr).astype(np.int64)
+    slot_deg = np.repeat(deg, np.diff(L.var_ptr))
+    slot_size = tsize[cls]
+    if increase_mode == "T":
+        mod_off, mod_size = None, E
+    else:
+        span = (slot_deg > 0) & (arity[cls] == slot_deg + 1)
+        size = np.where(span, slot_size, 0)
+        start = np.cumsum(size) - size
+        mod_off = np.where(span, start, -1).astype(np.int64)
+        mod_size = int(size.sum())
+    viol_ref = None
+    if violation != "NZ" and L.n_factors:
+        viol_ref = np.zeros(L.n_factors, dtype=np.float64)
+        for c in L.classes:
+            t = L.tables[c.table_base:c.table_base + c.n_factors * c.table_size].reshape(c.n_factors, c.table_size)
+            viol_ref[c.first_factor:c.first_factor + c.n_factors] = t.min(1) if violation == "NM" else t.max(1)
+    pos = np.empty(E, dtype=np.int64)
+    pos[L.canon_var_edge] = np.arange(E)
+    canon_slot = pos[L.slot_canon_edge] if E else np.zeros(0, np.int64)
+    canon_size = np.zeros(E, dtype=np.int64)
+    canon_size[canon_slot] = slot_size
+    canon_mod_off = np.concatenate([[0], np.cumsum(canon_size)]).astype(np.int64)
+    return dict(mod_off=mod_off, mod_size=int(mod_size), viol_ref=viol_ref, canon_slot=canon_slot,
+                canon_mod_off=canon_mod_off)
+
+
+def gdba_modifiers_view(h, mods, base_mod, increase_mode):
+    """Flattened modifiers as reads see them (canonical variable, slot and table entry order) from the
+    int32 counts `mods` laid out by gdba_host_arrays `h`."""
+    off = h["canon_mod_off"]
+    out = np.full(int(off[-1]), base_mod, dtype=np.int32)
+    for s, cs in enumerate(h["canon_slot"]):
+        a, b = off[cs], off[cs + 1]
+        if increase_mode == "T":
+            out[a:b] += mods[s]
+        elif h["mod_off"][s] >= 0:
+            out[a:b] += mods[h["mod_off"][s]:h["mod_off"][s] + (b - a)]
+    return out
+
+
+class GdbaEngine(_EngineBase):
+    """All-variables-at-once GDBA (pydcop/algorithms/gdba.py; parameters :181-185).
+
+    modifier       A (base + m, m from 0) | M (base * m, m from 1)
+    violation      NZ (entry != 0) | NM (entry != table min) | MX (entry == table max), on the base table
+    increase_mode  E | R | C | T: which modifiers a breakout raises (E / R / C only on a constraint that spans
+                   the variable's neighbourhood, where the reference reads them; T every entry)
+    stop_cycle     0 = run forever; else rounds stop when round + 1 >= stop_cycle (mgm_gpu's convention;
+                   the reference has none)
+    var_rank       canonical order: position of each variable's NAME in sorted order, the tie break of
+                   gdba.py:657-658 (default: the canonical index)
+    isolated_value canonical order: value index of the variables without neighbours (optimal_cost_value);
+                   default: argopt of the own cost with ties broken on the value index
+    """
+
+    def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", modifier="A",
+                 violation="NZ", increase_mode="E", stop_cycle=0, seed=0, var_rank=None, isolated_value=None):
+        self.lib = _cabi.load()
+        self.device = _require_cuda(device)
+        self.layout = L = layout
+        self.precision = precision
+        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        if mode not in ("min", "max"):
+            raise ValueError(f"invalid mode {mode!r}")
+        for name, v, ok in (("modifier", modifier, _cabi.GDBA_MODIFIERS),
+                            ("violation", violation, _cabi.GDBA_VIOLATIONS),
+                            ("increase_mode", increase_mode, _cabi.GDBA_INCREASE_MODES)):
+            if v not in ok:
+                raise ValueError(f"invalid {name} {v!r}: expected one of {sorted(ok)}")
+        self.modifier, self.increase_mode = modifier, increase_mode
+        h = mgm_host_arrays(L, mode, var_rank, isolated_value)
+        self.has_nbr_host = h["has_nbr"]
+        self.gh = g = gdba_host_arrays(L, h["nbr_ptr"], increase_mode, violation)
+        self.modifier_bytes = g["mod_size"] * 4
+        n = max(L.n_vars, 1)
+        with torch.cuda.device(self.device):
+            self.tables = self._dev(L.tables, tdt)
+            self.unary = self._dev(L.unary, tdt)
+            self.unary_off = self._dev(L.unary_off, torch.int64)
+            self.viol_ref = self._dev(g["viol_ref"], tdt) if g["viol_ref"] is not None else None
+            self.dom_size = self._dev(L.dom_size, torch.int32)
+            self.var_id = self._dev(L.var_order, torch.int32)
+            self.var_rank = self._dev(h["var_rank"], torch.int32)
+            self.edge_var = self._dev(L.edge_var, torch.int32)
+            self.edge_class = self._dev(L.edge_class, torch.int32)
+            self.var_ptr = self._dev(L.var_ptr, torch.int32)
+            self.slot_edge = self._dev(L.slot_edge, torch.int32)
+            self.nbr_ptr = self._dev(h["nbr_ptr"], torch.int32)
+            self.nbr_idx = self._dev(h["nbr_idx"], torch.int32)
+            self.init_value = self._dev(L.init_value, torch.int32)
+            value0 = np.resize(h["value0"], n) if L.n_vars else np.zeros(1, np.int32)
+            self.value = [self._dev(value0, torch.int32), self._dev(value0, torch.int32)]
+            self.cost = self._dev(np.resize(h["cost0"], n) if L.n_vars else np.zeros(1), tdt)
+            self.has_cost = self._dev((~np.resize(h["has_nbr"], n)).astype(np.uint8) if L.n_vars
+                                      else np.zeros(1, np.uint8), torch.uint8)
+            z = lambda k, dt: torch.zeros(max(k, 1), dtype=dt, device=self.device)  # noqa: E731
+            self.improve, self.new_value, self.breakout = z(n, tdt), z(n, torch.int32), z(n, torch.uint8)
+            self.violated = z(L.n_edges, torch.uint8)
+            self.mod = z(g["mod_size"], torch.int32)
+            self.mod_off = self._dev(g["mod_off"], torch.int64) if g["mod_off"] is not None else None
+        self._classes = _class_array(L)
+        d = _cabi.FgGdbaDesc()
+        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
+        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
+        d.classes = C.cast(self._classes, C.POINTER(FgClass))
+        d.dev_tables, d.dev_unary, d.dev_unary_off = _ptr(self.tables), _ptr(self.unary), _ptr(self.unary_off)
+        d.dev_viol_ref = _ptr(self.viol_ref)
+        d.dev_dom_size, d.dev_var_id, d.dev_var_rank = _ptr(self.dom_size), _ptr(self.var_id), _ptr(self.var_rank)
+        d.dev_edge_var, d.dev_edge_class = _ptr(self.edge_var), _ptr(self.edge_class)
+        d.dev_var_ptr, d.dev_slot_edge = _ptr(self.var_ptr), _ptr(self.slot_edge)
+        d.dev_nbr_ptr, d.dev_nbr_idx = _ptr(self.nbr_ptr), _ptr(self.nbr_idx)
+        d.dev_init_value = _ptr(self.init_value)
+        d.dev_value[0], d.dev_value[1] = _ptr(self.value[0]), _ptr(self.value[1])
+        d.dev_cost, d.dev_has_cost, d.dev_improve = _ptr(self.cost), _ptr(self.has_cost), _ptr(self.improve)
+        d.dev_new_value, d.dev_violated = _ptr(self.new_value), _ptr(self.violated)
+        d.dev_breakout = _ptr(self.breakout)
+        d.dev_mod, d.dev_mod_off, d.mod_size = _ptr(self.mod), _ptr(self.mod_off), g["mod_size"]
+        d.mode_max = int(mode == "max")
+        d.modifier, d.violation = _cabi.GDBA_MODIFIERS[modifier], _cabi.GDBA_VIOLATIONS[violation]
+        d.increase_mode = _cabi.GDBA_INCREASE_MODES[increase_mode]
+        d.stop_cycle, d.seed = int(stop_cycle or 0), int(seed) & (2 ** 64 - 1)
+        self._desc = d
+        self._h = C.c_void_p()
+        self._check(self.lib.fg_gdba_create(C.byref(d), C.byref(self._h)), "fg_gdba_create")
+
+    def _last_error(self):
+        return (self.lib.fg_gdba_last_error(self._h) or b"").decode()
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self.lib.fg_gdba_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def init(self):
+        with torch.cuda.device(self.device):
+            self._check(self.lib.fg_gdba_init(self._h, self._stream()), "fg_gdba_init")
+        return self
+
+    def step(self, n_cycles=1):
+        with torch.cuda.device(self.device):
+            self._check(self.lib.fg_gdba_step(self._h, int(n_cycles), self._stream()), "fg_gdba_step")
+        return self
+
+    def _current(self):
+        c, f = C.c_int64(), C.c_int32()
+        self.lib.fg_gdba_current(self._h, C.byref(c), C.byref(f))
+        return c.value, bool(f.value)
+
+    @property
+    def cycle(self):
+        return self._current()[0]
+
+    @property
+    def finished(self):
+        return self._current()[1]
+
+    @property
+    def launch_count(self):
+        return int(self.lib.fg_gdba_launch_count(self._h))
+
+    def _value_buffer(self):
+        return self.value[self.cycle % 2]
+
+    def values(self):
+        """(value index, current cost or NaN while the reference's is None) per variable,
+        canonical variable order."""
+        L = self.layout
+        n = L.n_vars
+        cost = self.cost[:n].double().cpu().numpy()
+        cost[self.has_cost[:n].cpu().numpy() == 0] = np.nan
+        return L.vars_to_canonical(self._value_buffer()[:n].cpu().numpy()), L.vars_to_canonical(cost)
+
+    def record(self):
+        """State of the last round, canonical order: improve (NaN without neighbours), new_value (-1
+        without neighbours), violated per canonical slot, breakout, modifiers (see `modifiers`)."""
+        L = self.layout
+        n = L.n_vars
+        conn = self.has_nbr_host[:n]
+        host = lambda t: t[:n].cpu().numpy()  # noqa: E731
+        viol = np.zeros(L.n_edges, dtype=np.uint8)
+        viol[self.gh["canon_slot"]] = self.violated[:L.n_edges].cpu().numpy()
+        return dict(improve=L.vars_to_canonical(np.where(conn, host(self.improve).astype(np.float64), np.nan)),
+                    new_value=L.vars_to_canonical(np.where(conn, host(self.new_value), -1).astype(np.int32)),
+                    violated=viol, breakout=L.vars_to_canonical(host(self.breakout)), modifiers=self.modifiers())
+
+    def modifiers(self):
+        """Every modifier as a read sees it, flattened: canonical variable, its slots in node.constraints
+        order, the constraint's table entries."""
+        return gdba_modifiers_view(self.gh, self.mod.cpu().numpy(), 0 if self.modifier == "A" else 1,
+                                   self.increase_mode)
+
+    def solution_cost(self, infinity=float("inf"), unary=None):
+        """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
+        out = self._solution_cost(self._value_buffer(), infinity, unary).cpu().numpy()
+        return float(out[0]), int(out[1])

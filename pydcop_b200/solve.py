@@ -1,5 +1,5 @@
 """Direct solve: a DCOP file (or arrays, or a pyDcop DCOP object) -> GPU engine -> result dict
-(algorithms: maxsum, dsa, adsa, mgm, mgm2).
+(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba).
 
 The plugin modules (pydcop_b200/algorithms/) keep pyDcop's orchestrator, agents and one Python
 computation object per graph node around the engine — that is the drop-in path, and it is what
@@ -10,7 +10,7 @@ pydcop/commands/solve.py:611-624): status, assignment, cost, violation, time, cy
 msg_size.
 
 Parameters and defaults are the reference algorithms' own (maxsum.py:212-220, dsa.py:130-135,
-mgm.py:78-81, mgm2.py:139-143).
+mgm.py:78-81, mgm2.py:139-143, gdba.py:181-185; GDBA adds `stop_cycle` with MGM's convention).
 MaxSum has no termination test of its own (maxsum.py: it runs until `stop_cycle` or the
 orchestrator's timeout), so one of `stop_cycle` / `timeout` is required here as well; status is
 FINISHED when `stop_cycle` was reached and TIMEOUT otherwise, as in the reference
@@ -35,14 +35,17 @@ DSA_DEFAULTS = {"probability": 0.7, "p_mode": "fixed", "variant": "B", "stop_cyc
 ADSA_DEFAULTS = {"period": 0.5, "probability": 0.7, "variant": "B", "stop_cycle": 0}   # adsa.py:121-125 + stop_cycle
 MGM_DEFAULTS = {"break_mode": "lexic", "stop_cycle": 0}
 MGM2_DEFAULTS = {"threshold": 0.5, "favor": "unilateral", "stop_cycle": 0}
+GDBA_DEFAULTS = {"modifier": "A", "violation": "NZ", "increase_mode": "E", "stop_cycle": 0}
 DEFAULTS = {"maxsum": MAXSUM_DEFAULTS, "dsa": DSA_DEFAULTS, "mgm": MGM_DEFAULTS, "adsa": ADSA_DEFAULTS,
-            "mgm2": MGM2_DEFAULTS}
+            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS}
 _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "start_messages": ("leafs", "leafs_vars", "all"),
             "p_mode": ("fixed", "arity"), "variant": ("A", "B", "C"),
-            "break_mode": ("lexic", "random"), "favor": ("unilateral", "no", "coordinated")}
+            "break_mode": ("lexic", "random"), "favor": ("unilateral", "no", "coordinated"),
+            "modifier": ("A", "M"), "violation": ("NZ", "NM", "MX"), "increase_mode": ("E", "R", "C", "T")}
 ALGOS = {"maxsum": "maxsum", "maxsum_gpu": "maxsum", "dsa": "dsa", "dsa_gpu": "dsa",
-         "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa", "mgm2": "mgm2", "mgm2_gpu": "mgm2"}
+         "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa", "mgm2": "mgm2", "mgm2_gpu": "mgm2",
+         "gdba": "gdba", "gdba_gpu": "gdba"}
 
 
 def check_params(kind: str, params: Optional[Dict[str, Any]]) -> Dict[str, Any]:
@@ -136,7 +139,12 @@ def name_rank(dcop: ingest.DcopArrays) -> np.ndarray:
 
 
 def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
-    from .engine import DsaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+    from .engine import DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+    if kind == "gdba":
+        return GdbaEngine(layout, device=device, precision=precision, mode=mode,
+                          modifier=params["modifier"], violation=params["violation"],
+                          increase_mode=params["increase_mode"], stop_cycle=params["stop_cycle"],
+                          seed=seed or 0, var_rank=name_rank(dcop), isolated_value=isolated_values(dcop, mode))
     if kind == "mgm2":
         return Mgm2Engine(layout, device=device, precision=precision, mode=mode,
                           threshold=params["threshold"], favor=params["favor"],
@@ -166,7 +174,7 @@ def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, par
     from .multigpu import ShardedMaxSum, broadcast_owner
     from .multigpu_dsa import ShardedDsa
     rank, world = dist.get_rank(), dist.get_world_size()
-    if kind in ("mgm", "mgm2"):
+    if kind in ("mgm", "mgm2", "gdba"):
         raise ValueError(f"{kind} is not sharded: run it on one GPU")
     kw = dict(sharded_kwargs or {})
     dev = device if device is not None else (torch.device("cuda", torch.cuda.current_device())
@@ -206,7 +214,7 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     noise).
 
     problem      see `load`
-    algo         maxsum | dsa | adsa | mgm | mgm2 (the *_gpu spellings of the plugin modules are accepted)
+    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba (the *_gpu spellings of the plugin modules are accepted)
     algo_params  the reference's parameter names; `stop_cycle` bounds the run in cycles
     timeout      wall-clock bound in seconds (checked every `chunk` cycles)
     precision    f32 | f64 (f64 reproduces the reference's double arithmetic bit for bit)
