@@ -557,6 +557,64 @@ int fg_gdba_step(fg_gdba_t h, int32_t n_cycles, void *stream);
 int fg_gdba_current(fg_gdba_t h, int64_t *cycle, int32_t *finished);
 int64_t fg_gdba_launch_count(fg_gdba_t h);
 
+/* ------------------------------------------------------------------------------------------
+ * DPOP  (pydcop/algorithms/dpop.py: exact UTIL / VALUE propagation over a DFS pseudo-tree).  Every
+ * per-node array is in CANONICAL variable order; the tree, the separators, the term descriptors and
+ * the schedule come from the host (pydcop_b200/pseudotree.py), so a run is a fixed sequence of
+ * launches with nothing read back in between:
+ *   UTIL  util_launches in order: kind 0 = one warp per segment [first, first + count) of
+ *         dev_util_seg_ptr, walking its nodes bottom-up; kind 1 = node `first` on the whole grid
+ *   VALUE value_launches in order (kind 0 only): one warp per heavy path, top down
+ * Summation order, argopt and the unresolved rule: csrc/dpop_kernels.cuh.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t kind, first, count, reserved;
+} fg_dpop_launch_t;
+
+typedef struct {
+  int32_t abi_version, precision;
+  int32_t n_vars, mode_max;
+  int64_t n_terms, n_tdims;
+  int64_t arena_size;              /* T elements of dev_arena */
+  const void *dev_unary;           /* T[...] the layout's variable costs (internal order) */
+  const void *dev_tables;          /* T[...] the layout's class-major constraint tables */
+  void *dev_arena;                 /* T[arena_size] every node's UTIL */
+  const int32_t *dev_dom_size;     /* [n_vars] */
+  const int64_t *dev_unary_off;    /* [n_vars] */
+  const int64_t *dev_util_off;     /* [n_vars] */
+  const int64_t *dev_util_size;    /* [n_vars] */
+  const int32_t *dev_sep_ptr;      /* [n_vars+1] */
+  const int32_t *dev_sep_var;      /* separators, root side first, at most FG_DPOP_MAX_SEP (32) each */
+  const int32_t *dev_term_ptr;     /* [n_vars+1] */
+  const int32_t *dev_term_kind;    /* [n_terms] 0 = child UTIL (arena), 1 = constraint (tables) */
+  const int64_t *dev_term_base;    /* [n_terms] */
+  const int64_t *dev_term_own;     /* [n_terms] */
+  const int32_t *dev_tdim_ptr;     /* [n_terms+1] */
+  const int32_t *dev_tdim_pos;     /* [n_tdims] */
+  const int64_t *dev_tdim_stride;  /* [n_tdims] */
+  const int32_t *dev_util_nodes;   /* UTIL segments' nodes, bottom-up */
+  const int32_t *dev_util_seg_ptr; /* [n_util_segs+1] */
+  const int32_t *dev_value_nodes;  /* heavy paths' nodes, top-down */
+  const int32_t *dev_value_seg_ptr; /* [n_value_segs+1] */
+  int32_t n_util_segs, n_value_segs;
+  int32_t n_util_launches, n_value_launches;
+  const fg_dpop_launch_t *util_launches;   /* HOST */
+  const fg_dpop_launch_t *value_launches;  /* HOST */
+  int32_t *dev_value;              /* [n_vars] chosen value index */
+  void *dev_cost;                  /* T[n_vars] the chosen value's joined entry (NaN when unresolved) */
+  int32_t *dev_unresolved;         /* [1] nodes where no value reached the best (the reference raises) */
+  int32_t max_sep, reserved0;
+} fg_dpop_desc_t;
+
+typedef struct fg_dpop *fg_dpop_t;
+
+int fg_dpop_create(const fg_dpop_desc_t *desc, fg_dpop_t *out);
+int fg_dpop_destroy(fg_dpop_t h);
+const char *fg_dpop_last_error(fg_dpop_t h);
+/* both phases: every UTIL launch, then every VALUE launch; the unresolved count is reset first. */
+int fg_dpop_run(fg_dpop_t h, void *stream);
+int64_t fg_dpop_launch_count(fg_dpop_t h);
+
 /* Solution cost (next-tier row §8f.1; pydcop/dcop/dcop.py:319-367 `solution_cost`, called by the
  * orchestrator at the end of a run and at every metric tick, orchestrator.py:1229-1231): over the factors
  * of every non-ghost class the table entry at the assignment, over the first n_vars variables

@@ -117,6 +117,27 @@ class FgGdbaDesc(C.Structure):
                 ("mod_size", C.c_int64), ("seed", C.c_uint64)]
 
 
+class FgDpopLaunch(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("first", C.c_int32), ("count", C.c_int32), ("reserved", C.c_int32)]
+
+
+class FgDpopDesc(C.Structure):
+    _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
+                ("n_vars", C.c_int32), ("mode_max", C.c_int32),
+                ("n_terms", C.c_int64), ("n_tdims", C.c_int64), ("arena_size", C.c_int64),
+                ("dev_unary", P), ("dev_tables", P), ("dev_arena", P),
+                ("dev_dom_size", P), ("dev_unary_off", P), ("dev_util_off", P), ("dev_util_size", P),
+                ("dev_sep_ptr", P), ("dev_sep_var", P), ("dev_term_ptr", P), ("dev_term_kind", P),
+                ("dev_term_base", P), ("dev_term_own", P), ("dev_tdim_ptr", P), ("dev_tdim_pos", P),
+                ("dev_tdim_stride", P), ("dev_util_nodes", P), ("dev_util_seg_ptr", P),
+                ("dev_value_nodes", P), ("dev_value_seg_ptr", P),
+                ("n_util_segs", C.c_int32), ("n_value_segs", C.c_int32),
+                ("n_util_launches", C.c_int32), ("n_value_launches", C.c_int32),
+                ("util_launches", C.POINTER(FgDpopLaunch)), ("value_launches", C.POINTER(FgDpopLaunch)),
+                ("dev_value", P), ("dev_cost", P), ("dev_unresolved", P),
+                ("max_sep", C.c_int32), ("reserved0", C.c_int32)]
+
+
 GDBA_MODIFIERS = {"A": 0, "M": 1}
 GDBA_VIOLATIONS = {"NZ": 0, "NM": 1, "MX": 2}
 GDBA_INCREASE_MODES = {"E": 0, "R": 1, "C": 2, "T": 3}
@@ -204,6 +225,11 @@ SYMBOLS = {
     "fg_gdba_step": (C.c_int, [P, C.c_int32, P]),
     "fg_gdba_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "fg_gdba_launch_count": (C.c_int64, [P]),
+    "fg_dpop_create": (C.c_int, [C.POINTER(FgDpopDesc), C.POINTER(P)]),
+    "fg_dpop_destroy": (C.c_int, [P]),
+    "fg_dpop_last_error": (C.c_char_p, [P]),
+    "fg_dpop_run": (C.c_int, [P, P]),
+    "fg_dpop_launch_count": (C.c_int64, [P]),
     "fg_solution_cost": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
                                    C.c_int32, P, P, C.c_double, P, P]),
 }

@@ -59,6 +59,7 @@ class GpuSession:
         self.lock = threading.RLock()
         self.variables: Dict[str, Any] = {}       # name -> variable object
         self.var_links: Dict[str, List[str]] = {}  # name -> constraint names in `links` order
+        self.tree_links: Dict[str, list] = {}      # dpop: name -> (type, target) of its PseudoTreeLinks
         self.constraints: Dict[str, Any] = {}     # name -> constraint object
         self.needed_factors: set = set()
         self.needed_vars: set = set()
@@ -124,6 +125,11 @@ class GpuSession:
                 self.needed_vars.update(v.name for v in c.dimensions)
             self.members.add(name)
             self._set_params(params, mode)
+
+    def add_tree_links(self, name, links):
+        """The node's pseudo-tree links (parent, children, pseudo_parent, pseudo_children), in order."""
+        with self.lock:
+            self.tree_links[name] = [(l.type, l.target) for l in links if l.source == name]
 
     def add_factor(self, name, constraint, params=None, mode="min"):
         with self.lock:
@@ -232,8 +238,10 @@ class GpuSession:
         p = dict(self.params)
         if factory is not None:
             return factory(self.kind, layout, inst, dict(p, mode=self.mode))
-        from ..engine import DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+        from ..engine import DpopEngine, DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
         precision = p.get("precision", "f64")
+        if self.kind == "dpop":
+            return DpopEngine(layout, inst["tree"], precision=precision, mode=self.mode)
         if self.kind == "gdba":  # variables are packed in name order: rank == index
             return GdbaEngine(layout, precision=precision, mode=self.mode, modifier=p.get("modifier", "A"),
                               violation=p.get("violation", "NZ"), increase_mode=p.get("increase_mode", "E"),
@@ -271,9 +279,11 @@ class GpuSession:
                     rnd = random.Random(seed) if seed else random
                     inst["unary"] = inst["unary"] + np.array(
                         [rnd.uniform(0, noise) for _ in range(len(inst["unary"]))])
+            elif self.kind == "dpop":
+                inst["tree"] = self._pseudo_tree(inst)
             else:
                 inst["isolated_value"] = self._isolated_values(inst)
-            layout = build_layout(**{k: v for k, v in inst.items() if k != "isolated_value"})
+            layout = build_layout(**{k: v for k, v in inst.items() if k not in ("isolated_value", "tree")})
             engine = self._make_engine(layout, inst)
             engine.init()
             stop_cycle = int(self.params.get("stop_cycle", 0) or 0)
@@ -313,6 +323,15 @@ class GpuSession:
             dom = domain_values(self.variables[n])
             vals[n] = (dom[int(idx[i])], float(costs[i]) if costs is not None else 0.0)
         self.snapshot = Snapshot(cycle, vals, None, finished)
+
+    def _pseudo_tree(self, inst):
+        """The orchestrator's pseudo-tree over the packed arrays; each node joins the constraints it owns
+        in its node.constraints order (dpop.py:191-199)."""
+        from ..pseudotree import tree_from_links
+        cidx = {n: i for i, n in enumerate(sorted(self.constraints))}
+        con_order = [[cidx[c] for c in self.var_links[n]] for n in self.var_order]
+        return tree_from_links(self.var_order, self.tree_links, inst["dom_size"], inst["factor_ptr"],
+                               inst["edge_var"], con_order)
 
     def _isolated_values(self, inst):
         """DSA on_start for a variable without neighbours (dsa.py:278-289): argopt of

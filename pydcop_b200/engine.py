@@ -1097,3 +1097,146 @@ class GdbaEngine(_EngineBase):
         """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
         out = self._solution_cost(self._value_buffer(), infinity, unary).cpu().numpy()
         return float(out[0]), int(out[1])
+
+
+class DpopEngine(_EngineBase):
+    """DPOP (pydcop/algorithms/dpop.py) on a pseudo-tree (pydcop_b200.pseudotree): one `step()` runs the
+    UTIL phase bottom-up and the VALUE phase top-down as a fixed, host-computed sequence of launches
+    (pseudotree.schedule), after which `finished` is true.  Every node's UTIL stays in one arena.
+
+    tree  a completed PseudoTree over the layout's canonical variables and constraints (build_tree, or
+          tree_from_links on the plugin path)
+    """
+
+    def __init__(self, layout: FactorGraphLayout, tree, device=None, precision="f64", mode="min"):
+        from . import pseudotree as pt
+        self.lib = _cabi.load()
+        self.device = _require_cuda(device)
+        self.layout = L = layout
+        self.tree = tree
+        self.precision = precision
+        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        if mode not in ("min", "max"):
+            raise ValueError(f"invalid mode {mode!r}")
+        if tree.n_vars != L.n_vars or len(tree.owner) != L.n_factors:
+            raise ValueError("the pseudo-tree does not match the layout")
+        elem = np.dtype(self.np_dtype).itemsize
+        self._util_off, arena = pt.arena_layout(tree)
+        big_u, big_sep = pt.largest_separator(tree)
+        self.util_bytes = arena * elem
+        free, _ = torch.cuda.mem_get_info(self.device)
+        if self.util_bytes > free:
+            names = ", ".join(str(v) for v in big_sep)
+            raise EngineError(
+                f"DPOP needs {self.util_bytes} bytes of UTIL tables but {free} bytes of device memory are free; "
+                f"the largest separator is that of variable {big_u}: {len(big_sep)} variables [{names}] "
+                f"({tree.util_size[big_u]} entries)")
+        max_sep = max((len(s) for s in tree.sep), default=0)
+        if max_sep > pt.MAX_SEP:
+            raise EngineError(f"a separator of {max_sep} variables: the kernels decode at most {pt.MAX_SEP}")
+        self.sched = s = pt.schedule(tree)
+        d_ = pt.terms(tree, L)
+        self.unresolved_host = None
+        with torch.cuda.device(self.device):
+            self.tables = self._dev(L.tables, tdt)
+            self.unary = self._dev(L.unary, tdt)
+            self.arena = torch.empty(max(arena, 1), dtype=tdt, device=self.device)
+            self.dev = {k: self._dev(v, torch.int64 if v.dtype == np.int64 else torch.int32)
+                        for k, v in d_.items() if k != "arena_size"}
+            self.nodes = {k: self._dev(getattr(s, k), torch.int32)
+                          for k in ("util_nodes", "util_seg_ptr", "value_nodes", "value_seg_ptr")}
+            n = max(L.n_vars, 1)
+            self.value = torch.zeros(n, dtype=torch.int32, device=self.device)
+            self.cost = torch.zeros(n, dtype=tdt, device=self.device)
+            self.unresolved_dev = torch.zeros(1, dtype=torch.int32, device=self.device)
+        launches = lambda ls: (_cabi.FgDpopLaunch * max(1, len(ls)))(*[_cabi.FgDpopLaunch(*l, 0) for l in ls])  # noqa: E731
+        self._ul, self._vl = launches(s.util_launches), launches(s.value_launches)
+        self._classes = _class_array(L)
+        dv = self.dev
+        d = _cabi.FgDpopDesc()
+        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
+        d.n_vars, d.mode_max = L.n_vars, int(mode == "max")
+        d.n_terms, d.n_tdims, d.arena_size = len(d_["term_kind"]), len(d_["tdim_pos"]), arena
+        d.dev_unary, d.dev_tables, d.dev_arena = _ptr(self.unary), _ptr(self.tables), _ptr(self.arena)
+        for k in ("dom_size", "unary_off", "util_off", "util_size", "sep_ptr", "sep_var", "term_ptr", "term_kind",
+                  "term_base", "term_own", "tdim_ptr", "tdim_pos", "tdim_stride"):
+            setattr(d, "dev_" + k, _ptr(dv[k]))
+        for k, t in self.nodes.items():
+            setattr(d, "dev_" + k, _ptr(t))
+        d.n_util_segs, d.n_value_segs = len(s.util_seg_ptr) - 1, len(s.value_seg_ptr) - 1
+        d.n_util_launches, d.n_value_launches = len(s.util_launches), len(s.value_launches)
+        d.util_launches = C.cast(self._ul, C.POINTER(_cabi.FgDpopLaunch))
+        d.value_launches = C.cast(self._vl, C.POINTER(_cabi.FgDpopLaunch))
+        d.dev_value, d.dev_cost, d.dev_unresolved = _ptr(self.value), _ptr(self.cost), _ptr(self.unresolved_dev)
+        d.max_sep = max_sep
+        self._desc = d
+        self._h = C.c_void_p()
+        self._done = False
+        self._check(self.lib.fg_dpop_create(C.byref(d), C.byref(self._h)), "fg_dpop_create")
+
+    def _last_error(self):
+        return (self.lib.fg_dpop_last_error(self._h) or b"").decode()
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self.lib.fg_dpop_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def init(self):
+        self._done = False
+        return self
+
+    def step(self, n_cycles=1):
+        """Both phases (DPOP is not iterative: further steps do nothing)."""
+        if not self._done and n_cycles > 0:
+            with torch.cuda.device(self.device):
+                self._check(self.lib.fg_dpop_run(self._h, self._stream()), "fg_dpop_run")
+            self._done = True
+        return self
+
+    @property
+    def finished(self):
+        return self._done
+
+    @property
+    def cycle(self):
+        return 0
+
+    @property
+    def launch_count(self):
+        return int(self.lib.fg_dpop_launch_count(self._h))
+
+    @property
+    def unresolved(self):
+        """Nodes where no value reached the best (the reference raises IndexError there)."""
+        return int(self.unresolved_dev.item())
+
+    def values(self):
+        """(value index, the chosen value's joined entry — the reference's reported cost) per variable,
+        canonical order."""
+        n = self.layout.n_vars
+        return self.value[:n].cpu().numpy(), self.cost[:n].double().cpu().numpy()
+
+    def util(self, var):
+        """(separator as canonical variable indices, root side first; the UTIL table shaped by their
+        domain sizes) of canonical variable `var`."""
+        off = self._util_off
+        sep = self.tree.sep[var]
+        n = self.tree.util_size[var]
+        shape = tuple(int(self.layout.canon_dom_size[v]) for v in sep)
+        return sep, self.arena[off[var]:off[var] + n].double().cpu().numpy().reshape(shape)
+
+    def solution_cost(self, infinity=float("inf"), unary=None):
+        """(cost, violations) of the assignment on the device (dcop.py:319-367)."""
+        L = self.layout
+        with torch.cuda.device(self.device):
+            internal = self.value[:max(L.n_vars, 1)][torch.as_tensor(L.var_order.astype(np.int64), device=self.device)] \
+                if L.n_vars else self.value
+            out = self._solution_cost(internal.contiguous(), infinity, unary).cpu().numpy()
+        return float(out[0]), int(out[1])

@@ -137,3 +137,30 @@ def algorithmic_bytes_per_cycle_inst(inst, value_bytes=4):
     deg = np.bincount(ev, minlength=len(dom)).astype(np.int64)
     b += int((w * dom + deg * (3 * w * dom + 6) + 12).sum())
     return b
+
+
+def bounded_separator_instance(n_vars, d, back, span=2, p_back=1.0, seed=0, float_costs=False):
+    """DPOP workloads: a random tree (the parent of variable i is one of the `span` variables before it, so
+    the tree is deep) plus, from each variable with probability `p_back`, one binary constraint to each of
+    its ancestors 2..back+1 levels up.  Every constraint joins a variable to an ancestor, so pseudo-tree
+    separators stay near `back` + 1 variables (tools/dpop_throughput.py reports the ones the DFS actually
+    builds).  Tables are integers(0,10) (or uniform floats), no variable costs."""
+    rng = np.random.default_rng(seed)
+    parent = np.zeros(n_vars, dtype=np.int64)
+    if n_vars > 1:
+        i = np.arange(1, n_vars)
+        parent[1:] = i - 1 - (rng.integers(0, span, size=n_vars - 1) % i)
+    pairs = [np.stack([parent[1:], np.arange(1, n_vars)], 1)]
+    anc = parent.copy()
+    for _ in range(back):
+        anc = np.where(anc > 0, parent[anc], -1) if n_vars else anc
+        take = (anc >= 0) & (rng.uniform(size=n_vars) < p_back)
+        take[0] = False
+        pairs.append(np.stack([anc[take], np.nonzero(take)[0]], 1))
+        anc = np.where(anc >= 0, anc, 0)
+    scopes = np.concatenate(pairs).astype(np.int32) if n_vars > 1 else np.zeros((0, 2), np.int32)
+    n_f = len(scopes)
+    tables = (rng.uniform(-5, 5, size=n_f * d * d) if float_costs
+              else rng.integers(0, 10, size=n_f * d * d).astype(np.float64))
+    return dict(dom_size=np.full(n_vars, d, dtype=np.int32), factor_ptr=np.arange(0, 2 * n_f + 1, 2, dtype=np.int64),
+                edge_var=scopes.reshape(-1), tables=tables, unary=np.zeros(n_vars * d))

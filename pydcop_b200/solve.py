@@ -1,5 +1,5 @@
 """Direct solve: a DCOP file (or arrays, or a pyDcop DCOP object) -> GPU engine -> result dict
-(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba).
+(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba, dpop).
 
 The plugin modules (pydcop_b200/algorithms/) keep pyDcop's orchestrator, agents and one Python
 computation object per graph node around the engine — that is the drop-in path, and it is what
@@ -14,7 +14,9 @@ mgm.py:78-81, mgm2.py:139-143, gdba.py:181-185; GDBA adds `stop_cycle` with MGM'
 MaxSum has no termination test of its own (maxsum.py: it runs until `stop_cycle` or the
 orchestrator's timeout), so one of `stop_cycle` / `timeout` is required here as well; status is
 FINISHED when `stop_cycle` was reached and TIMEOUT otherwise, as in the reference
-(orchestrator.py:1262, commands/solve.py:560-580).
+(orchestrator.py:1262, commands/solve.py:560-580).  DPOP is exact and not iterative: it needs neither,
+runs its UTIL and VALUE phases once on the pseudo-tree pydcop_b200.pseudotree builds, and is FINISHED at
+cycle 0.
 
 No CPU path: the engines raise EngineError without a CUDA device.  `engine_factory` exists so
 the host logic can be tested without one.
@@ -37,7 +39,7 @@ MGM_DEFAULTS = {"break_mode": "lexic", "stop_cycle": 0}
 MGM2_DEFAULTS = {"threshold": 0.5, "favor": "unilateral", "stop_cycle": 0}
 GDBA_DEFAULTS = {"modifier": "A", "violation": "NZ", "increase_mode": "E", "stop_cycle": 0}
 DEFAULTS = {"maxsum": MAXSUM_DEFAULTS, "dsa": DSA_DEFAULTS, "mgm": MGM_DEFAULTS, "adsa": ADSA_DEFAULTS,
-            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS}
+            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS, "dpop": {}}
 _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "start_messages": ("leafs", "leafs_vars", "all"),
             "p_mode": ("fixed", "arity"), "variant": ("A", "B", "C"),
@@ -45,13 +47,15 @@ _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "modifier": ("A", "M"), "violation": ("NZ", "NM", "MX"), "increase_mode": ("E", "R", "C", "T")}
 ALGOS = {"maxsum": "maxsum", "maxsum_gpu": "maxsum", "dsa": "dsa", "dsa_gpu": "dsa",
          "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa", "mgm2": "mgm2", "mgm2_gpu": "mgm2",
-         "gdba": "gdba", "gdba_gpu": "gdba"}
+         "gdba": "gdba", "gdba_gpu": "gdba", "dpop": "dpop", "dpop_gpu": "dpop"}
 
 
 def check_params(kind: str, params: Optional[Dict[str, Any]]) -> Dict[str, Any]:
     """Defaults + type / choice validation, the job of AlgoParameterDef
     (pydcop/algorithms/__init__.py:180-290): unknown names and invalid values raise ValueError."""
     defaults = DEFAULTS[kind]
+    if not defaults and params:   # DPOP: exact and not iterative, so no stop_cycle either
+        raise ValueError(f"{kind} takes no parameters: unknown algorithm parameter(s) {sorted(params)}")
     out = dict(defaults)
     for k, v in (params or {}).items():
         if k not in defaults:
@@ -139,7 +143,12 @@ def name_rank(dcop: ingest.DcopArrays) -> np.ndarray:
 
 
 def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
-    from .engine import DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+    from .engine import DpopEngine, DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+    if kind == "dpop":
+        from .pseudotree import build_tree
+        a = dcop.arrays
+        return DpopEngine(layout, build_tree(a["dom_size"], a["factor_ptr"], a["edge_var"]), device=device,
+                          precision=precision, mode=mode)
     if kind == "gdba":
         return GdbaEngine(layout, device=device, precision=precision, mode=mode,
                           modifier=params["modifier"], violation=params["violation"],
@@ -174,7 +183,7 @@ def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, par
     from .multigpu import ShardedMaxSum, broadcast_owner
     from .multigpu_dsa import ShardedDsa
     rank, world = dist.get_rank(), dist.get_world_size()
-    if kind in ("mgm", "mgm2", "gdba"):
+    if kind in ("mgm", "mgm2", "gdba", "dpop"):
         raise ValueError(f"{kind} is not sharded: run it on one GPU")
     kw = dict(sharded_kwargs or {})
     dev = device if device is not None else (torch.device("cuda", torch.cuda.current_device())
@@ -214,7 +223,8 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     noise).
 
     problem      see `load`
-    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba (the *_gpu spellings of the plugin modules are accepted)
+    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba | dpop (the *_gpu spellings of the plugin modules are
+                 accepted)
     algo_params  the reference's parameter names; `stop_cycle` bounds the run in cycles
     timeout      wall-clock bound in seconds (checked every `chunk` cycles)
     precision    f32 | f64 (f64 reproduces the reference's double arithmetic bit for bit)
@@ -225,7 +235,7 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
         raise ValueError(f"unknown algorithm {algo!r}: expected one of {sorted(ALGOS)}")
     kind = ALGOS[algo]
     params = check_params(kind, algo_params)
-    stop_cycle = int(params["stop_cycle"])
+    stop_cycle = 1 if kind == "dpop" else int(params["stop_cycle"])   # DPOP: both phases in one step
     if not stop_cycle and timeout is None:
         raise ValueError(f"{kind} does not stop by itself: give algo_params['stop_cycle'] or a timeout")
     if distributed is None:
@@ -282,7 +292,7 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     else:                                  # engine seam of the CPU tests
         violation, cost = solution_cost(dcop, idx, infinity)
     return {"status": status, "assignment": dcop.assignment(idx), "cost": cost,
-            "violation": violation, "time": time.perf_counter() - t0, "cycle": cycle,
+            "violation": violation, "time": time.perf_counter() - t0, "cycle": 0 if kind == "dpop" else cycle,
             "msg_count": 0, "msg_size": 0,  # nothing crosses an agent boundary
             "algo": kind, "precision": precision, "n_gpus": n_gpus,
             "ingest_time": t_packed - t0,
