@@ -238,35 +238,10 @@ class GpuSession:
         p = dict(self.params)
         if factory is not None:
             return factory(self.kind, layout, inst, dict(p, mode=self.mode))
-        from ..engine import DpopEngine, DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
-        precision = p.get("precision", "f64")
-        if self.kind == "dpop":
-            return DpopEngine(layout, inst["tree"], precision=precision, mode=self.mode)
-        if self.kind == "gdba":  # variables are packed in name order: rank == index
-            return GdbaEngine(layout, precision=precision, mode=self.mode, modifier=p.get("modifier", "A"),
-                              violation=p.get("violation", "NZ"), increase_mode=p.get("increase_mode", "E"),
-                              stop_cycle=p.get("stop_cycle", 0), seed=p.get("seed", 0),
-                              isolated_value=inst.get("isolated_value"))
-        if self.kind == "mgm2":  # variables are packed in name order: rank == index
-            return Mgm2Engine(layout, precision=precision, mode=self.mode,
-                              threshold=p.get("threshold", 0.5), favor=p.get("favor", "unilateral"),
-                              stop_cycle=p.get("stop_cycle", 0), seed=p.get("seed", 0))
-        if self.kind == "mgm":  # variables are packed in name order: rank == index
-            return MgmEngine(layout, precision=precision, mode=self.mode,
-                             stop_cycle=p.get("stop_cycle", 0), seed=p.get("seed", 0),
-                             break_mode=p.get("break_mode", "lexic"),
-                             isolated_value=inst.get("isolated_value"))
-        if self.kind == "maxsum":
-            return MaxSumEngine(layout, precision=precision, mode=self.mode,
-                                damping=p.get("damping", 0.5),
-                                damping_nodes=p.get("damping_nodes", "both"),
-                                stability=p.get("stability", 0.1),
-                                start_messages=p.get("start_messages", "leafs"), record_sent=False)
-        return DsaEngine(layout, precision=precision, mode=self.mode,
-                         probability=p.get("probability", 0.7), p_mode=p.get("p_mode", "fixed"),
-                         variant=p.get("variant", "B"), stop_cycle=p.get("stop_cycle", 0),
-                         seed=p.get("seed", 0), isolated_value=inst.get("isolated_value"),
-                         var_costs=(self.kind == "adsa"))   # A-DSA: candidates carry the variable's own cost
+        from ..engine import make_engine
+        # variables are packed in name order: the name rank equals the index (no var_rank)
+        return make_engine(self.kind, layout, p, mode=self.mode, precision=p.get("precision", "f64"),
+                           seed=p.get("seed", 0), isolated_value=inst.get("isolated_value"), tree=inst.get("tree"))
 
     def _run(self):
         try:

@@ -1,22 +1,14 @@
 // DPOP: C-ABI entry points fg_dpop_* and their kernels (csrc/dpop_kernels.cuh, which states the
 // floating-point operand order).  Its own translation unit, so the other families are compiled exactly
 // as before.
-#include <cstdio>
-#include <new>
-#include <vector>
-
-#include "common.cuh"
+#include "handle.cuh"
 #include "dpop_kernels.cuh"
 
-struct fg_dpop {
+struct fg_dpop : fg_handle_base {   // no class table: classes stays empty
   fg_dpop_desc_t d;
   std::vector<fg_dpop_launch_t> util_launches, value_launches;
-  int64_t launches = 0;
   int n_sm = 132;
-  char err[512] = {0};
 };
-
-static char g_dpop_static_err[64] = "invalid handle";
 
 static DpopNodes dpop_nodes(const fg_dpop_desc_t &d) {
   return DpopNodes{d.dev_dom_size, d.dev_unary_off, d.dev_util_off, d.dev_util_size, d.dev_sep_ptr,
@@ -40,13 +32,8 @@ static bool dpop_check_launches(fg_dpop *h, const std::vector<fg_dpop_launch_t> 
 }
 
 extern "C" int fg_dpop_create(const fg_dpop_desc_t *desc, fg_dpop_t *out) {
-  if (!desc || !out) return FG_ERR_ARG;
-  *out = nullptr;
-  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
-  fg_dpop *h = new (std::nothrow) fg_dpop();
+  fg_dpop *h = fg_alloc(desc, out);
   if (!h) return FG_ERR_ARG;
-  h->d = *desc;
-  *out = h;
   if (desc->precision != FG_F32 && desc->precision != FG_F64) {
     snprintf(h->err, sizeof(h->err), "precision %d is not FG_F32 (0) or FG_F64 (1)", desc->precision);
     return FG_ERR_ARG;
@@ -82,24 +69,17 @@ extern "C" int fg_dpop_create(const fg_dpop_desc_t *desc, fg_dpop_t *out) {
   if (!dpop_check_launches(h, h->util_launches, desc->n_util_segs, true, "UTIL") ||
       !dpop_check_launches(h, h->value_launches, desc->n_value_segs, false, "VALUE"))
     return FG_ERR_ARG;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    cudaGetLastError();
-    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
-    return FG_ERR_CUDA;
-  }
+  int rc = fg_require_device(h);
+  if (rc != FG_OK) return rc;
   int dev = 0;
   CUDA_TRY(h, cudaGetDevice(&dev));
   CUDA_TRY(h, cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev));
   return FG_OK;
 }
 
-extern "C" int fg_dpop_destroy(fg_dpop_t h) {
-  delete h;
-  return FG_OK;
-}
+extern "C" int fg_dpop_destroy(fg_dpop_t h) { return fg_close(h); }
 
-extern "C" const char *fg_dpop_last_error(fg_dpop_t h) { return h ? h->err : g_dpop_static_err; }
+extern "C" const char *fg_dpop_last_error(fg_dpop_t h) { return fg_last_error(h); }
 
 static inline unsigned dpop_warp_blocks(int n_warps) { return (unsigned)((n_warps + 3) / 4); }
 
@@ -137,4 +117,4 @@ extern "C" int fg_dpop_run(fg_dpop_t h, void *stream) {
   return h->d.precision == FG_F64 ? dpop_run_t<double>(h, st) : dpop_run_t<float>(h, st);
 }
 
-extern "C" int64_t fg_dpop_launch_count(fg_dpop_t h) { return h ? h->launches : -1; }
+extern "C" int64_t fg_dpop_launch_count(fg_dpop_t h) { return fg_launch_count(h); }

@@ -1,12 +1,9 @@
 // C-ABI of the pydcop_b200 engine (include/pydcop_b200.h): handle management and kernel launch
 // sequencing.  No torch, no host-side arithmetic on messages, no CPU fallback.
-#include <cstdio>
 #include <cstring>
-#include <new>
 #include <type_traits>
-#include <vector>
 
-#include "common.cuh"
+#include "handle.cuh"
 #include "dsa_generic.cuh"
 #include "maxsum_generic.cuh"
 #include "maxsum_fast.cuh"
@@ -25,19 +22,16 @@ inline unsigned blocks_for(int64_t n, int threads) { return (unsigned)((n + thre
 
 }  // namespace
 
-struct fg_maxsum {
+struct fg_maxsum : fg_handle_base {   // dev_classes unused: the plans own their device tables
   cudaStream_t side_stream = nullptr;   // variable side runs here, concurrently with the factor side
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   fg_maxsum_desc_t d;
-  std::vector<fg_class_t> classes;
   std::vector<fg_varclass_t> varclasses;
   MaxSumFastPlan fast;
   MaxSumWarpPlan warp;   // warp-autonomous kernels (round 2) over the same classes
   TiledRtPlan tiled_rt;  // factor classes of other shapes on the runtime-dimension tiled kernel (maxsum_tiled_rt.cuh)
   bool fast_first = true;   // tiled kernels in cycle 1 as well (PYDCOP_B200_FAST_FIRST=0: generic kernels)
   int cur = 0;
-  int64_t cycle = 0;
-  int64_t launches = 0;
   // multi-GPU: push plan + device-side barrier (fg_maxsum_shard_*)
   bool has_halo = false;
   bool split_push = true;   // r rows right behind the factor side, q rows on the side stream (PYDCOP_B200_PUSH_SPLIT=0: one push after the join)
@@ -56,23 +50,15 @@ struct fg_maxsum {
   fg_halo_plan_t halo;
   uint64_t epoch = 0;
   cudaEvent_t *prof = nullptr;   // fg_maxsum_shard_profile: 8 timing events recorded inside a cycle
-  char err[512] = {0};
 };
 
-struct fg_dsa {
+struct fg_dsa : fg_handle_base {
   fg_dsa_desc_t d;
-  std::vector<fg_class_t> classes;
-  fg_class_t *dev_classes = nullptr;
   int cur = 0;
-  int64_t cycle = 0;
-  int64_t launches = 0;
   bool has_halo = false;
   fg_halo_plan_t halo;
   uint64_t epoch = 0;
-  char err[512] = {0};
 };
-
-static char g_static_err[256] = "invalid handle";
 
 extern "C" int fg_abi_version(void) { return FG_ABI_VERSION; }
 
@@ -82,49 +68,23 @@ extern "C" int fg_device_count(void) {
   return n;
 }
 
-static int check_class(const fg_class_t &c, char *err, size_t n) {
-  if (c.arity < 1 || c.arity > FG_MAX_ARITY) { snprintf(err, n, "class arity %d out of range", c.arity); return FG_ERR_ARG; }
-  int64_t ts = 1; int rt = 0;
-  for (int i = 0; i < c.arity; ++i) {
-    if (c.dom[i] < 1 || c.dom[i] > FG_MAX_DOM) { snprintf(err, n, "domain size %d out of range", c.dom[i]); return FG_ERR_ARG; }
-    if (c.row_off[i] < rt) { snprintf(err, n, "row_off overlaps the previous row"); return FG_ERR_ARG; }
-    ts *= c.dom[i]; rt = c.row_off[i] + c.dom[i];
-  }
-  if (ts != c.table_size || rt > c.row_total) { snprintf(err, n, "class size mismatch"); return FG_ERR_ARG; }
-  return FG_OK;
-}
-
 // ---------------------------------------------------------------------------------------------
 // MaxSum
 // ---------------------------------------------------------------------------------------------
 extern "C" int fg_maxsum_create(const fg_maxsum_desc_t *desc, fg_maxsum_t *out) {
-  if (!desc || !out) return FG_ERR_ARG;
-  *out = nullptr;
-  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
-  if (desc->precision != FG_F32 && desc->precision != FG_F64) return FG_ERR_ARG;
-  fg_maxsum *h = new (std::nothrow) fg_maxsum();
-  if (!h) return FG_ERR_ARG;
-  h->d = *desc;
-  h->classes.assign(desc->classes, desc->classes + desc->n_classes);
-  h->d.classes = h->classes.data();
+  int rc = fg_open(desc, out);
+  if (rc != FG_OK) return rc;
+  fg_maxsum *h = *out;
   if (desc->n_varclasses > 0 && desc->varclasses)
     h->varclasses.assign(desc->varclasses, desc->varclasses + desc->n_varclasses);
   h->d.varclasses = h->varclasses.data();
-  *out = h;
-  for (auto &c : h->classes) {
-    int rc = check_class(c, h->err, sizeof(h->err));
-    if (rc != FG_OK) return rc;
-  }
   int64_t covered = 0;
   for (auto &vc : h->varclasses) covered += vc.n_slots;
   if (covered != desc->n_edges) {
     snprintf(h->err, sizeof(h->err), "variable classes cover %lld slots, expected %d", (long long)covered, desc->n_edges);
     return FG_ERR_ARG;
   }
-  if (fg_device_count() <= 0) {
-    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
-    return FG_ERR_CUDA;
-  }
+  if ((rc = fg_require_device(h)) != FG_OK) return rc;
   maxsum_fast_plan(h->d, h->classes, h->varclasses, h->fast);
   if (maxsum_warp_plan(h->d, h->varclasses, h->fast, h->warp) != FG_OK) {
     snprintf(h->err, sizeof(h->err), "tile descriptors of the variable side: %s", cudaGetErrorString(cudaGetLastError()));
@@ -169,7 +129,7 @@ extern "C" int fg_maxsum_destroy(fg_maxsum_t h) {
   return FG_OK;
 }
 
-extern "C" const char *fg_maxsum_last_error(fg_maxsum_t h) { return h ? h->err : g_static_err; }
+extern "C" const char *fg_maxsum_last_error(fg_maxsum_t h) { return fg_last_error(h); }
 
 template <typename T>
 static int maxsum_init_t(fg_maxsum *h, cudaStream_t st) {
@@ -383,7 +343,7 @@ extern "C" int fg_maxsum_current(fg_maxsum_t h, int32_t *buf_index, int64_t *cyc
   return FG_OK;
 }
 
-extern "C" int64_t fg_maxsum_launch_count(fg_maxsum_t h) { return h ? h->launches : -1; }
+extern "C" int64_t fg_maxsum_launch_count(fg_maxsum_t h) { return fg_launch_count(h); }
 
 extern "C" int fg_maxsum_kernel_plan(fg_maxsum_t h, int32_t *family, int32_t n_classes) {
   if (!h || !family || n_classes != (int32_t)h->classes.size()) return FG_ERR_ARG;
@@ -717,43 +677,20 @@ extern "C" int fg_halo_push(int32_t precision, const void *dev_r, const void *de
 // DSA
 // ---------------------------------------------------------------------------------------------
 extern "C" int fg_dsa_create(const fg_dsa_desc_t *desc, fg_dsa_t *out) {
-  if (!desc || !out) return FG_ERR_ARG;
-  *out = nullptr;
-  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
-  if (desc->precision != FG_F32 && desc->precision != FG_F64) return FG_ERR_ARG;
-  fg_dsa *h = new (std::nothrow) fg_dsa();
-  if (!h) return FG_ERR_ARG;
-  h->d = *desc;
-  h->classes.assign(desc->classes, desc->classes + desc->n_classes);
-  h->d.classes = h->classes.data();
-  *out = h;
-  for (auto &c : h->classes) {
-    int rc = check_class(c, h->err, sizeof(h->err));
-    if (rc != FG_OK) return rc;
-  }
-  if (fg_device_count() <= 0) {
-    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
-    return FG_ERR_CUDA;
-  }
+  int rc = fg_open(desc, out);
+  if (rc != FG_OK) return rc;
+  fg_dsa *h = *out;
+  if ((rc = fg_require_device(h)) != FG_OK) return rc;
   {  // experiment knob: L2 -> DRAM fetch granularity hint (32 | 64 | 128 bytes) for the sparse row reads
     const int g = fg_env_int("PYDCOP_B200_L2_FETCH", 0);
     if (g == 32 || g == 64 || g == 128) { cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)g); cudaGetLastError(); }
   }
-  // the class table is the one device allocation the library owns (a few hundred bytes)
-  size_t bytes = sizeof(fg_class_t) * (h->classes.empty() ? 1 : h->classes.size());
-  CUDA_TRY(h, cudaMalloc(&h->dev_classes, bytes));
-  if (!h->classes.empty())
-    CUDA_TRY(h, cudaMemcpy(h->dev_classes, h->classes.data(), sizeof(fg_class_t) * h->classes.size(), cudaMemcpyHostToDevice));
-  return FG_OK;
+  return fg_upload_classes(h);
 }
 
-extern "C" int fg_dsa_destroy(fg_dsa_t h) {
-  if (h && h->dev_classes) cudaFree(h->dev_classes);
-  delete h;
-  return FG_OK;
-}
+extern "C" int fg_dsa_destroy(fg_dsa_t h) { return fg_close(h); }
 
-extern "C" const char *fg_dsa_last_error(fg_dsa_t h) { return h ? h->err : g_static_err; }
+extern "C" const char *fg_dsa_last_error(fg_dsa_t h) { return fg_last_error(h); }
 
 static DsaSide dsa_side(const fg_dsa *h) {
   const fg_dsa_desc_t &d = h->d;
@@ -839,7 +776,7 @@ extern "C" int fg_dsa_current(fg_dsa_t h, int32_t *buf_index, int64_t *cycle) {
   return FG_OK;
 }
 
-extern "C" int64_t fg_dsa_launch_count(fg_dsa_t h) { return h ? h->launches : -1; }
+extern "C" int64_t fg_dsa_launch_count(fg_dsa_t h) { return fg_launch_count(h); }
 
 extern "C" int fg_dsa_shard_attach(fg_dsa_t h, const fg_halo_plan_t *plan) {
   if (!h) return FG_ERR_ARG;

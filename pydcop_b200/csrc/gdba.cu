@@ -1,23 +1,12 @@
 // GDBA for all variables at once: C-ABI entry points fg_gdba_* and their kernels
 // (csrc/gdba_kernels.cuh, which states the floating-point operand order).  Its own translation unit,
 // so the MaxSum / DSA / MGM / MGM-2 code is compiled exactly as before.
-#include <cstdio>
-#include <new>
-#include <vector>
-
-#include "common.cuh"
+#include "handle.cuh"
 #include "gdba_kernels.cuh"
 
-struct fg_gdba {
+struct fg_gdba : fg_handle_base {
   fg_gdba_desc_t d;
-  std::vector<fg_class_t> classes;
-  fg_class_t *dev_classes = nullptr;
-  int64_t cycle = 0;
-  int64_t launches = 0;
-  char err[512] = {0};
 };
-
-static char g_gdba_static_err[64] = "invalid handle";
 
 static inline unsigned gdba_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
@@ -28,34 +17,9 @@ static MgmSide gdba_side(const fg_gdba *h) {
 }
 
 extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
-  if (!desc || !out) return FG_ERR_ARG;
-  *out = nullptr;
-  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
-  if (desc->precision != FG_F32 && desc->precision != FG_F64) return FG_ERR_ARG;
-  fg_gdba *h = new (std::nothrow) fg_gdba();
-  if (!h) return FG_ERR_ARG;
-  h->d = *desc;
-  h->classes.assign(desc->classes, desc->classes + desc->n_classes);
-  h->d.classes = h->classes.data();
-  *out = h;
-  for (auto &c : h->classes) {
-    if (c.arity < 1 || c.arity > FG_MAX_ARITY) {
-      snprintf(h->err, sizeof(h->err), "class arity %d out of range", c.arity);
-      return FG_ERR_ARG;
-    }
-    int64_t ts = 1;
-    for (int i = 0; i < c.arity; ++i) {
-      if (c.dom[i] < 1 || c.dom[i] > FG_MAX_DOM) {
-        snprintf(h->err, sizeof(h->err), "domain size %d out of range", c.dom[i]);
-        return FG_ERR_ARG;
-      }
-      ts *= c.dom[i];
-    }
-    if (ts != c.table_size) {
-      snprintf(h->err, sizeof(h->err), "class size mismatch");
-      return FG_ERR_ARG;
-    }
-  }
+  int rc = fg_open(desc, out);
+  if (rc != FG_OK) return rc;
+  fg_gdba *h = *out;
   if (desc->modifier != FG_GDBA_MODIFIER_A && desc->modifier != FG_GDBA_MODIFIER_M) {
     snprintf(h->err, sizeof(h->err), "modifier %d is not one of A (0), M (1)", desc->modifier);
     return FG_ERR_ARG;
@@ -92,26 +56,13 @@ extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
     snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
     return FG_ERR_ARG;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    cudaGetLastError();
-    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
-    return FG_ERR_CUDA;
-  }
-  size_t bytes = sizeof(fg_class_t) * (h->classes.empty() ? 1 : h->classes.size());
-  CUDA_TRY(h, cudaMalloc(&h->dev_classes, bytes));
-  if (!h->classes.empty())
-    CUDA_TRY(h, cudaMemcpy(h->dev_classes, h->classes.data(), sizeof(fg_class_t) * h->classes.size(), cudaMemcpyHostToDevice));
-  return FG_OK;
+  if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  return fg_upload_classes(h);
 }
 
-extern "C" int fg_gdba_destroy(fg_gdba_t h) {
-  if (h && h->dev_classes) cudaFree(h->dev_classes);
-  delete h;
-  return FG_OK;
-}
+extern "C" int fg_gdba_destroy(fg_gdba_t h) { return fg_close(h); }
 
-extern "C" const char *fg_gdba_last_error(fg_gdba_t h) { return h ? h->err : g_gdba_static_err; }
+extern "C" const char *fg_gdba_last_error(fg_gdba_t h) { return fg_last_error(h); }
 
 extern "C" int fg_gdba_init(fg_gdba_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
@@ -127,8 +78,6 @@ extern "C" int fg_gdba_init(fg_gdba_t h, void *stream) {
   h->cycle = 0;
   return FG_OK;
 }
-
-static bool gdba_finished(const fg_gdba *h) { return h->d.stop_cycle && h->cycle + 1 >= h->d.stop_cycle; }
 
 template <typename T>
 static int gdba_cycle_t(fg_gdba *h, cudaStream_t st) {
@@ -155,21 +104,9 @@ static int gdba_cycle_t(fg_gdba *h, cudaStream_t st) {
 }
 
 extern "C" int fg_gdba_step(fg_gdba_t h, int32_t n_cycles, void *stream) {
-  if (!h) return FG_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  for (int i = 0; i < n_cycles; ++i) {
-    if (gdba_finished(h)) break;
-    int rc = h->d.precision == FG_F64 ? gdba_cycle_t<double>(h, st) : gdba_cycle_t<float>(h, st);
-    if (rc != FG_OK) return rc;
-  }
-  return FG_OK;
+  return fg_step(h, n_cycles, stream, gdba_cycle_t<float>, gdba_cycle_t<double>);
 }
 
-extern "C" int fg_gdba_current(fg_gdba_t h, int64_t *cycle, int32_t *finished) {
-  if (!h) return FG_ERR_ARG;
-  if (cycle) *cycle = h->cycle;
-  if (finished) *finished = gdba_finished(h) ? 1 : 0;
-  return FG_OK;
-}
+extern "C" int fg_gdba_current(fg_gdba_t h, int64_t *cycle, int32_t *finished) { return fg_current(h, cycle, finished); }
 
-extern "C" int64_t fg_gdba_launch_count(fg_gdba_t h) { return h ? h->launches : -1; }
+extern "C" int64_t fg_gdba_launch_count(fg_gdba_t h) { return fg_launch_count(h); }

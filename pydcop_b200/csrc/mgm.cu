@@ -7,25 +7,14 @@
 //   relation value of x  = ((f1(x) + f2(x)) + f3(x)) ...   in node.constraints order (mgm.py:443)
 //   evaluation           = best + own cost(CURRENT value) + neighbours' costs       (:446-452)
 //   gain                 = current_cost - evaluation                                (:381)
-#include <cstdio>
-#include <new>
-#include <vector>
-
-#include "common.cuh"
+#include "handle.cuh"
 #include "mgm_kernels.cuh"
 #include "mgm_fast_kernels.cuh"
 #include "mgm_cached_kernels.cuh"
 
-struct fg_mgm {
+struct fg_mgm : fg_handle_base {
   fg_mgm_desc_t d;
-  std::vector<fg_class_t> classes;
-  fg_class_t *dev_classes = nullptr;
-  int64_t cycle = 0;
-  int64_t launches = 0;
-  char err[512] = {0};
 };
-
-static char g_mgm_static_err[64] = "invalid handle";
 
 static inline unsigned mgm_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
@@ -36,59 +25,21 @@ static MgmSide mgm_side(const fg_mgm *h) {
 }
 
 extern "C" int fg_mgm_create(const fg_mgm_desc_t *desc, fg_mgm_t *out) {
-  if (!desc || !out) return FG_ERR_ARG;
-  *out = nullptr;
-  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
-  if (desc->precision != FG_F32 && desc->precision != FG_F64) return FG_ERR_ARG;
-  fg_mgm *h = new (std::nothrow) fg_mgm();
-  if (!h) return FG_ERR_ARG;
-  h->d = *desc;
-  h->classes.assign(desc->classes, desc->classes + desc->n_classes);
-  h->d.classes = h->classes.data();
-  *out = h;
-  for (auto &c : h->classes) {
-    if (c.arity < 1 || c.arity > FG_MAX_ARITY) {
-      snprintf(h->err, sizeof(h->err), "class arity %d out of range", c.arity);
-      return FG_ERR_ARG;
-    }
-    int64_t ts = 1;
-    for (int i = 0; i < c.arity; ++i) {
-      if (c.dom[i] < 1 || c.dom[i] > FG_MAX_DOM) {
-        snprintf(h->err, sizeof(h->err), "domain size %d out of range", c.dom[i]);
-        return FG_ERR_ARG;
-      }
-      ts *= c.dom[i];
-    }
-    if (ts != c.table_size) {
-      snprintf(h->err, sizeof(h->err), "class size mismatch");
-      return FG_ERR_ARG;
-    }
-  }
+  int rc = fg_open(desc, out);
+  if (rc != FG_OK) return rc;
+  fg_mgm *h = *out;
   if (desc->n_vars > 0 && (!desc->dev_nbr_ptr || !desc->dev_value || !desc->dev_cost || !desc->dev_has_cost ||
                            !desc->dev_gain || !desc->dev_new_value || !desc->dev_var_rank || !desc->dev_var_id)) {
     snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
     return FG_ERR_ARG;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    cudaGetLastError();
-    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
-    return FG_ERR_CUDA;
-  }
-  size_t bytes = sizeof(fg_class_t) * (h->classes.empty() ? 1 : h->classes.size());
-  CUDA_TRY(h, cudaMalloc(&h->dev_classes, bytes));
-  if (!h->classes.empty())
-    CUDA_TRY(h, cudaMemcpy(h->dev_classes, h->classes.data(), sizeof(fg_class_t) * h->classes.size(), cudaMemcpyHostToDevice));
-  return FG_OK;
+  if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  return fg_upload_classes(h);
 }
 
-extern "C" int fg_mgm_destroy(fg_mgm_t h) {
-  if (h && h->dev_classes) cudaFree(h->dev_classes);
-  delete h;
-  return FG_OK;
-}
+extern "C" int fg_mgm_destroy(fg_mgm_t h) { return fg_close(h); }
 
-extern "C" const char *fg_mgm_last_error(fg_mgm_t h) { return h ? h->err : g_mgm_static_err; }
+extern "C" const char *fg_mgm_last_error(fg_mgm_t h) { return fg_last_error(h); }
 
 extern "C" int fg_mgm_init(fg_mgm_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
@@ -105,8 +56,6 @@ extern "C" int fg_mgm_init(fg_mgm_t h, void *stream) {
   h->cycle = 0;
   return FG_OK;
 }
-
-static bool mgm_finished(const fg_mgm *h) { return h->d.stop_cycle && h->cycle + 1 >= h->d.stop_cycle; }
 
 template <typename T, int D, int U>
 static void mgm_gain_fast_launch(fg_mgm *h, cudaStream_t st) {
@@ -171,21 +120,9 @@ static int mgm_cycle_t(fg_mgm *h, cudaStream_t st) {
 }
 
 extern "C" int fg_mgm_step(fg_mgm_t h, int32_t n_cycles, void *stream) {
-  if (!h) return FG_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  for (int i = 0; i < n_cycles; ++i) {
-    if (mgm_finished(h)) break;
-    int rc = h->d.precision == FG_F64 ? mgm_cycle_t<double>(h, st) : mgm_cycle_t<float>(h, st);
-    if (rc != FG_OK) return rc;
-  }
-  return FG_OK;
+  return fg_step(h, n_cycles, stream, mgm_cycle_t<float>, mgm_cycle_t<double>);
 }
 
-extern "C" int fg_mgm_current(fg_mgm_t h, int64_t *cycle, int32_t *finished) {
-  if (!h) return FG_ERR_ARG;
-  if (cycle) *cycle = h->cycle;
-  if (finished) *finished = mgm_finished(h) ? 1 : 0;
-  return FG_OK;
-}
+extern "C" int fg_mgm_current(fg_mgm_t h, int64_t *cycle, int32_t *finished) { return fg_current(h, cycle, finished); }
 
-extern "C" int64_t fg_mgm_launch_count(fg_mgm_t h) { return h ? h->launches : -1; }
+extern "C" int64_t fg_mgm_launch_count(fg_mgm_t h) { return fg_launch_count(h); }

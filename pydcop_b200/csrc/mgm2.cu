@@ -8,23 +8,12 @@
 //   offer gain            = current_cost - cost                                   (:553)
 //   global gain           = (current_cost - cost over the other constraints) + offer gain (:593)
 //   cost after a move     = current_cost - potential_gain                         (:941, :986)
-#include <cstdio>
-#include <new>
-#include <vector>
-
-#include "common.cuh"
+#include "handle.cuh"
 #include "mgm2_kernels.cuh"
 
-struct fg_mgm2 {
+struct fg_mgm2 : fg_handle_base {
   fg_mgm2_desc_t d;
-  std::vector<fg_class_t> classes;
-  fg_class_t *dev_classes = nullptr;
-  int64_t cycle = 0;
-  int64_t launches = 0;
-  char err[512] = {0};
 };
-
-static char g_mgm2_static_err[64] = "invalid handle";
 
 static inline unsigned mgm2_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
@@ -35,34 +24,9 @@ static MgmSide mgm2_side(const fg_mgm2 *h) {
 }
 
 extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
-  if (!desc || !out) return FG_ERR_ARG;
-  *out = nullptr;
-  if (desc->abi_version != FG_ABI_VERSION) return FG_ERR_ARG;
-  if (desc->precision != FG_F32 && desc->precision != FG_F64) return FG_ERR_ARG;
-  fg_mgm2 *h = new (std::nothrow) fg_mgm2();
-  if (!h) return FG_ERR_ARG;
-  h->d = *desc;
-  h->classes.assign(desc->classes, desc->classes + desc->n_classes);
-  h->d.classes = h->classes.data();
-  *out = h;
-  for (auto &c : h->classes) {
-    if (c.arity < 1 || c.arity > FG_MAX_ARITY) {
-      snprintf(h->err, sizeof(h->err), "class arity %d out of range", c.arity);
-      return FG_ERR_ARG;
-    }
-    int64_t ts = 1;
-    for (int i = 0; i < c.arity; ++i) {
-      if (c.dom[i] < 1 || c.dom[i] > FG_MAX_DOM) {
-        snprintf(h->err, sizeof(h->err), "domain size %d out of range", c.dom[i]);
-        return FG_ERR_ARG;
-      }
-      ts *= c.dom[i];
-    }
-    if (ts != c.table_size) {
-      snprintf(h->err, sizeof(h->err), "class size mismatch");
-      return FG_ERR_ARG;
-    }
-  }
+  int rc = fg_open(desc, out);
+  if (rc != FG_OK) return rc;
+  fg_mgm2 *h = *out;
   if (desc->favor < FG_MGM2_FAVOR_UNILATERAL || desc->favor > FG_MGM2_FAVOR_COORDINATED) {
     snprintf(h->err, sizeof(h->err), "favor %d is not one of unilateral (0), no (1), coordinated (2)", desc->favor);
     return FG_ERR_ARG;
@@ -88,26 +52,13 @@ extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
     snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
     return FG_ERR_ARG;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    cudaGetLastError();
-    snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
-    return FG_ERR_CUDA;
-  }
-  size_t bytes = sizeof(fg_class_t) * (h->classes.empty() ? 1 : h->classes.size());
-  CUDA_TRY(h, cudaMalloc(&h->dev_classes, bytes));
-  if (!h->classes.empty())
-    CUDA_TRY(h, cudaMemcpy(h->dev_classes, h->classes.data(), sizeof(fg_class_t) * h->classes.size(), cudaMemcpyHostToDevice));
-  return FG_OK;
+  if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  return fg_upload_classes(h);
 }
 
-extern "C" int fg_mgm2_destroy(fg_mgm2_t h) {
-  if (h && h->dev_classes) cudaFree(h->dev_classes);
-  delete h;
-  return FG_OK;
-}
+extern "C" int fg_mgm2_destroy(fg_mgm2_t h) { return fg_close(h); }
 
-extern "C" const char *fg_mgm2_last_error(fg_mgm2_t h) { return h ? h->err : g_mgm2_static_err; }
+extern "C" const char *fg_mgm2_last_error(fg_mgm2_t h) { return fg_last_error(h); }
 
 template <typename T>
 static void mgm2_init_t(fg_mgm2 *h, cudaStream_t st) {
@@ -130,8 +81,6 @@ extern "C" int fg_mgm2_init(fg_mgm2_t h, void *stream) {
   h->cycle = 0;
   return FG_OK;
 }
-
-static bool mgm2_finished(const fg_mgm2 *h) { return h->d.stop_cycle && h->cycle + 1 >= h->d.stop_cycle; }
 
 template <typename T>
 static int mgm2_cycle_t(fg_mgm2 *h, cudaStream_t st) {
@@ -164,21 +113,9 @@ static int mgm2_cycle_t(fg_mgm2 *h, cudaStream_t st) {
 }
 
 extern "C" int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream) {
-  if (!h) return FG_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  for (int i = 0; i < n_cycles; ++i) {
-    if (mgm2_finished(h)) break;
-    int rc = h->d.precision == FG_F64 ? mgm2_cycle_t<double>(h, st) : mgm2_cycle_t<float>(h, st);
-    if (rc != FG_OK) return rc;
-  }
-  return FG_OK;
+  return fg_step(h, n_cycles, stream, mgm2_cycle_t<float>, mgm2_cycle_t<double>);
 }
 
-extern "C" int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished) {
-  if (!h) return FG_ERR_ARG;
-  if (cycle) *cycle = h->cycle;
-  if (finished) *finished = mgm2_finished(h) ? 1 : 0;
-  return FG_OK;
-}
+extern "C" int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished) { return fg_current(h, cycle, finished); }
 
-extern "C" int64_t fg_mgm2_launch_count(fg_mgm2_t h) { return h ? h->launches : -1; }
+extern "C" int64_t fg_mgm2_launch_count(fg_mgm2_t h) { return fg_launch_count(h); }

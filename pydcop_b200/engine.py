@@ -6,6 +6,7 @@ kernels); torch only owns the buffers.  There is no CPU path: constructing an en
 CUDA device raises EngineError.
 """
 import ctypes as C
+import functools
 import os
 from typing import Optional
 
@@ -63,7 +64,120 @@ def _ptr(t: Optional[torch.Tensor]):
         else C.c_void_p(0)
 
 
+def _addr(a):
+    """Address of a torch tensor (device) or numpy array (host); NULL for None or an empty one."""
+    if isinstance(a, np.ndarray):
+        return C.c_void_p(a.ctypes.data if a.size else 0)
+    return _ptr(a)
+
+
+def fill_desc(d, arrays, scalars=(), prefix="dev_"):
+    """d.<prefix><name> = the address of every array of `arrays` (name -> tensor, numpy array or None; a list of two
+    fills a double-buffer field), then d.<name> = value for every scalar field.  An unknown field raises."""
+    for name in [prefix + k for k in arrays] + list(dict(scalars)):
+        if not hasattr(type(d), name):
+            raise AttributeError(f"{type(d).__name__} has no field {name}")
+    for name, a in arrays.items():
+        if isinstance(a, list):
+            for b, x in enumerate(a):
+                getattr(d, prefix + name)[b] = _addr(x)
+        else:
+            setattr(d, prefix + name, _addr(a))
+    for name, v in dict(scalars).items():
+        setattr(d, name, v)
+    return d
+
+
+def fill_header(d, precision, layout, classes):
+    """The fields every descriptor with a class table starts with; `classes` from _class_array(layout)."""
+    L = layout
+    d.abi_version, d.precision = _cabi.FG_ABI_VERSION, PRECISIONS[precision][0]
+    d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
+    d.classes = C.cast(classes, C.POINTER(FgClass))
+    return d
+
+
+def host_state(state):
+    """The state of a host-array plan as numpy arrays (what the engines allocate on the device)."""
+    return {k: np.full(max(n, 1), 0 if fill is None else fill, dtype=dt) for k, (n, dt, fill) in state.items()}
+
+
+_TORCH_DTYPES = {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64,
+                 np.dtype(np.int32): torch.int32, np.dtype(np.int64): torch.int64, np.dtype(np.uint8): torch.uint8}
+
+
 class _EngineBase:
+    """Lifecycle of an engine's handle: FAMILY names its fg_<FAMILY>_* functions.  Subclasses build the descriptor,
+    call _create and supply _assignment (the current value of every variable, internal order, on the device)."""
+    FAMILY = None
+
+    def _open(self, layout, device, precision):
+        self.lib = _cabi.load()
+        self.device = _require_cuda(device)
+        self.layout = layout
+        self.precision = precision
+        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        return tdt
+
+    def _fn(self, name):
+        return getattr(self.lib, f"fg_{self.FAMILY}_{name}")
+
+    def _create(self, d):
+        self._desc, self._h = d, C.c_void_p()
+        self._check(self._fn("create")(C.byref(d), C.byref(self._h)), f"fg_{self.FAMILY}_create")
+
+    def _upload(self, inputs, state):
+        """Every input of a host-array plan through _dev, in order (None stays None), then the state allocated on the
+        device without a host copy (fill None: uninitialised).  Returns name -> tensor, or a list of two."""
+        out = {}
+        with torch.cuda.device(self.device):
+            for k, a in inputs.items():
+                if isinstance(a, list):
+                    out[k] = [self._dev(x, _TORCH_DTYPES[x.dtype]) for x in a]
+                else:
+                    out[k] = None if a is None else self._dev(a, _TORCH_DTYPES[a.dtype])
+            for k, (n, dt, fill) in state.items():
+                dt = _TORCH_DTYPES[np.dtype(dt)]
+                out[k] = (torch.empty(max(n, 1), dtype=dt, device=self.device) if fill is None
+                          else torch.full((max(n, 1),), fill, dtype=dt, device=self.device))
+        return out
+
+    def _last_error(self):
+        return (self._fn("last_error")(self._h) or b"").decode()
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self._fn("destroy")(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def init(self):
+        with torch.cuda.device(self.device):
+            self._check(self._fn("init")(self._h, self._stream()), f"fg_{self.FAMILY}_init")
+        return self
+
+    def step(self, n_cycles=1):
+        with torch.cuda.device(self.device):
+            self._check(self._fn("step")(self._h, int(n_cycles), self._stream()), f"fg_{self.FAMILY}_step")
+        return self
+
+    @property
+    def launch_count(self):
+        return int(self._fn("launch_count")(self._h))
+
+    def solution_cost(self, infinity=float("inf"), unary=None):
+        """(cost, violations) of the current assignment, reduced on the device (pydcop/dcop/dcop.py:319-367;
+        `infinity` as `pydcop solve -i`).  `unary`: the variables' own costs in canonical order (MaxSum: WITHOUT its
+        noise); default: variable costs are not added."""
+        with torch.cuda.device(self.device):
+            out = self._solution_cost(self._assignment(), infinity, unary).cpu().numpy()
+        return float(out[0]), int(out[1])
+
     def _dev(self, a, dtype):
         a = np.ascontiguousarray(a)
         if not a.flags.writeable:      # e.g. a read-only memory map of the binary container
@@ -114,7 +228,32 @@ class _EngineBase:
             return self._cost_out
 
 
-class MaxSumEngine(_EngineBase):
+class _CycleEngine(_EngineBase):
+    """MaxSum and DSA: a cycle is computed into the other message / value buffer, then committed;
+    fg_<family>_current reports (current buffer, cycle)."""
+
+    def cycle_compute(self):
+        with torch.cuda.device(self.device):
+            self._check(self._fn("cycle_compute")(self._h, self._stream()), f"fg_{self.FAMILY}_cycle_compute")
+
+    def cycle_commit(self):
+        self._check(self._fn("cycle_commit")(self._h), f"fg_{self.FAMILY}_cycle_commit")
+
+    def _current(self):
+        b, c = C.c_int32(), C.c_int64()
+        self._fn("current")(self._h, C.byref(b), C.byref(c))
+        return b.value, c.value
+
+    @property
+    def cur(self):
+        return self._current()[0]
+
+    @property
+    def cycle(self):
+        return self._current()[1]
+
+
+class MaxSumEngine(_CycleEngine):
     """All-edges-at-once synchronous MaxSum.
 
     Parameters mirror the reference's algo_params (pydcop/algorithms/maxsum.py:212-220); `noise`
@@ -122,15 +261,13 @@ class MaxSumEngine(_EngineBase):
     State after `init()` is the reference's cycle 0 (on_start); each `step()` cycle is one
     synchronous round of every factor's and every variable's on_new_cycle.
     """
+    FAMILY = "maxsum"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
                  damping=0.5, damping_nodes="both", stability=0.1, start_messages="leafs",
                  record_sent=True):
-        self.lib = _cabi.load()
-        self.device = _require_cuda(device)
-        self.layout = L = layout
-        self.precision = precision
-        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        L = layout
+        tdt = self._open(layout, device, precision)
         if damping_nodes not in ("vars", "factors", "both", "none"):
             raise ValueError(f"invalid damping_nodes {damping_nodes!r}")
         if start_messages not in _cabi.START_MESSAGES:
@@ -163,87 +300,22 @@ class MaxSumEngine(_EngineBase):
             self.value = z(L.n_vars, torch.int32)
             self.value_cost = z(L.n_vars, tdt)
         self._classes = _class_array(L)
-        d = FgMaxSumDesc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
-        d.n_vars, d.n_factors, d.n_edges = L.n_vars, L.n_factors, L.n_edges
-        d.n_classes, d.n_msg_r, d.n_msg_q = len(L.classes), L.n_msg, L.n_msg_q
+        d = fill_header(FgMaxSumDesc(), precision, L, self._classes)
+        d.n_msg_r, d.n_msg_q = L.n_msg, L.n_msg_q
         d.uniform_dom, d.max_degree = L.uniform_dom, L.max_degree
-        d.classes = C.cast(self._classes, C.POINTER(FgClass))
         self._varclasses = _varclass_array(L)
         d.n_varclasses = len(L.var_classes)
         d.varclasses = C.cast(self._varclasses, C.POINTER(FgVarClass))
-        d.dev_tables, d.dev_unary = _ptr(self.tables), _ptr(self.unary)
-        d.dev_dom_size, d.dev_unary_off = _ptr(self.dom_size), _ptr(self.unary_off)
-        d.dev_var_ptr, d.dev_var_qbase = _ptr(self.var_ptr), _ptr(self.var_qbase)
-        d.dev_slot_roff, d.dev_edge_qoff = _ptr(self.slot_roff), _ptr(self.edge_qoff)
-        d.dev_slot_roff32, d.dev_edge_qoff32 = _ptr(self.slot_roff32), _ptr(self.edge_qoff32)
-        d.dev_slot_edge, d.dev_slot_var = _ptr(self.slot_edge), _ptr(self.slot_var)
-        d.dev_init_value = _ptr(self.init_value)
-        for b in range(2):
-            d.dev_q[b], d.dev_r[b] = self.q[b].data_ptr(), self.r[b].data_ptr()
-        d.dev_q_valid, d.dev_r_valid = _ptr(self.q_valid), _ptr(self.r_valid)
-        d.dev_q_cnt, d.dev_r_cnt = _ptr(self.q_cnt), _ptr(self.r_cnt)
-        d.dev_q_sent, d.dev_r_sent = _ptr(self.q_sent), _ptr(self.r_sent)
-        d.dev_value, d.dev_value_cost = _ptr(self.value), _ptr(self.value_cost)
+        fill_desc(d, {k: getattr(self, k) for k in (
+            "tables", "unary", "dom_size", "unary_off", "var_ptr", "var_qbase", "slot_roff", "edge_qoff", "slot_roff32",
+            "edge_qoff32", "slot_edge", "slot_var", "init_value", "q", "r", "q_valid", "r_valid", "q_cnt", "r_cnt",
+            "q_sent", "r_sent", "value", "value_cost")})
         d.mode_max = int(mode == "max")
         d.damp_vars = int(damping_nodes in ("vars", "both"))
         d.damp_factors = int(damping_nodes in ("factors", "both"))
         d.start_messages = _cabi.START_MESSAGES[start_messages]
         d.damping, d.stability = float(damping), float(stability)
-        self._desc = d
-        self._h = C.c_void_p()
-        rc = self.lib.fg_maxsum_create(C.byref(d), C.byref(self._h))
-        self._check(rc, "fg_maxsum_create")
-
-    def _last_error(self):
-        return (self.lib.fg_maxsum_last_error(self._h) or b"").decode()
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.fg_maxsum_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    # -- driving -----------------------------------------------------------------------------
-    def init(self):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_maxsum_init(self._h, self._stream()), "fg_maxsum_init")
-        return self
-
-    def step(self, n_cycles=1):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_maxsum_step(self._h, int(n_cycles), self._stream()),
-                        "fg_maxsum_step")
-        return self
-
-    def cycle_compute(self):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_maxsum_cycle_compute(self._h, self._stream()),
-                        "fg_maxsum_cycle_compute")
-
-    def cycle_commit(self):
-        self._check(self.lib.fg_maxsum_cycle_commit(self._h), "fg_maxsum_cycle_commit")
-
-    @property
-    def cur(self):
-        b, c = C.c_int32(), C.c_int64()
-        self.lib.fg_maxsum_current(self._h, C.byref(b), C.byref(c))
-        return b.value
-
-    @property
-    def cycle(self):
-        b, c = C.c_int32(), C.c_int64()
-        self.lib.fg_maxsum_current(self._h, C.byref(b), C.byref(c))
-        return c.value
-
-    @property
-    def launch_count(self):
-        return int(self.lib.fg_maxsum_launch_count(self._h))
+        self._create(d)
 
     KERNEL_FAMILIES = {-1: "ghost", 0: "generic", 1: "pipe", 2: "warp", 3: "tiled_rt"}
 
@@ -288,12 +360,8 @@ class MaxSumEngine(_EngineBase):
             out["r_sent"] = L.edges_to_canonical(self.r_sent.cpu().numpy()[:L.n_edges])
         return out
 
-    def solution_cost(self, infinity=float("inf"), unary=None):
-        """(cost, violations) of the currently selected assignment, reduced on the device
-        (pydcop/dcop/dcop.py:319-367; `infinity` as `pydcop solve -i`).  `unary`: the variables' own
-        costs in canonical order WITHOUT MaxSum's noise (default: variable costs are not added)."""
-        out = self._solution_cost(self.value, infinity, unary).cpu().numpy()
-        return float(out[0]), int(out[1])
+    def _assignment(self):
+        return self.value
 
     def values(self):
         """(value index, reported cost) per variable, in the caller's canonical variable order."""
@@ -348,8 +416,9 @@ def dsa_fast_arrays(layout: FactorGraphLayout, tables: torch.Tensor, mode="min")
             opt[torch.from_numpy(f).to(dev)].contiguous(), D)
 
 
-class DsaEngine(_EngineBase):
+class DsaEngine(_CycleEngine):
     """All-variables-at-once DSA-A/B/C (pydcop/algorithms/dsa.py:130-135 parameters)."""
+    FAMILY = "dsa"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
                  probability=0.7, p_mode="fixed", variant="B", stop_cycle=0, seed=0,
@@ -359,11 +428,8 @@ class DsaEngine(_EngineBase):
         var_global_id / frozen (canonical order) serve the multi-GPU partition
         (pydcop_b200/multigpu_dsa.py): the Philox counter of each variable when the layout is a
         shard of a larger problem, and the ghost variables whose value is only copied through."""
-        self.lib = _cabi.load()
-        self.device = _require_cuda(device)
-        self.layout = L = layout
-        self.precision = precision
-        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        L = layout
+        tdt = self._open(layout, device, precision)
         if variant not in _cabi.DSA_VARIANTS:
             raise ValueError(f"invalid variant {variant!r}")
         if p_mode not in ("fixed", "arity"):
@@ -424,80 +490,18 @@ class DsaEngine(_EngineBase):
                 self.row_cache = torch.zeros(max(L.n_edges * fast_dom, 4), dtype=tdt, device=self.device)
                 self.slot_last = torch.full((max(L.n_edges, 1),), 255, dtype=torch.uint8, device=self.device)
         self._classes = _class_array(L)
-        d = FgDsaDesc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
-        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
-        d.classes = C.cast(self._classes, C.POINTER(FgClass))
-        d.dev_tables, d.dev_dom_size = _ptr(self.tables), _ptr(self.dom_size)
-        d.dev_var_id = _ptr(self.var_id)
-        d.dev_edge_var, d.dev_edge_class = _ptr(self.edge_var), _ptr(self.edge_class)
-        d.dev_var_ptr, d.dev_slot_edge = _ptr(self.var_ptr), _ptr(self.slot_edge)
-        d.dev_has_nbr, d.dev_prob, d.dev_con_opt = _ptr(self.has_nbr), _ptr(self.prob), _ptr(self.con_opt)
-        d.dev_value[0], d.dev_value[1] = self.value[0].data_ptr(), self.value[1].data_ptr()
-        d.dev_value_cost = _ptr(self.value_cost)
-        d.dev_tables_or, d.dev_slot_nbr = _ptr(self.tables_or), _ptr(self.slot_nbr)
-        d.dev_slot_tab, d.dev_slot_opt = _ptr(self.slot_tab), _ptr(self.slot_opt)
+        d = fill_header(FgDsaDesc(), precision, L, self._classes)
+        fill_desc(d, {k: getattr(self, k) for k in (
+            "tables", "dom_size", "var_id", "edge_var", "edge_class", "var_ptr", "slot_edge", "has_nbr", "prob",
+            "con_opt", "value", "value_cost", "tables_or", "slot_nbr", "slot_tab", "slot_opt", "var_cost", "unary_off",
+            "row_cache", "slot_last")})
         d.fast_dom = fast_dom
         d.mode_max, d.variant = int(mode == "max"), _cabi.DSA_VARIANTS[variant]
         d.stop_cycle, d.seed = int(stop_cycle), int(seed) & (2 ** 64 - 1)
-        d.dev_var_cost, d.dev_unary_off = _ptr(self.var_cost), _ptr(self.unary_off)
-        d.dev_row_cache, d.dev_slot_last = _ptr(self.row_cache), _ptr(self.slot_last)
-        self._desc = d
-        self._h = C.c_void_p()
-        self._check(self.lib.fg_dsa_create(C.byref(d), C.byref(self._h)), "fg_dsa_create")
+        self._create(d)
 
-    def _last_error(self):
-        return (self.lib.fg_dsa_last_error(self._h) or b"").decode()
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.fg_dsa_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def init(self):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_dsa_init(self._h, self._stream()), "fg_dsa_init")
-        return self
-
-    def step(self, n_cycles=1):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_dsa_step(self._h, int(n_cycles), self._stream()), "fg_dsa_step")
-        return self
-
-    def cycle_compute(self):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_dsa_cycle_compute(self._h, self._stream()), "fg_dsa_cycle_compute")
-
-    def cycle_commit(self):
-        self._check(self.lib.fg_dsa_cycle_commit(self._h), "fg_dsa_cycle_commit")
-
-    def _current(self):
-        b, c = C.c_int32(), C.c_int64()
-        self.lib.fg_dsa_current(self._h, C.byref(b), C.byref(c))
-        return b.value, c.value
-
-    @property
-    def cur(self):
-        return self._current()[0]
-
-    @property
-    def cycle(self):
-        return self._current()[1]
-
-    @property
-    def launch_count(self):
-        return int(self.lib.fg_dsa_launch_count(self._h))
-
-    def solution_cost(self, infinity=float("inf"), unary=None):
-        """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
-        out = self._solution_cost(self.value[self.cur], infinity, unary).cpu().numpy()
-        return float(out[0]), int(out[1])
+    def _assignment(self):
+        return self.value[self.cur]
 
     def values(self):
         """Current value index per variable, canonical variable order."""
@@ -567,118 +571,48 @@ def mgm_host_arrays(layout: FactorGraphLayout, mode="min", var_rank=None, isolat
                 value0=value0, cost0=cost0)
 
 
-class MgmEngine(_EngineBase):
-    """All-variables-at-once MGM (pydcop/algorithms/mgm.py; parameters :78-81).
+def _per_var(layout, a, dtype):
+    """A per-variable input: `a` in `dtype`, or one zero without variables."""
+    return np.ascontiguousarray(a, dtype) if layout.n_vars else np.zeros(1, dtype)
 
-    var_rank       canonical order: position of each variable's NAME in sorted order, the
-                   lexicographic tie break of mgm.py:574-583 (default: the canonical index)
-    isolated_value canonical order: value index of the variables without neighbours
-                   (optimal_cost_value over the real domain values, relations.py:1641-1669);
-                   default: argopt of the own cost with ties broken on the value index
-    `break_mode` is accepted for the reference's signature; its 'random' branch is dead code in
-    the reference (mgm.py:541 compares with the `random` module) and both settings act as 'lexic'.
-    """
 
-    def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
-                 stop_cycle=0, seed=0, break_mode="lexic", var_rank=None, isolated_value=None):
-        self.lib = _cabi.load()
-        self.device = _require_cuda(device)
-        self.layout = L = layout
-        self.precision = precision
-        prec, tdt, self.np_dtype = PRECISIONS[precision]
-        if break_mode not in ("lexic", "random"):
-            raise ValueError(f"invalid break_mode {break_mode!r}")
-        if mode not in ("min", "max"):
-            raise ValueError(f"invalid mode {mode!r}")
-        h = mgm_host_arrays(L, mode, var_rank, isolated_value)
-        nbr_ptr, nbr_idx, has_nbr, rank = h["nbr_ptr"], h["nbr_idx"], h["has_nbr"], h["var_rank"]
-        value0, cost0 = h["value0"], h["cost0"]
-        self.has_nbr_host = has_nbr
-        with torch.cuda.device(self.device):
-            self.tables = self._dev(L.tables, tdt)
-            self.unary = self._dev(L.unary, tdt)
-            self.unary_off = self._dev(L.unary_off, torch.int64)
-            self.dom_size = self._dev(L.dom_size, torch.int32)
-            self.var_id = self._dev(L.var_order, torch.int32)
-            self.var_rank = self._dev(rank, torch.int32)
-            self.edge_var = self._dev(L.edge_var, torch.int32)
-            self.edge_class = self._dev(L.edge_class, torch.int32)
-            self.var_ptr = self._dev(L.var_ptr, torch.int32)
-            self.slot_edge = self._dev(L.slot_edge, torch.int32)
-            self.nbr_ptr = self._dev(nbr_ptr, torch.int32)
-            self.nbr_idx = self._dev(nbr_idx, torch.int32)
-            self.init_value = self._dev(L.init_value, torch.int32)
-            n = max(L.n_vars, 1)
-            self.value = self._dev(np.resize(value0, n) if L.n_vars else np.zeros(1, np.int32), torch.int32)
-            self.cost = self._dev(np.resize(cost0, n) if L.n_vars else np.zeros(1), tdt)
-            self.has_cost = self._dev((~np.resize(has_nbr, n)).astype(np.uint8) if L.n_vars
-                                      else np.zeros(1, np.uint8), torch.uint8)
-            self.gain = torch.zeros(n, dtype=tdt, device=self.device)
-            self.new_value = torch.zeros(n, dtype=torch.int32, device=self.device)
-        self._classes = _class_array(L)
-        d = FgMgmDesc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
-        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
-        d.classes = C.cast(self._classes, C.POINTER(FgClass))
-        d.dev_tables, d.dev_unary, d.dev_unary_off = _ptr(self.tables), _ptr(self.unary), _ptr(self.unary_off)
-        d.dev_dom_size, d.dev_var_id, d.dev_var_rank = _ptr(self.dom_size), _ptr(self.var_id), _ptr(self.var_rank)
-        d.dev_edge_var, d.dev_edge_class = _ptr(self.edge_var), _ptr(self.edge_class)
-        d.dev_var_ptr, d.dev_slot_edge = _ptr(self.var_ptr), _ptr(self.slot_edge)
-        d.dev_nbr_ptr, d.dev_nbr_idx = _ptr(self.nbr_ptr), _ptr(self.nbr_idx)
-        d.dev_init_value = _ptr(self.init_value)
-        d.dev_value, d.dev_cost, d.dev_has_cost = _ptr(self.value), _ptr(self.cost), _ptr(self.has_cost)
-        d.dev_gain, d.dev_new_value = _ptr(self.gain), _ptr(self.new_value)
-        d.mode_max, d.stop_cycle, d.seed = int(mode == "max"), int(stop_cycle), int(seed) & (2 ** 64 - 1)
-        # the fast value-phase kernel on the DSA fast-path arrays (binary constraints over one domain size
-        # in {4, 8, 10, 16, 20}), 2 incidences per trip by default.  PYDCOP_B200_MGM_FAST=0|2|4
-        self.fast_chunk = 0
-        chunk = int(os.environ.get("PYDCOP_B200_MGM_FAST", "2") or 0)
-        if chunk in (2, 4):
-            with torch.cuda.device(self.device):
-                fast = dsa_fast_arrays(L, self.tables, mode)
-            if fast is not None and fast[4] in (4, 8, 10, 16, 20):
-                self.tables_or, self.slot_tab, self.slot_nbr, _, fast_dom = fast
-                d.dev_tables_or, d.dev_slot_nbr, d.dev_slot_tab = (_ptr(self.tables_or), _ptr(self.slot_nbr),
-                                                                   _ptr(self.slot_tab))
-                d.fast_dom, d.fast_chunk = fast_dom, chunk
-                self.fast_chunk = chunk
-                self.row_cache = self.slot_last = None
-                if os.environ.get("PYDCOP_B200_MGM_CACHE", "1") != "0":   # active-row array (csrc/mgm_cached_kernels.cuh)
-                    with torch.cuda.device(self.device):
-                        self.row_cache = torch.zeros(max(L.n_edges * fast_dom, 4), dtype=tdt, device=self.device)
-                        self.slot_last = torch.full((max(L.n_edges, 1),), 255, dtype=torch.uint8, device=self.device)
-                    d.dev_row_cache, d.dev_slot_last = _ptr(self.row_cache), _ptr(self.slot_last)
-        self._desc = d
-        self._h = C.c_void_p()
-        self._check(self.lib.fg_mgm_create(C.byref(d), C.byref(self._h)), "fg_mgm_create")
+def _neighbourhood_inputs(layout, dt, h):
+    """The constraint tables and the neighbourhood arrays MGM, MGM-2 and GDBA all upload (h: mgm_host_arrays)."""
+    L = layout
+    i32 = lambda a: np.ascontiguousarray(a, np.int32)  # noqa: E731
+    return dict(tables=np.ascontiguousarray(L.tables, dt), dom_size=i32(L.dom_size), var_id=i32(L.var_order),
+                var_rank=i32(h["var_rank"]), edge_var=i32(L.edge_var), edge_class=i32(L.edge_class),
+                var_ptr=i32(L.var_ptr), slot_edge=i32(L.slot_edge), nbr_ptr=i32(h["nbr_ptr"]),
+                nbr_idx=i32(h["nbr_idx"]), init_value=i32(L.init_value))
 
-    def _last_error(self):
-        return (self.lib.fg_mgm_last_error(self._h) or b"").decode()
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.fg_mgm_destroy(self._h)
-            self._h = C.c_void_p()
+def _seed(seed):
+    return int(seed) & (2 ** 64 - 1)
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
-    def init(self):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_mgm_init(self._h, self._stream()), "fg_mgm_init")
-        return self
+def mgm_plan(layout: FactorGraphLayout, precision="f32", mode="min", stop_cycle=0, seed=0, var_rank=None,
+             isolated_value=None):
+    """MgmEngine's host-array plan: (inputs: name -> array in its final dtype, in upload order; state: name ->
+    (length, dtype, fill); the descriptor's scalar fields).  Every name is a dev_<name> field of fg_mgm_desc_t."""
+    L = layout
+    dt = PRECISIONS[precision][2]
+    h = mgm_host_arrays(L, mode, var_rank, isolated_value)
+    nb = _neighbourhood_inputs(L, dt, h)
+    inputs = dict(tables=nb.pop("tables"), unary=np.ascontiguousarray(L.unary, dt),
+                  unary_off=np.ascontiguousarray(L.unary_off, np.int64), **nb,
+                  value=_per_var(L, h["value0"], np.int32), cost=_per_var(L, h["cost0"], dt),
+                  has_cost=_per_var(L, ~h["has_nbr"], np.uint8))
+    state = dict(gain=(L.n_vars, dt, 0), new_value=(L.n_vars, np.int32, 0))
+    return inputs, state, dict(mode_max=int(mode == "max"), stop_cycle=int(stop_cycle), seed=_seed(seed))
 
-    def step(self, n_cycles=1):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_mgm_step(self._h, int(n_cycles), self._stream()), "fg_mgm_step")
-        return self
+
+class _LocalSearchEngine(_EngineBase):
+    """MGM, MGM-2 and GDBA: fg_<family>_current reports (round, finished); each variable's cost is known once
+    has_cost is set."""
 
     def _current(self):
         c, f = C.c_int64(), C.c_int32()
-        self.lib.fg_mgm_current(self._h, C.byref(c), C.byref(f))
+        self._fn("current")(self._h, C.byref(c), C.byref(f))
         return c.value, bool(f.value)
 
     @property
@@ -689,10 +623,6 @@ class MgmEngine(_EngineBase):
     def finished(self):
         return self._current()[1]
 
-    @property
-    def launch_count(self):
-        return int(self.lib.fg_mgm_launch_count(self._h))
-
     def values(self):
         """(value index, current cost or NaN while the reference's is None) per variable,
         canonical variable order."""
@@ -700,12 +630,58 @@ class MgmEngine(_EngineBase):
         n = L.n_vars
         cost = self.cost[:n].double().cpu().numpy()
         cost[self.has_cost[:n].cpu().numpy() == 0] = np.nan
-        return L.vars_to_canonical(self.value[:n].cpu().numpy()), L.vars_to_canonical(cost)
+        return L.vars_to_canonical(self._assignment()[:n].cpu().numpy()), L.vars_to_canonical(cost)
 
-    def solution_cost(self, infinity=float("inf"), unary=None):
-        """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
-        out = self._solution_cost(self.value, infinity, unary).cpu().numpy()
-        return float(out[0]), int(out[1])
+
+class MgmEngine(_LocalSearchEngine):
+    """All-variables-at-once MGM (pydcop/algorithms/mgm.py; parameters :78-81).
+
+    var_rank       canonical order: position of each variable's NAME in sorted order, the
+                   lexicographic tie break of mgm.py:574-583 (default: the canonical index)
+    isolated_value canonical order: value index of the variables without neighbours
+                   (optimal_cost_value over the real domain values, relations.py:1641-1669);
+                   default: argopt of the own cost with ties broken on the value index
+    `break_mode` is accepted for the reference's signature; its 'random' branch is dead code in
+    the reference (mgm.py:541 compares with the `random` module) and both settings act as 'lexic'.
+    """
+    FAMILY = "mgm"
+
+    def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
+                 stop_cycle=0, seed=0, break_mode="lexic", var_rank=None, isolated_value=None):
+        L = layout
+        tdt = self._open(layout, device, precision)
+        if break_mode not in ("lexic", "random"):
+            raise ValueError(f"invalid break_mode {break_mode!r}")
+        if mode not in ("min", "max"):
+            raise ValueError(f"invalid mode {mode!r}")
+        inputs, state, scalars = mgm_plan(L, precision, mode, stop_cycle, seed, var_rank, isolated_value)
+        self.has_nbr_host = np.diff(inputs["nbr_ptr"]) > 0
+        t = self._upload(inputs, state)
+        self.__dict__.update(t)
+        self._classes = _class_array(L)
+        d = fill_desc(fill_header(FgMgmDesc(), precision, L, self._classes), t, scalars)
+        # the fast value-phase kernel on the DSA fast-path arrays (binary constraints over one domain size
+        # in {4, 8, 10, 16, 20}), 2 incidences per trip by default.  PYDCOP_B200_MGM_FAST=0|2|4
+        self.fast_chunk = 0
+        chunk = int(os.environ.get("PYDCOP_B200_MGM_FAST", "2") or 0)
+        if chunk in (2, 4):
+            with torch.cuda.device(self.device):
+                fast = dsa_fast_arrays(L, self.tables, mode)
+            if fast is not None and fast[4] in (4, 8, 10, 16, 20):
+                self.tables_or, self.slot_tab, self.slot_nbr, _, fast_dom = fast
+                d.fast_dom, d.fast_chunk = fast_dom, chunk
+                self.fast_chunk = chunk
+                self.row_cache = self.slot_last = None
+                if os.environ.get("PYDCOP_B200_MGM_CACHE", "1") != "0":   # active-row array (csrc/mgm_cached_kernels.cuh)
+                    with torch.cuda.device(self.device):
+                        self.row_cache = torch.zeros(max(L.n_edges * fast_dom, 4), dtype=tdt, device=self.device)
+                        self.slot_last = torch.full((max(L.n_edges, 1),), 255, dtype=torch.uint8, device=self.device)
+                fill_desc(d, {k: getattr(self, k) for k in ("tables_or", "slot_nbr", "slot_tab", "row_cache",
+                                                            "slot_last")})
+        self._create(d)
+
+    def _assignment(self):
+        return self.value
 
     def gains(self):
         """(gain, intended value) of the last round per variable, canonical order."""
@@ -732,7 +708,25 @@ def mgm2_offer_offsets(layout: FactorGraphLayout, nbr_ptr, nbr_idx):
     return off[:-1].copy(), int(off[-1])
 
 
-class Mgm2Engine(_EngineBase):
+def mgm2_plan(layout: FactorGraphLayout, precision="f32", mode="min", threshold=0.5, favor="unilateral",
+              stop_cycle=0, seed=0, var_rank=None):
+    """Mgm2Engine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan."""
+    L = layout
+    dt = PRECISIONS[precision][2]
+    h = mgm_host_arrays(L, mode, var_rank)
+    offer_off, offer_size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
+    inputs = dict(**_neighbourhood_inputs(L, dt, h), offer_off=_per_var(L, offer_off, np.int64))
+    n = L.n_vars
+    state = dict(value=(n, np.int32, 0), potential_value=(n, np.int32, 0), answer_value=(n, np.int32, 0),
+                 partner=(n, np.int32, -1), cost=(n, dt, 0), gain=(n, dt, 0), local_cost=(n, dt, 0),
+                 answer_gain=(n, dt, 0), has_cost=(n, np.uint8, 0), offerer=(n, np.uint8, 0),
+                 committed=(n, np.uint8, 0), go=(n, np.uint8, 0), answer=(n, np.uint8, 0),
+                 offer=(offer_size, dt, 0))
+    return inputs, state, dict(mode_max=int(mode == "max"), favor=_cabi.MGM2_FAVORS[favor], threshold=float(threshold),
+                               stop_cycle=int(stop_cycle or 0), seed=_seed(seed))
+
+
+class Mgm2Engine(_LocalSearchEngine):
     """All-variables-at-once MGM-2 (pydcop/algorithms/mgm2.py; parameters :139-143).
 
     threshold  a variable offers a coordinated move when its draw u < threshold
@@ -743,117 +737,27 @@ class Mgm2Engine(_EngineBase):
     Variable costs are not part of MGM-2's costs (assignment_cost without them); a variable without
     neighbours takes a drawn value among its best over its unary constraints on the device.
     """
+    FAMILY = "mgm2"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
                  threshold=0.5, favor="unilateral", stop_cycle=0, seed=0, var_rank=None):
-        self.lib = _cabi.load()
-        self.device = _require_cuda(device)
-        self.layout = L = layout
-        self.precision = precision
-        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        L = layout
+        self._open(layout, device, precision)
         if mode not in ("min", "max"):
             raise ValueError(f"invalid mode {mode!r}")
         if favor not in _cabi.MGM2_FAVORS:
             raise ValueError(f"invalid favor {favor!r}: expected one of {sorted(_cabi.MGM2_FAVORS)}")
-        h = mgm_host_arrays(L, mode, var_rank)
-        self.nbr_ptr_host, self.nbr_idx_host = h["nbr_ptr"], h["nbr_idx"]
-        self.has_nbr_host = h["has_nbr"]
-        offer_off, offer_size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
-        self.offer_bytes = offer_size * np.dtype(self.np_dtype).itemsize
-        n = max(L.n_vars, 1)
-        with torch.cuda.device(self.device):
-            self.tables = self._dev(L.tables, tdt)
-            self.dom_size = self._dev(L.dom_size, torch.int32)
-            self.var_id = self._dev(L.var_order, torch.int32)
-            self.var_rank = self._dev(h["var_rank"], torch.int32)
-            self.edge_var = self._dev(L.edge_var, torch.int32)
-            self.edge_class = self._dev(L.edge_class, torch.int32)
-            self.var_ptr = self._dev(L.var_ptr, torch.int32)
-            self.slot_edge = self._dev(L.slot_edge, torch.int32)
-            self.nbr_ptr = self._dev(h["nbr_ptr"], torch.int32)
-            self.nbr_idx = self._dev(h["nbr_idx"], torch.int32)
-            self.init_value = self._dev(L.init_value, torch.int32)
-            self.offer_off = self._dev(np.resize(offer_off, n) if L.n_vars else np.zeros(1, np.int64), torch.int64)
-            z = lambda dt: torch.zeros(n, dtype=dt, device=self.device)  # noqa: E731
-            self.value, self.potential_value, self.answer_value = z(torch.int32), z(torch.int32), z(torch.int32)
-            self.partner = torch.full((n,), -1, dtype=torch.int32, device=self.device)
-            self.cost, self.gain, self.local_cost, self.answer_gain = z(tdt), z(tdt), z(tdt), z(tdt)
-            self.has_cost, self.offerer, self.committed = z(torch.uint8), z(torch.uint8), z(torch.uint8)
-            self.go, self.answer = z(torch.uint8), z(torch.uint8)
-            self.offer = torch.zeros(max(offer_size, 1), dtype=tdt, device=self.device)
+        inputs, state, scalars = mgm2_plan(L, precision, mode, threshold, favor, stop_cycle, seed, var_rank)
+        self.nbr_ptr_host, self.nbr_idx_host = inputs["nbr_ptr"], inputs["nbr_idx"]
+        self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
+        self.offer_bytes = state["offer"][0] * np.dtype(self.np_dtype).itemsize
+        t = self._upload(inputs, state)
+        self.__dict__.update(t)
         self._classes = _class_array(L)
-        d = _cabi.FgMgm2Desc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
-        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
-        d.classes = C.cast(self._classes, C.POINTER(FgClass))
-        d.dev_tables, d.dev_dom_size = _ptr(self.tables), _ptr(self.dom_size)
-        d.dev_var_id, d.dev_var_rank = _ptr(self.var_id), _ptr(self.var_rank)
-        d.dev_edge_var, d.dev_edge_class = _ptr(self.edge_var), _ptr(self.edge_class)
-        d.dev_var_ptr, d.dev_slot_edge = _ptr(self.var_ptr), _ptr(self.slot_edge)
-        d.dev_nbr_ptr, d.dev_nbr_idx = _ptr(self.nbr_ptr), _ptr(self.nbr_idx)
-        d.dev_init_value = _ptr(self.init_value)
-        d.dev_value, d.dev_cost, d.dev_has_cost = _ptr(self.value), _ptr(self.cost), _ptr(self.has_cost)
-        d.dev_gain, d.dev_potential_value = _ptr(self.gain), _ptr(self.potential_value)
-        d.dev_local_cost, d.dev_offerer, d.dev_partner = _ptr(self.local_cost), _ptr(self.offerer), _ptr(self.partner)
-        d.dev_committed, d.dev_go = _ptr(self.committed), _ptr(self.go)
-        d.dev_answer, d.dev_answer_value = _ptr(self.answer), _ptr(self.answer_value)
-        d.dev_answer_gain = _ptr(self.answer_gain)
-        d.dev_offer_off, d.dev_offer = _ptr(self.offer_off), _ptr(self.offer)
-        d.mode_max, d.favor, d.threshold = int(mode == "max"), _cabi.MGM2_FAVORS[favor], float(threshold)
-        d.stop_cycle, d.seed = int(stop_cycle or 0), int(seed) & (2 ** 64 - 1)
-        self._desc = d
-        self._h = C.c_void_p()
-        self._check(self.lib.fg_mgm2_create(C.byref(d), C.byref(self._h)), "fg_mgm2_create")
+        self._create(fill_desc(fill_header(_cabi.FgMgm2Desc(), precision, L, self._classes), t, scalars))
 
-    def _last_error(self):
-        return (self.lib.fg_mgm2_last_error(self._h) or b"").decode()
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.fg_mgm2_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def init(self):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_mgm2_init(self._h, self._stream()), "fg_mgm2_init")
-        return self
-
-    def step(self, n_cycles=1):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_mgm2_step(self._h, int(n_cycles), self._stream()), "fg_mgm2_step")
-        return self
-
-    def _current(self):
-        c, f = C.c_int64(), C.c_int32()
-        self.lib.fg_mgm2_current(self._h, C.byref(c), C.byref(f))
-        return c.value, bool(f.value)
-
-    @property
-    def cycle(self):
-        return self._current()[0]
-
-    @property
-    def finished(self):
-        return self._current()[1]
-
-    @property
-    def launch_count(self):
-        return int(self.lib.fg_mgm2_launch_count(self._h))
-
-    def values(self):
-        """(value index, current cost or NaN while the reference's is None) per variable,
-        canonical variable order."""
-        L = self.layout
-        n = L.n_vars
-        cost = self.cost[:n].double().cpu().numpy()
-        cost[self.has_cost[:n].cpu().numpy() == 0] = np.nan
-        return L.vars_to_canonical(self.value[:n].cpu().numpy()), L.vars_to_canonical(cost)
+    def _assignment(self):
+        return self.value
 
     def record(self):
         """State of the last cycle per variable, canonical order: local_cost and gain (NaN without
@@ -874,11 +778,6 @@ class Mgm2Engine(_EngineBase):
                    potential_value=np.where(conn, host(self.potential_value), -1).astype(np.int32),
                    go=host(self.go))
         return {k: L.vars_to_canonical(v) for k, v in out.items()}
-
-    def solution_cost(self, infinity=float("inf"), unary=None):
-        """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
-        out = self._solution_cost(self.value, infinity, unary).cpu().numpy()
-        return float(out[0]), int(out[1])
 
 
 def gdba_host_arrays(layout: FactorGraphLayout, nbr_ptr, increase_mode="E", violation="NZ"):
@@ -936,7 +835,31 @@ def gdba_modifiers_view(h, mods, base_mod, increase_mode):
     return out
 
 
-class GdbaEngine(_EngineBase):
+def gdba_plan(layout: FactorGraphLayout, precision="f32", mode="min", modifier="A", violation="NZ", increase_mode="E",
+              stop_cycle=0, seed=0, var_rank=None, isolated_value=None):
+    """GdbaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
+    buffer, and viol_ref / mod_off are None where the modes do not read them."""
+    L = layout
+    dt = PRECISIONS[precision][2]
+    h = mgm_host_arrays(L, mode, var_rank, isolated_value)
+    g = gdba_host_arrays(L, h["nbr_ptr"], increase_mode, violation)
+    nb = _neighbourhood_inputs(L, dt, h)
+    value0 = _per_var(L, h["value0"], np.int32)
+    inputs = dict(tables=nb.pop("tables"), unary=np.ascontiguousarray(L.unary, dt),
+                  unary_off=np.ascontiguousarray(L.unary_off, np.int64),
+                  viol_ref=None if g["viol_ref"] is None else np.ascontiguousarray(g["viol_ref"], dt), **nb,
+                  value=[value0, value0.copy()], cost=_per_var(L, h["cost0"], dt), has_cost=_per_var(L, ~h["has_nbr"], np.uint8),
+                  mod_off=None if g["mod_off"] is None else np.ascontiguousarray(g["mod_off"], np.int64))
+    n = L.n_vars
+    state = dict(improve=(n, dt, 0), new_value=(n, np.int32, 0), breakout=(n, np.uint8, 0),
+                 violated=(L.n_edges, np.uint8, 0), mod=(g["mod_size"], np.int32, 0))
+    return inputs, state, dict(mode_max=int(mode == "max"), modifier=_cabi.GDBA_MODIFIERS[modifier],
+                               violation=_cabi.GDBA_VIOLATIONS[violation],
+                               increase_mode=_cabi.GDBA_INCREASE_MODES[increase_mode], mod_size=g["mod_size"],
+                               stop_cycle=int(stop_cycle or 0), seed=_seed(seed))
+
+
+class GdbaEngine(_LocalSearchEngine):
     """All-variables-at-once GDBA (pydcop/algorithms/gdba.py; parameters :181-185).
 
     modifier       A (base + m, m from 0) | M (base * m, m from 1)
@@ -950,14 +873,12 @@ class GdbaEngine(_EngineBase):
     isolated_value canonical order: value index of the variables without neighbours (optimal_cost_value);
                    default: argopt of the own cost with ties broken on the value index
     """
+    FAMILY = "gdba"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", modifier="A",
                  violation="NZ", increase_mode="E", stop_cycle=0, seed=0, var_rank=None, isolated_value=None):
-        self.lib = _cabi.load()
-        self.device = _require_cuda(device)
-        self.layout = L = layout
-        self.precision = precision
-        prec, tdt, self.np_dtype = PRECISIONS[precision]
+        L = layout
+        self._open(layout, device, precision)
         if mode not in ("min", "max"):
             raise ValueError(f"invalid mode {mode!r}")
         for name, v, ok in (("modifier", modifier, _cabi.GDBA_MODIFIERS),
@@ -965,114 +886,24 @@ class GdbaEngine(_EngineBase):
                             ("increase_mode", increase_mode, _cabi.GDBA_INCREASE_MODES)):
             if v not in ok:
                 raise ValueError(f"invalid {name} {v!r}: expected one of {sorted(ok)}")
-        self.modifier, self.increase_mode = modifier, increase_mode
-        h = mgm_host_arrays(L, mode, var_rank, isolated_value)
-        self.has_nbr_host = h["has_nbr"]
-        self.gh = g = gdba_host_arrays(L, h["nbr_ptr"], increase_mode, violation)
-        self.modifier_bytes = g["mod_size"] * 4
-        n = max(L.n_vars, 1)
-        with torch.cuda.device(self.device):
-            self.tables = self._dev(L.tables, tdt)
-            self.unary = self._dev(L.unary, tdt)
-            self.unary_off = self._dev(L.unary_off, torch.int64)
-            self.viol_ref = self._dev(g["viol_ref"], tdt) if g["viol_ref"] is not None else None
-            self.dom_size = self._dev(L.dom_size, torch.int32)
-            self.var_id = self._dev(L.var_order, torch.int32)
-            self.var_rank = self._dev(h["var_rank"], torch.int32)
-            self.edge_var = self._dev(L.edge_var, torch.int32)
-            self.edge_class = self._dev(L.edge_class, torch.int32)
-            self.var_ptr = self._dev(L.var_ptr, torch.int32)
-            self.slot_edge = self._dev(L.slot_edge, torch.int32)
-            self.nbr_ptr = self._dev(h["nbr_ptr"], torch.int32)
-            self.nbr_idx = self._dev(h["nbr_idx"], torch.int32)
-            self.init_value = self._dev(L.init_value, torch.int32)
-            value0 = np.resize(h["value0"], n) if L.n_vars else np.zeros(1, np.int32)
-            self.value = [self._dev(value0, torch.int32), self._dev(value0, torch.int32)]
-            self.cost = self._dev(np.resize(h["cost0"], n) if L.n_vars else np.zeros(1), tdt)
-            self.has_cost = self._dev((~np.resize(h["has_nbr"], n)).astype(np.uint8) if L.n_vars
-                                      else np.zeros(1, np.uint8), torch.uint8)
-            z = lambda k, dt: torch.zeros(max(k, 1), dtype=dt, device=self.device)  # noqa: E731
-            self.improve, self.new_value, self.breakout = z(n, tdt), z(n, torch.int32), z(n, torch.uint8)
-            self.violated = z(L.n_edges, torch.uint8)
-            self.mod = z(g["mod_size"], torch.int32)
-            self.mod_off = self._dev(g["mod_off"], torch.int64) if g["mod_off"] is not None else None
+        self.modifier, self.violation, self.increase_mode = modifier, violation, increase_mode
+        inputs, state, scalars = gdba_plan(L, precision, mode, modifier, violation, increase_mode, stop_cycle, seed,
+                                           var_rank, isolated_value)
+        self.nbr_ptr_host = inputs["nbr_ptr"]
+        self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
+        self.modifier_bytes = scalars["mod_size"] * 4
+        t = self._upload(inputs, state)
+        self.__dict__.update(t)
         self._classes = _class_array(L)
-        d = _cabi.FgGdbaDesc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
-        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
-        d.classes = C.cast(self._classes, C.POINTER(FgClass))
-        d.dev_tables, d.dev_unary, d.dev_unary_off = _ptr(self.tables), _ptr(self.unary), _ptr(self.unary_off)
-        d.dev_viol_ref = _ptr(self.viol_ref)
-        d.dev_dom_size, d.dev_var_id, d.dev_var_rank = _ptr(self.dom_size), _ptr(self.var_id), _ptr(self.var_rank)
-        d.dev_edge_var, d.dev_edge_class = _ptr(self.edge_var), _ptr(self.edge_class)
-        d.dev_var_ptr, d.dev_slot_edge = _ptr(self.var_ptr), _ptr(self.slot_edge)
-        d.dev_nbr_ptr, d.dev_nbr_idx = _ptr(self.nbr_ptr), _ptr(self.nbr_idx)
-        d.dev_init_value = _ptr(self.init_value)
-        d.dev_value[0], d.dev_value[1] = _ptr(self.value[0]), _ptr(self.value[1])
-        d.dev_cost, d.dev_has_cost, d.dev_improve = _ptr(self.cost), _ptr(self.has_cost), _ptr(self.improve)
-        d.dev_new_value, d.dev_violated = _ptr(self.new_value), _ptr(self.violated)
-        d.dev_breakout = _ptr(self.breakout)
-        d.dev_mod, d.dev_mod_off, d.mod_size = _ptr(self.mod), _ptr(self.mod_off), g["mod_size"]
-        d.mode_max = int(mode == "max")
-        d.modifier, d.violation = _cabi.GDBA_MODIFIERS[modifier], _cabi.GDBA_VIOLATIONS[violation]
-        d.increase_mode = _cabi.GDBA_INCREASE_MODES[increase_mode]
-        d.stop_cycle, d.seed = int(stop_cycle or 0), int(seed) & (2 ** 64 - 1)
-        self._desc = d
-        self._h = C.c_void_p()
-        self._check(self.lib.fg_gdba_create(C.byref(d), C.byref(self._h)), "fg_gdba_create")
+        self._create(fill_desc(fill_header(_cabi.FgGdbaDesc(), precision, L, self._classes), t, scalars))
 
-    def _last_error(self):
-        return (self.lib.fg_gdba_last_error(self._h) or b"").decode()
+    @functools.cached_property
+    def gh(self):
+        """gdba_host_arrays of the layout: where each slot's modifiers are, for the canonical readback."""
+        return gdba_host_arrays(self.layout, self.nbr_ptr_host, self.increase_mode, self.violation)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.fg_gdba_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def init(self):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_gdba_init(self._h, self._stream()), "fg_gdba_init")
-        return self
-
-    def step(self, n_cycles=1):
-        with torch.cuda.device(self.device):
-            self._check(self.lib.fg_gdba_step(self._h, int(n_cycles), self._stream()), "fg_gdba_step")
-        return self
-
-    def _current(self):
-        c, f = C.c_int64(), C.c_int32()
-        self.lib.fg_gdba_current(self._h, C.byref(c), C.byref(f))
-        return c.value, bool(f.value)
-
-    @property
-    def cycle(self):
-        return self._current()[0]
-
-    @property
-    def finished(self):
-        return self._current()[1]
-
-    @property
-    def launch_count(self):
-        return int(self.lib.fg_gdba_launch_count(self._h))
-
-    def _value_buffer(self):
+    def _assignment(self):
         return self.value[self.cycle % 2]
-
-    def values(self):
-        """(value index, current cost or NaN while the reference's is None) per variable,
-        canonical variable order."""
-        L = self.layout
-        n = L.n_vars
-        cost = self.cost[:n].double().cpu().numpy()
-        cost[self.has_cost[:n].cpu().numpy() == 0] = np.nan
-        return L.vars_to_canonical(self._value_buffer()[:n].cpu().numpy()), L.vars_to_canonical(cost)
 
     def record(self):
         """State of the last round, canonical order: improve (NaN without neighbours), new_value (-1
@@ -1093,10 +924,27 @@ class GdbaEngine(_EngineBase):
         return gdba_modifiers_view(self.gh, self.mod.cpu().numpy(), 0 if self.modifier == "A" else 1,
                                    self.increase_mode)
 
-    def solution_cost(self, infinity=float("inf"), unary=None):
-        """(cost, violations) of the current assignment on the device (dcop.py:319-367)."""
-        out = self._solution_cost(self._value_buffer(), infinity, unary).cpu().numpy()
-        return float(out[0]), int(out[1])
+
+def dpop_plan(layout: FactorGraphLayout, tree, sched, precision="f64", mode="min"):
+    """DpopEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan, for the pseudo-tree
+    `tree` and its pseudotree.schedule `sched`; the scalars carry the launch lists."""
+    from . import pseudotree as pt
+    L = layout
+    dt = PRECISIONS[precision][2]
+    terms = pt.terms(tree, L)
+    arena = terms.pop("arena_size")
+    inputs = dict(tables=np.ascontiguousarray(L.tables, dt), unary=np.ascontiguousarray(L.unary, dt), **terms,
+                  **{k: getattr(sched, k) for k in ("util_nodes", "util_seg_ptr", "value_nodes", "value_seg_ptr")})
+    state = dict(arena=(arena, dt, None), value=(L.n_vars, np.int32, 0), cost=(L.n_vars, dt, 0),
+                 unresolved=(1, np.int32, 0))
+    launches = lambda ls: C.cast((_cabi.FgDpopLaunch * max(1, len(ls)))(*[_cabi.FgDpopLaunch(*l, 0) for l in ls]),  # noqa: E731
+                                 C.POINTER(_cabi.FgDpopLaunch))
+    return inputs, state, dict(
+        n_vars=L.n_vars, mode_max=int(mode == "max"), n_terms=len(terms["term_kind"]),
+        n_tdims=len(terms["tdim_pos"]), arena_size=arena, n_util_segs=len(sched.util_seg_ptr) - 1,
+        n_value_segs=len(sched.value_seg_ptr) - 1, n_util_launches=len(sched.util_launches),
+        n_value_launches=len(sched.value_launches), util_launches=launches(sched.util_launches),
+        value_launches=launches(sched.value_launches), max_sep=max((len(s) for s in tree.sep), default=0))
 
 
 class DpopEngine(_EngineBase):
@@ -1107,15 +955,13 @@ class DpopEngine(_EngineBase):
     tree  a completed PseudoTree over the layout's canonical variables and constraints (build_tree, or
           tree_from_links on the plugin path)
     """
+    FAMILY = "dpop"
 
     def __init__(self, layout: FactorGraphLayout, tree, device=None, precision="f64", mode="min"):
         from . import pseudotree as pt
-        self.lib = _cabi.load()
-        self.device = _require_cuda(device)
-        self.layout = L = layout
+        L = layout
+        self._open(layout, device, precision)
         self.tree = tree
-        self.precision = precision
-        prec, tdt, self.np_dtype = PRECISIONS[precision]
         if mode not in ("min", "max"):
             raise ValueError(f"invalid mode {mode!r}")
         if tree.n_vars != L.n_vars or len(tree.owner) != L.n_factors:
@@ -1134,59 +980,16 @@ class DpopEngine(_EngineBase):
         max_sep = max((len(s) for s in tree.sep), default=0)
         if max_sep > pt.MAX_SEP:
             raise EngineError(f"a separator of {max_sep} variables: the kernels decode at most {pt.MAX_SEP}")
-        self.sched = s = pt.schedule(tree)
-        d_ = pt.terms(tree, L)
-        self.unresolved_host = None
-        with torch.cuda.device(self.device):
-            self.tables = self._dev(L.tables, tdt)
-            self.unary = self._dev(L.unary, tdt)
-            self.arena = torch.empty(max(arena, 1), dtype=tdt, device=self.device)
-            self.dev = {k: self._dev(v, torch.int64 if v.dtype == np.int64 else torch.int32)
-                        for k, v in d_.items() if k != "arena_size"}
-            self.nodes = {k: self._dev(getattr(s, k), torch.int32)
-                          for k in ("util_nodes", "util_seg_ptr", "value_nodes", "value_seg_ptr")}
-            n = max(L.n_vars, 1)
-            self.value = torch.zeros(n, dtype=torch.int32, device=self.device)
-            self.cost = torch.zeros(n, dtype=tdt, device=self.device)
-            self.unresolved_dev = torch.zeros(1, dtype=torch.int32, device=self.device)
-        launches = lambda ls: (_cabi.FgDpopLaunch * max(1, len(ls)))(*[_cabi.FgDpopLaunch(*l, 0) for l in ls])  # noqa: E731
-        self._ul, self._vl = launches(s.util_launches), launches(s.value_launches)
+        self.sched = pt.schedule(tree)
+        inputs, state, scalars = dpop_plan(L, tree, self.sched, precision, mode)
+        self.dev = self._upload(inputs, state)
+        self.arena, self.value, self.cost = self.dev["arena"], self.dev["value"], self.dev["cost"]
+        self.tables, self.unresolved_dev = self.dev["tables"], self.dev["unresolved"]
         self._classes = _class_array(L)
-        dv = self.dev
         d = _cabi.FgDpopDesc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, prec
-        d.n_vars, d.mode_max = L.n_vars, int(mode == "max")
-        d.n_terms, d.n_tdims, d.arena_size = len(d_["term_kind"]), len(d_["tdim_pos"]), arena
-        d.dev_unary, d.dev_tables, d.dev_arena = _ptr(self.unary), _ptr(self.tables), _ptr(self.arena)
-        for k in ("dom_size", "unary_off", "util_off", "util_size", "sep_ptr", "sep_var", "term_ptr", "term_kind",
-                  "term_base", "term_own", "tdim_ptr", "tdim_pos", "tdim_stride"):
-            setattr(d, "dev_" + k, _ptr(dv[k]))
-        for k, t in self.nodes.items():
-            setattr(d, "dev_" + k, _ptr(t))
-        d.n_util_segs, d.n_value_segs = len(s.util_seg_ptr) - 1, len(s.value_seg_ptr) - 1
-        d.n_util_launches, d.n_value_launches = len(s.util_launches), len(s.value_launches)
-        d.util_launches = C.cast(self._ul, C.POINTER(_cabi.FgDpopLaunch))
-        d.value_launches = C.cast(self._vl, C.POINTER(_cabi.FgDpopLaunch))
-        d.dev_value, d.dev_cost, d.dev_unresolved = _ptr(self.value), _ptr(self.cost), _ptr(self.unresolved_dev)
-        d.max_sep = max_sep
-        self._desc = d
-        self._h = C.c_void_p()
+        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, PRECISIONS[precision][0]
         self._done = False
-        self._check(self.lib.fg_dpop_create(C.byref(d), C.byref(self._h)), "fg_dpop_create")
-
-    def _last_error(self):
-        return (self.lib.fg_dpop_last_error(self._h) or b"").decode()
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.fg_dpop_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._create(fill_desc(d, self.dev, scalars))
 
     def init(self):
         self._done = False
@@ -1209,10 +1012,6 @@ class DpopEngine(_EngineBase):
         return 0
 
     @property
-    def launch_count(self):
-        return int(self.lib.fg_dpop_launch_count(self._h))
-
-    @property
     def unresolved(self):
         """Nodes where no value reached the best (the reference raises IndexError there)."""
         return int(self.unresolved_dev.item())
@@ -1232,11 +1031,36 @@ class DpopEngine(_EngineBase):
         shape = tuple(int(self.layout.canon_dom_size[v]) for v in sep)
         return sep, self.arena[off[var]:off[var] + n].double().cpu().numpy().reshape(shape)
 
-    def solution_cost(self, infinity=float("inf"), unary=None):
-        """(cost, violations) of the assignment on the device (dcop.py:319-367)."""
+    def _assignment(self):
+        """The canonical-order values in the layout's internal order."""
         L = self.layout
-        with torch.cuda.device(self.device):
-            internal = self.value[:max(L.n_vars, 1)][torch.as_tensor(L.var_order.astype(np.int64), device=self.device)] \
-                if L.n_vars else self.value
-            out = self._solution_cost(internal.contiguous(), infinity, unary).cpu().numpy()
-        return float(out[0]), int(out[1])
+        return (self.value[:max(L.n_vars, 1)][torch.as_tensor(L.var_order.astype(np.int64), device=self.device)]
+                .contiguous() if L.n_vars else self.value)
+
+
+def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precision="f32", device=None, seed=0,
+                var_rank=None, isolated_value=None, tree=None):
+    """The single-GPU engine of algorithm `kind` (a value of solve.ALGOS) over `layout`.  `params`: its algorithm
+    parameters, the missing ones taking solve.DEFAULTS; var_rank / isolated_value in canonical order as the engines
+    take them (var_rank None: the canonical index); tree: DPOP's pseudo-tree.  MaxSum records no sent flags."""
+    from .solve import DEFAULTS
+    p = dict(DEFAULTS[kind], **params)
+    if kind == "dpop":
+        return DpopEngine(layout, tree=tree, device=device, precision=precision, mode=mode)
+    if kind == "gdba":
+        return GdbaEngine(layout, device=device, precision=precision, mode=mode, modifier=p["modifier"],
+                          violation=p["violation"], increase_mode=p["increase_mode"], stop_cycle=p["stop_cycle"],
+                          seed=seed, var_rank=var_rank, isolated_value=isolated_value)
+    if kind == "mgm2":
+        return Mgm2Engine(layout, device=device, precision=precision, mode=mode, threshold=p["threshold"],
+                          favor=p["favor"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank)
+    if kind == "mgm":
+        return MgmEngine(layout, device=device, precision=precision, mode=mode, stop_cycle=p["stop_cycle"], seed=seed,
+                         break_mode=p["break_mode"], var_rank=var_rank, isolated_value=isolated_value)
+    if kind == "maxsum":
+        return MaxSumEngine(layout, device=device, precision=precision, mode=mode, damping=p["damping"],
+                            damping_nodes=p["damping_nodes"], stability=p["stability"],
+                            start_messages=p["start_messages"], record_sent=False)
+    return DsaEngine(layout, device=device, precision=precision, mode=mode, probability=p["probability"],
+                     p_mode=p.get("p_mode", "fixed"), variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed,
+                     isolated_value=isolated_value, var_costs=(kind == "adsa"))   # A-DSA: candidates carry own costs

@@ -143,35 +143,19 @@ def name_rank(dcop: ingest.DcopArrays) -> np.ndarray:
 
 
 def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
-    from .engine import DpopEngine, DsaEngine, GdbaEngine, MaxSumEngine, Mgm2Engine, MgmEngine
+    from .engine import make_engine
+    tree = var_rank = isolated_value = None
     if kind == "dpop":
         from .pseudotree import build_tree
         a = dcop.arrays
-        return DpopEngine(layout, build_tree(a["dom_size"], a["factor_ptr"], a["edge_var"]), device=device,
-                          precision=precision, mode=mode)
-    if kind == "gdba":
-        return GdbaEngine(layout, device=device, precision=precision, mode=mode,
-                          modifier=params["modifier"], violation=params["violation"],
-                          increase_mode=params["increase_mode"], stop_cycle=params["stop_cycle"],
-                          seed=seed or 0, var_rank=name_rank(dcop), isolated_value=isolated_values(dcop, mode))
-    if kind == "mgm2":
-        return Mgm2Engine(layout, device=device, precision=precision, mode=mode,
-                          threshold=params["threshold"], favor=params["favor"],
-                          stop_cycle=params["stop_cycle"], seed=seed or 0, var_rank=name_rank(dcop))
-    if kind == "mgm":
-        return MgmEngine(layout, device=device, precision=precision, mode=mode,
-                         stop_cycle=params["stop_cycle"], seed=seed or 0,
-                         break_mode=params["break_mode"], var_rank=name_rank(dcop),
-                         isolated_value=isolated_values(dcop, mode))
-    if kind == "maxsum":
-        return MaxSumEngine(layout, device=device, precision=precision, mode=mode,
-                            damping=params["damping"], damping_nodes=params["damping_nodes"],
-                            stability=params["stability"], start_messages=params["start_messages"],
-                            record_sent=False)
-    return DsaEngine(layout, device=device, precision=precision, mode=mode,
-                     probability=params["probability"], p_mode=params.get("p_mode", "fixed"),
-                     variant=params["variant"], stop_cycle=params["stop_cycle"], seed=seed or 0,
-                     isolated_value=isolated_values(dcop, mode), var_costs=(kind == "adsa"))
+        tree = build_tree(a["dom_size"], a["factor_ptr"], a["edge_var"])
+    else:
+        if kind != "mgm2":
+            isolated_value = isolated_values(dcop, mode)
+        if kind in ("mgm", "mgm2", "gdba"):
+            var_rank = name_rank(dcop)
+    return make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=seed or 0,
+                       var_rank=var_rank, isolated_value=isolated_value, tree=tree)
 
 
 def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, partition, halo, sharded_kwargs):

@@ -115,3 +115,37 @@ def test_create_validates_its_descriptor_before_touching_the_device():
         assert b"no CPU fallback" in lib.fg_maxsum_last_error(h)
         lib.fg_maxsum_destroy(h)
         assert lib.fg_device_count() <= 0
+
+
+@pytest.mark.parametrize("family", ["mgm", "mgm2", "gdba", "dpop"])
+def test_plan_passes_every_create_check(family):
+    """The descriptor a family's host-array plan fills (host arrays here) passes every argument check of
+    fg_<family>_create: without a device the one refusal left is FG_ERR_CUDA."""
+    import ctypes as C
+    import torch
+    from pydcop_b200 import _cabi, build_layout, engine as E, pseudotree as pt
+    from pydcop_b200.generators import bounded_separator_instance
+    inst = bounded_separator_instance(14, 4, back=3, span=1, seed=6, float_costs=True)
+    L = build_layout(inst["dom_size"], inst["factor_ptr"], inst["edge_var"], inst["tables"], unary=inst["unary"])
+    if family == "dpop":
+        tree = pt.build_tree(inst["dom_size"], inst["factor_ptr"], inst["edge_var"])
+        inputs, state, scalars = E.dpop_plan(L, tree, pt.schedule(tree), "f64")
+        d = _cabi.FgDpopDesc()
+        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, _cabi.FG_F64
+    else:
+        plan, desc, kw = {"mgm": (E.mgm_plan, _cabi.FgMgmDesc, {}), "mgm2": (E.mgm2_plan, _cabi.FgMgm2Desc, {}),
+                          "gdba": (E.gdba_plan, _cabi.FgGdbaDesc, dict(violation="NM"))}[family]
+        inputs, state, scalars = plan(L, "f64", **kw)
+        classes = E._class_array(L)
+        d = E.fill_header(desc(), "f64", L, classes)
+    arrays = dict(inputs, **E.host_state(state))
+    E.fill_desc(d, arrays, scalars)
+    lib = _cabi.load()
+    h = C.c_void_p()
+    rc = getattr(lib, f"fg_{family}_create")(C.byref(d), C.byref(h))
+    msg = (getattr(lib, f"fg_{family}_last_error")(h) or b"").decode()
+    getattr(lib, f"fg_{family}_destroy")(h)
+    if torch.cuda.is_available():
+        assert rc == _cabi.FG_OK, msg
+    else:
+        assert rc == _cabi.FG_ERR_CUDA and "no CUDA device visible" in msg, (rc, msg)

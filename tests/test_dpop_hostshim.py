@@ -13,6 +13,7 @@ import pytest
 from _dpop_oracle import DpopOracle
 from conftest import ROOT
 from pydcop_b200 import _cabi, pseudotree as pt
+from pydcop_b200.engine import dpop_plan, fill_desc, host_state
 from pydcop_b200.layout import build_layout
 from test_dpop_cpu import NAMES, _integer_without_sentinel, check_against_golden, load, same, tree_of
 
@@ -35,34 +36,16 @@ def shim():
 
 
 class HostDpop:
-    """DpopEngine's descriptor with host arrays, run through the shim."""
+    """DpopEngine's plan (dpop_plan) with host arrays, run through the shim."""
 
     def __init__(self, lib, inst, tree, precision, mode):
-        dt = np.float64 if precision == "f64" else np.float32
         L = build_layout(inst["dom_size"], inst["factor_ptr"], inst["edge_var"], inst["tables"], unary=inst["unary"])
-        s = pt.schedule(tree)
-        d_ = pt.terms(tree, L)
-        c = np.ascontiguousarray
-        self.util_off = d_["util_off"]
-        k = dict(unary=c(L.unary, dt), tables=c(L.tables, dt), arena=np.zeros(max(d_["arena_size"], 1), dt),
-                 value=np.zeros(max(L.n_vars, 1), np.int32), cost=np.zeros(max(L.n_vars, 1), dt),
-                 unresolved=np.zeros(1, np.int32),
-                 **{n: c(getattr(s, n)) for n in ("util_nodes", "util_seg_ptr", "value_nodes", "value_seg_ptr")},
-                 **{n: c(v) for n, v in d_.items() if n != "arena_size"})
-        self.k = k
-        ptr = lambda a: C.c_void_p(a.ctypes.data)  # noqa: E731
-        launches = lambda ls: (_cabi.FgDpopLaunch * max(1, len(ls)))(*[_cabi.FgDpopLaunch(*l, 0) for l in ls])  # noqa: E731
-        self._ul, self._vl = launches(s.util_launches), launches(s.value_launches)
+        inputs, state, scalars = dpop_plan(L, tree, pt.schedule(tree), precision, mode)
+        self.util_off = inputs["util_off"]
+        self.k = k = dict(inputs, **host_state(state))
         d = _cabi.FgDpopDesc()
-        d.precision = _cabi.FG_F64 if precision == "f64" else _cabi.FG_F32
-        d.n_vars, d.mode_max = L.n_vars, int(mode == "max")
-        for n in ("unary", "tables", "arena", "dom_size", "unary_off", "util_off", "util_size", "sep_ptr", "sep_var",
-                  "term_ptr", "term_kind", "term_base", "term_own", "tdim_ptr", "tdim_pos", "tdim_stride",
-                  "util_nodes", "util_seg_ptr", "value_nodes", "value_seg_ptr", "value", "cost", "unresolved"):
-            setattr(d, "dev_" + n, ptr(k[n]) if k[n].size else None)
-        d.n_util_launches, d.n_value_launches = len(s.util_launches), len(s.value_launches)
-        d.util_launches = C.cast(self._ul, C.POINTER(_cabi.FgDpopLaunch))
-        d.value_launches = C.cast(self._vl, C.POINTER(_cabi.FgDpopLaunch))
+        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, _cabi.FG_F64 if precision == "f64" else _cabi.FG_F32
+        fill_desc(d, k, scalars)
         lib.dpop_host_run(C.byref(d))
         n = L.n_vars
         self.value, self.cost = k["value"][:n], k["cost"][:n].astype(np.float64)

@@ -14,7 +14,8 @@ import oracle as orc
 from _gdba_oracle import GdbaOracle
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
-from pydcop_b200.engine import _class_array, gdba_host_arrays, gdba_modifiers_view, mgm_host_arrays
+from pydcop_b200.engine import (_class_array, fill_desc, fill_header, gdba_host_arrays, gdba_modifiers_view,
+                                gdba_plan, host_state, mgm_host_arrays)
 from pydcop_b200.layout import layout_from_instance
 from test_gdba_cpu import check_trajectory
 from test_mgm2_hostshim import random_mgm2_instance
@@ -39,46 +40,21 @@ def shim():
 
 
 class HostGdba:
-    """GdbaEngine's arrays and driving API over the host-shimmed kernels."""
+    """GdbaEngine's plan (gdba_plan) and driving API over the host-shimmed kernels."""
 
     def __init__(self, lib, layout, precision="f64", mode="min", modifier="A", violation="NZ", increase_mode="E",
                  stop_cycle=0, seed=0, var_rank=None, **_):
         self.lib, self.L = lib, layout
-        L = layout
-        dt = np.float64 if precision == "f64" else np.float32
-        h = mgm_host_arrays(L, mode, var_rank)
-        self.has_nbr = h["has_nbr"]
-        self.gh = g = gdba_host_arrays(L, h["nbr_ptr"], increase_mode, violation)
+        inputs, state, scalars = gdba_plan(layout, precision, mode, modifier, violation, increase_mode, stop_cycle,
+                                           seed, var_rank)
+        self.has_nbr = np.diff(inputs["nbr_ptr"]) > 0
+        self.gh = gdba_host_arrays(layout, inputs["nbr_ptr"], increase_mode, violation)
         self.base_mod, self.increase_mode = (0 if modifier == "A" else 1), increase_mode
-        c = np.ascontiguousarray
-        n = max(L.n_vars, 1)
-        z = lambda k, t: np.zeros(max(k, 1), t)  # noqa: E731
-        self.k = k = dict(
-            tables=c(L.tables, dt), unary=c(L.unary, dt), unary_off=c(L.unary_off, np.int64),
-            dom_size=c(L.dom_size, np.int32), var_id=c(L.var_order, np.int32), var_rank=c(h["var_rank"], np.int32),
-            edge_var=c(L.edge_var, np.int32), edge_class=c(L.edge_class, np.int32), var_ptr=c(L.var_ptr, np.int32),
-            slot_edge=c(L.slot_edge, np.int32), nbr_ptr=c(h["nbr_ptr"], np.int32), nbr_idx=c(h["nbr_idx"], np.int32),
-            init_value=c(L.init_value, np.int32), cost=c(np.resize(h["cost0"], n), dt),
-            has_cost=(~np.resize(h["has_nbr"], n)).astype(np.uint8), improve=z(n, dt), new_value=z(n, np.int32),
-            violated=z(L.n_edges, np.uint8), breakout=z(n, np.uint8), mod=z(g["mod_size"], np.int32))
-        if g["viol_ref"] is not None:
-            k["viol_ref"] = c(g["viol_ref"], dt)
-        if g["mod_off"] is not None:
-            k["mod_off"] = c(g["mod_off"], np.int64)
-        self.value = [c(np.resize(h["value0"], n), np.int32) for _ in range(2)]
-        self.classes = _class_array(L)
-        d = _cabi.FgGdbaDesc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, (_cabi.FG_F64 if precision == "f64" else _cabi.FG_F32)
-        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
-        d.classes = C.cast(self.classes, C.POINTER(_cabi.FgClass))
-        for name, a in k.items():
-            setattr(d, "dev_" + name, P(a.ctypes.data))
-        d.dev_value[0], d.dev_value[1] = P(self.value[0].ctypes.data), P(self.value[1].ctypes.data)
-        d.mode_max = int(mode == "max")
-        d.modifier, d.violation = _cabi.GDBA_MODIFIERS[modifier], _cabi.GDBA_VIOLATIONS[violation]
-        d.increase_mode, d.mod_size = _cabi.GDBA_INCREASE_MODES[increase_mode], g["mod_size"]
-        d.stop_cycle, d.seed = int(stop_cycle or 0), int(seed)
-        self.d, self.stop_cycle, self.cycle = d, int(stop_cycle or 0), 0
+        self.k = dict(inputs, **host_state(state))
+        self.value = self.k["value"]
+        self.classes = _class_array(layout)
+        self.d = fill_desc(fill_header(_cabi.FgGdbaDesc(), precision, layout, self.classes), self.k, scalars)
+        self.stop_cycle, self.cycle = scalars["stop_cycle"], 0
 
     @property
     def finished(self):

@@ -14,7 +14,8 @@ import oracle as orc
 from _mgm2_oracle import Mgm2Oracle
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
-from pydcop_b200.engine import _class_array, mgm2_offer_offsets, mgm_host_arrays
+from pydcop_b200.engine import (_class_array, fill_desc, fill_header, host_state, mgm2_offer_offsets,
+                                mgm2_plan, mgm_host_arrays)
 from pydcop_b200.generators import random_factor_graph
 from pydcop_b200.layout import default_var_csr, layout_from_instance
 from test_mgm2_cpu import check_trajectory
@@ -37,39 +38,18 @@ def shim():
 
 
 class HostMgm2:
-    """Mgm2Engine's arrays and driving API over the host-shimmed kernels."""
+    """Mgm2Engine's plan (mgm2_plan) and driving API over the host-shimmed kernels."""
 
     def __init__(self, lib, layout, precision="f64", mode="min", threshold=0.5, favor="unilateral",
                  stop_cycle=0, seed=0, var_rank=None, **_):
         self.lib, self.L = lib, layout
-        L = layout
-        dt = np.float64 if precision == "f64" else np.float32
-        h = mgm_host_arrays(L, mode, var_rank)
-        self.nbr_ptr, self.nbr_idx, self.has_nbr = h["nbr_ptr"], h["nbr_idx"], h["has_nbr"]
-        off, size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
-        c = np.ascontiguousarray
-        n = max(L.n_vars, 1)
-        z = lambda t: np.zeros(n, t)  # noqa: E731
-        self.k = k = dict(
-            tables=c(L.tables, dt), dom_size=c(L.dom_size, np.int32), var_id=c(L.var_order, np.int32),
-            var_rank=c(h["var_rank"], np.int32), edge_var=c(L.edge_var, np.int32),
-            edge_class=c(L.edge_class, np.int32), var_ptr=c(L.var_ptr, np.int32),
-            slot_edge=c(L.slot_edge, np.int32), nbr_ptr=c(h["nbr_ptr"], np.int32),
-            nbr_idx=c(h["nbr_idx"], np.int32), init_value=c(L.init_value, np.int32),
-            value=z(np.int32), cost=z(dt), has_cost=z(np.uint8), gain=z(dt), potential_value=z(np.int32),
-            local_cost=z(dt), offerer=z(np.uint8), partner=np.full(n, -1, np.int32), committed=z(np.uint8),
-            go=z(np.uint8), answer=z(np.uint8), answer_value=z(np.int32), answer_gain=z(dt),
-            offer_off=c(np.resize(off, n), np.int64), offer=np.zeros(max(size, 1), dt))
-        self.classes = _class_array(L)
-        d = _cabi.FgMgm2Desc()
-        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, (_cabi.FG_F64 if precision == "f64" else _cabi.FG_F32)
-        d.n_vars, d.n_factors, d.n_edges, d.n_classes = L.n_vars, L.n_factors, L.n_edges, len(L.classes)
-        d.classes = C.cast(self.classes, C.POINTER(_cabi.FgClass))
-        for name, a in k.items():
-            setattr(d, "dev_" + name, P(a.ctypes.data))
-        d.mode_max, d.favor, d.threshold = int(mode == "max"), _cabi.MGM2_FAVORS[favor], float(threshold)
-        d.stop_cycle, d.seed = int(stop_cycle or 0), int(seed)
-        self.d, self.stop_cycle, self.cycle = d, int(stop_cycle or 0), 0
+        inputs, state, scalars = mgm2_plan(layout, precision, mode, threshold, favor, stop_cycle, seed, var_rank)
+        self.nbr_ptr, self.nbr_idx = inputs["nbr_ptr"], inputs["nbr_idx"]
+        self.has_nbr = np.diff(self.nbr_ptr) > 0
+        self.k = dict(inputs, **host_state(state))
+        self.classes = _class_array(layout)
+        self.d = fill_desc(fill_header(_cabi.FgMgm2Desc(), precision, layout, self.classes), self.k, scalars)
+        self.stop_cycle, self.cycle = scalars["stop_cycle"], 0
 
     @property
     def finished(self):

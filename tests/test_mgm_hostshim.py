@@ -13,7 +13,7 @@ import pytest
 import oracle as orc
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
-from pydcop_b200.engine import _class_array, mgm_host_arrays
+from pydcop_b200.engine import _class_array, fill_desc, host_state, mgm_plan
 from pydcop_b200.generators import random_factor_graph
 from pydcop_b200.layout import default_var_csr, layout_from_instance
 
@@ -47,31 +47,17 @@ def shim():
 
 
 class HostMgm:
-    """MgmEngine's state and driving API over the host-shimmed kernels."""
+    """MgmEngine's plan (mgm_plan) and driving API over the host-shimmed kernels."""
 
     def __init__(self, lib, layout, precision="f64", mode="min", stop_cycle=0, seed=0, var_rank=None,
                  isolated_value=None, **_):
         self.lib, self.L = lib, layout
-        L = layout
-        dt = np.float64 if precision == "f64" else np.float32
-        h = mgm_host_arrays(L, mode, var_rank, isolated_value)
-        c = np.ascontiguousarray
-        n = max(L.n_vars, 1)
-        self.keep = dict(
-            classes=_class_array(L), dom_size=c(L.dom_size, np.int32), var_id=c(L.var_order, np.int32),
-            var_rank=c(h["var_rank"], np.int32), edge_var=c(L.edge_var, np.int32),
-            edge_class=c(L.edge_class, np.int32), var_ptr=c(L.var_ptr, np.int32),
-            slot_edge=c(L.slot_edge, np.int32), nbr_ptr=c(h["nbr_ptr"], np.int32),
-            nbr_idx=c(h["nbr_idx"], np.int32), unary_off=c(L.unary_off, np.int64),
-            init_value=c(L.init_value, np.int32), tables=c(L.tables, dt), unary=c(L.unary, dt),
-            value=c(np.resize(h["value0"], n), np.int32), cost=c(np.resize(h["cost0"], n), dt),
-            has_cost=c(~np.resize(h["has_nbr"], n), np.uint8), gain=np.zeros(n, dt),
-            new_value=np.zeros(n, np.int32))
-        a = _Arrays()
-        for k, v in self.keep.items():
-            setattr(a, k, C.cast(v, P) if k == "classes" else P(v.ctypes.data))
-        a.n_vars, a.mode_max, a.seed = L.n_vars, int(mode == "max"), int(seed)
-        a.precision = _cabi.FG_F64 if precision == "f64" else _cabi.FG_F32
+        inputs, state, scalars = mgm_plan(layout, precision, mode, stop_cycle, seed, var_rank, isolated_value)
+        self.classes = _class_array(layout)
+        self.keep = dict(inputs, **host_state(state))
+        a = fill_desc(_Arrays(), self.keep, {k: scalars[k] for k in ("mode_max", "seed")}, prefix="")
+        a.classes = C.cast(self.classes, P)
+        a.n_vars, a.precision = layout.n_vars, _cabi.FG_F64 if precision == "f64" else _cabi.FG_F32
         self.a, self.stop_cycle, self.cycle = a, int(stop_cycle), 0
 
     @property

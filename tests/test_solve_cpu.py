@@ -137,19 +137,30 @@ def test_infinity_counts_as_violation():
     assert S.solution_cost(d, [0, 0], infinity=float("inf")) == (0, 20000.0)
 
 
-def test_engine_construction_arguments_exist():
-    """_default_engine cannot run here (no GPU); at least bind its keyword arguments against the
-    engines' signatures so a renamed parameter fails on CPU."""
+def _calls(fn):
     import ast
+    return {n.func.id: n for n in ast.walk(ast.parse(inspect.getsource(fn).lstrip()))
+            if isinstance(n, ast.Call) and isinstance(n.func, ast.Name)}
+
+
+def test_make_engine_arguments_exist():
+    """The engines cannot be built here (no GPU); at least bind the keyword arguments of engine.make_engine's
+    constructor calls against all six engines' signatures, and those of its two callers (solve._default_engine,
+    GpuSession._make_engine) against make_engine's, so a renamed parameter fails on CPU."""
     from pydcop_b200 import engine as E
-    tree = ast.parse(inspect.getsource(S._default_engine))
-    calls = {n.func.id: n for n in ast.walk(tree)
-             if isinstance(n, ast.Call) and isinstance(n.func, ast.Name)}
-    for cls in (E.MaxSumEngine, E.DsaEngine, E.MgmEngine):
+    from pydcop_b200.algorithms._session import GpuSession
+    calls = _calls(E.make_engine)
+    for cls in (E.MaxSumEngine, E.DsaEngine, E.MgmEngine, E.Mgm2Engine, E.GdbaEngine, E.DpopEngine):
         names = {k.arg for k in calls[cls.__name__].keywords}
         sig = set(inspect.signature(cls.__init__).parameters)
         assert names and names <= sig, (cls.__name__, names - sig)
         assert len(calls[cls.__name__].args) == 1  # the layout
+    sig = inspect.signature(E.make_engine)
+    for caller in (S._default_engine, GpuSession._make_engine):
+        call = _calls(caller)["make_engine"]
+        names = {k.arg for k in call.keywords}
+        assert names and names <= set(sig.parameters), (caller.__name__, names - set(sig.parameters))
+        assert len(call.args) == 3  # kind, layout, params
 
 
 def test_cli_prints_json(tmp_path, capsys, monkeypatch):
