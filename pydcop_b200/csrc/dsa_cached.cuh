@@ -147,11 +147,12 @@ k_dsa_step_cached(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t
   }
   T best_cost = mode_max ? -Inf<T>::pos() : Inf<T>::pos();   // find_optimal (relations.py:1594-1638)
   int nbest = 0;
+  bool cur_best = false;   // the current value is one of the best
 #pragma unroll
   for (int x = 0; x < D; ++x) {
     const T cx = cost[x];
-    if (cx == best_cost) ++nbest;
-    else if (mode_max ? (cx > best_cost) : (cx < best_cost)) { best_cost = cx; nbest = 1; }
+    if (cx == best_cost) { ++nbest; cur_best |= x == cur; }
+    else if (mode_max ? (cx > best_cost) : (cx < best_cost)) { best_cost = cx; nbest = 1; cur_best = x == cur; }
   }
   const T delta = fg_abs<T>(cur_cost - best_cost);
   bool attempt = false, drop_cur = false;
@@ -160,7 +161,7 @@ k_dsa_step_cached(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t
   } else if (delta == (T)0) {
     if (variant == FG_DSA_C || (variant == FG_DSA_B && violated)) {
       attempt = true;
-      drop_cur = nbest > 1;
+      drop_cur = nbest > 1 && cur_best;
     }
   }
   int nvv = cur;

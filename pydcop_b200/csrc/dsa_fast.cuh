@@ -56,11 +56,12 @@ k_dsa_step_bin(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *_
   // find_optimal (relations.py:1594-1638)
   T best_cost = mode_max ? -Inf<T>::pos() : Inf<T>::pos();
   int nbest = 0;
+  bool cur_best = false;   // the current value is one of the best
 #pragma unroll
   for (int x = 0; x < D; ++x) {
     const T c = cost[x];
-    if (c == best_cost) ++nbest;
-    else if (mode_max ? (c > best_cost) : (c < best_cost)) { best_cost = c; nbest = 1; }
+    if (c == best_cost) { ++nbest; cur_best |= x == cur; }
+    else if (mode_max ? (c > best_cost) : (c < best_cost)) { best_cost = c; nbest = 1; cur_best = x == cur; }
   }
   const T delta = fg_abs<T>(cur_cost - best_cost);
   bool attempt = false, drop_cur = false;
@@ -69,7 +70,7 @@ k_dsa_step_bin(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *_
   } else if (delta == (T)0) {
     if (variant == FG_DSA_C || (variant == FG_DSA_B && violated)) {
       attempt = true;
-      drop_cur = nbest > 1;
+      drop_cur = nbest > 1 && cur_best;
     }
   }
   int nv = cur;

@@ -79,10 +79,11 @@ k_dsa_step_generic(DsaSide g, int n_vars, const T *__restrict__ tables,
   // find_optimal (relations.py:1594-1638): all values whose cost == best, in domain order
   T best_cost = mode_max ? -Inf<T>::pos() : Inf<T>::pos();
   int nbest = 0;
+  bool cur_best = false;   // the current value is one of the best
   for (int x = 0; x < d; ++x) {
     T c = cost[x];
-    if (c == best_cost) ++nbest;
-    else if (mode_max ? (c > best_cost) : (c < best_cost)) { best_cost = c; nbest = 1; }
+    if (c == best_cost) { ++nbest; cur_best |= x == cur; }
+    else if (mode_max ? (c > best_cost) : (c < best_cost)) { best_cost = c; nbest = 1; cur_best = x == cur; }
   }
   const T delta = fg_abs<T>(cur_cost - best_cost);
   bool attempt = false, drop_cur = false;
@@ -91,7 +92,9 @@ k_dsa_step_generic(DsaSide g, int n_vars, const T *__restrict__ tables,
   } else if (delta == (T)0) {
     if (variant == FG_DSA_C || (variant == FG_DSA_B && violated)) {
       attempt = true;
-      drop_cur = nbest > 1;  // best_values.remove(current_value), dsa.py:380-384
+      // best_values.remove(current_value), dsa.py:380-384.  With A-DSA's own costs delta == 0 does not make the
+      // current value one of the best (cur_cost leaves its own cost out), and then nothing is removed (adsa.py:294-299)
+      drop_cur = nbest > 1 && cur_best;
     }
   }
   int nv = cur;

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from _dpop_oracle import DpopOracle
+import _limits as LM
 from conftest import ROOT
 from pydcop_b200 import _cabi, pseudotree as pt
 from pydcop_b200.engine import dpop_plan, fill_desc, host_state
@@ -85,3 +86,19 @@ def test_shim_runs_big_and_light_nodes_like_the_oracle(shim):
     for u in range(t.n_vars):
         assert same(h.util(t, u), o.util[u]), u
     assert np.array_equal(h.value, o.value) and same(h.cost, o.cost)
+
+
+@pytest.mark.parametrize("precision,mode", [("f64", "min"), ("f32", "max")])
+@pytest.mark.parametrize("case", ["d256", "domain_one", "separator_32"])
+def test_shim_at_the_limits(shim, case, precision, mode):
+    """tests/_limits.py's DPOP instances: UTIL tables of 256^2 entries, variables with one value, and a separator
+    of FG_DPOP_MAX_SEP = 32 variables."""
+    inst = {"d256": LM.dpop_d256, "domain_one": LM.dpop_with_domain_one, "separator_32": lambda: LM.clique(33)}[case]()
+    dt = np.float64 if precision == "f64" else np.float32
+    t = pt.build_tree(inst["dom_size"], inst["factor_ptr"], inst["edge_var"])
+    h = HostDpop(shim, inst, t, precision, mode)
+    o = DpopOracle(inst, t, dt, mode).run()
+    for u in range(t.n_vars):
+        assert same(h.util(t, u), o.util[u]), u
+    assert np.array_equal(h.value, o.value) and same(h.cost, np.asarray(o.cost, dtype=dt))
+    assert h.unresolved == o.unresolved == 0

@@ -10,7 +10,9 @@ import numpy as np
 import pytest
 from hypothesis import given, settings, strategies as st
 
+import _limits as LM
 import oracle as orc
+from bench import oracle_instance
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
 from pydcop_b200.engine import _class_array
@@ -157,3 +159,20 @@ def test_generic_kernel_source_with_variable_costs_matches_reference_adsa(name, 
         if k:
             e.step()
         assert np.array_equal(e.values(), inst["value"][k]), k
+
+
+@pytest.mark.parametrize("precision", ["f64", "f32"])
+@pytest.mark.parametrize("case,variant,mode,var_costs", LM.DSA_RUNS)
+def test_generic_dsa_kernel_source_at_the_limits(case, variant, mode, var_costs, precision):
+    """The C-ABI limit instances of tests/_limits.py (domain sizes 1 and 256, all 256 values tied, arity 8, a hub
+    of degree 2400), as tests/test_gpu_limits.py runs them on the device."""
+    inst = LM.DSA[case]()
+    dt = np.float64 if precision == "f64" else np.float32
+    kw = dict(mode=mode, variant=variant, seed=7, probability=0.7, var_costs=var_costs)
+    e = HostDsa(inst, precision, **kw).init()
+    o = orc.DsaOracle(oracle_instance(inst, e.L), dt, **kw).init()
+    assert np.array_equal(e.values(), o.val)
+    for k in range(1, 11):
+        o.step()
+        e.step()
+        assert np.array_equal(e.values(), o.val), k

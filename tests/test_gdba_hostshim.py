@@ -10,6 +10,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import _limits as LM
 import oracle as orc
 from _gdba_oracle import GdbaOracle
 from conftest import GOLDEN_DIR, ROOT, golden_names
@@ -236,3 +237,15 @@ def test_kernel_source_isolated_variables(shim):
         assert val.tolist() == [want] and cost.tolist() == [inst["unary"][want]]
         o = GdbaOracle(inst, mode=mode).init().step(3)
         assert o.values()[0].tolist() == [want]
+
+
+@pytest.mark.parametrize("modifier,increase_mode", LM.GDBA_MODES)
+@pytest.mark.parametrize("case", list(LM.LOCAL))
+def test_kernel_source_at_the_limits(shim, case, modifier, increase_mode):
+    """Domain sizes 1 and 256 and the mix {1, 2, 256} (tests/_limits.py), as tests/test_gpu_limits.py runs them."""
+    inst = LM.gdba_instance(case)
+    kw = dict(mode="min", modifier=modifier, violation="NZ", increase_mode=increase_mode, seed=23)
+    o = GdbaOracle(inst, np.float64, **kw).init()
+    eng = HostGdba(shim, layout_from_instance(inst), precision="f64", var_rank=inst["var_rank"], **kw).init()
+    compare_with_oracle(eng, o, np.float64, 6)
+    assert o.stats["breakouts"] > 0

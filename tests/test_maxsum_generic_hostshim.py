@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 from hypothesis import given, settings, strategies as st
 
+import _limits as LM
 import oracle as orc
 from bench import oracle_instance
 from conftest import GOLDEN_DIR, ROOT, golden_names
@@ -155,11 +156,16 @@ def _mixed_instance(rng, n_vars, doms, shapes):
                 unary=rng.uniform(0, 0.5, size=int(dom_size.sum())))
 
 
-@pytest.mark.parametrize("case", ["high_arity", "big_domains", "hub", "unary_only", "max_arity", "max_domain", "no_factors"])
+@pytest.mark.parametrize("case", ["high_arity", "big_domains", "hub", "unary_only", "max_arity", "max_domain", "no_factors"]
+                         + ["limits_" + c for c in LM.MAXSUM])
 @pytest.mark.parametrize("precision", ["f64", "f32"])
 def test_generic_kernel_source_on_shapes_beyond_the_gpu_tests(case, precision):
+    """Small shapes of every kind, and the C-ABI limit instances of tests/_limits.py that
+    tests/test_gpu_limits.py runs on the device kernels."""
     rng = np.random.default_rng(hash(case) % 1000)
-    if case == "high_arity":          # arity 5 and 6 (FG_MAX_ARITY = 8), small domains
+    if case.startswith("limits_"):
+        inst = LM.MAXSUM[case[len("limits_"):]]()
+    elif case == "high_arity":        # arity 5 and 6 (FG_MAX_ARITY = 8), small domains
         inst = _mixed_instance(rng, 24, [2, 3], [(5, 6), (6, 3), (2, 10), (1, 3)])
     elif case == "big_domains":       # domains up to 40
         inst = _mixed_instance(rng, 14, [17, 33, 40], [(2, 12), (1, 2)])

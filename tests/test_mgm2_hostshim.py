@@ -10,6 +10,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import _limits as LM
 import oracle as orc
 from _mgm2_oracle import Mgm2Oracle
 from conftest import GOLDEN_DIR, ROOT, golden_names
@@ -238,3 +239,25 @@ def test_kernel_source_no_neighbors(shim):
         eng = HostMgm2(shim, layout_from_instance(inst), precision=precision, mode="max").init()
         val, cost = eng.values()
         assert val.tolist() == [9] and cost.tolist() == [18.0]
+
+
+@pytest.mark.parametrize("precision,mode,favor", [("f32", "min", "no"), ("f64", "max", "coordinated")])
+@pytest.mark.parametrize("case", list(LM.LOCAL))
+def test_kernel_source_at_the_limits(shim, case, precision, mode, favor):
+    """Domain sizes 1 and 256 and the mix {1, 2, 256} (tests/_limits.py), as tests/test_gpu_limits.py runs them."""
+    inst = LM.LOCAL[case]()
+    dt = np.float64 if precision == "f64" else np.float32
+    kw = dict(mode=mode, favor=favor, threshold=0.5, seed=19)
+    o = Mgm2Oracle(inst, dt, **kw).init()
+    eng = HostMgm2(shim, layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
+    assert np.array_equal(eng.values()[0], o.values()[0])
+    offers = 0
+    for k in range(1, 5):
+        o.step()
+        eng.step()
+        rec = o.record()
+        _assert_same(eng.record(), rec, dt, k)
+        assert np.array_equal(eng.values()[0], o.values()[0]), k
+        assert np.array_equal(eng.values()[1].astype(dt), o.values()[1].astype(dt), equal_nan=True), k
+        offers += int(rec["offerer"].sum())
+    assert offers > 0

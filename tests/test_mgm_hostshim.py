@@ -10,6 +10,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import _limits as LM
 import oracle as orc
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
@@ -203,3 +204,24 @@ def test_fast_value_phase_source_matches_generic_and_oracle(shim, d, mode, preci
             assert np.array_equal(gain.astype(dt), o.gain) and np.array_equal(new_value, o.new_val), k
         moved += int((prev != o.val).sum())
     assert moved > 0 and np.diff(inst["var_ptr"]).max() > 2 * chunk
+
+
+@pytest.mark.parametrize("mode", ["min", "max"])
+@pytest.mark.parametrize("precision", ["f64", "f32"])
+@pytest.mark.parametrize("case", list(LM.MGM))
+def test_kernel_source_at_the_limits(shim, case, precision, mode):
+    """Domain sizes 1 and 256 with every value tied (tests/_limits.py), as tests/test_gpu_limits.py runs them."""
+    inst = LM.MGM[case]()
+    dt = np.float64 if precision == "f64" else np.float32
+    o = orc.MgmOracle(inst, dt, mode=mode, seed=17).init()
+    eng = HostMgm(shim, layout_from_instance(inst), precision=precision, mode=mode, seed=17,
+                  var_rank=inst["var_rank"]).init()
+    assert np.array_equal(eng.values()[0], o.val)
+    for k in range(1, 9):
+        o.step()
+        eng.step()
+        val, cost = eng.values()
+        assert np.array_equal(val, o.val), k
+        assert np.array_equal(cost.astype(dt), o.cost, equal_nan=True), k
+        gain, new_value = eng.gains()
+        assert np.array_equal(gain.astype(dt), o.gain) and np.array_equal(new_value, o.new_val), k
