@@ -615,6 +615,81 @@ const char *fg_dpop_last_error(fg_dpop_t h);
 int fg_dpop_run(fg_dpop_t h, void *stream);
 int64_t fg_dpop_launch_count(fg_dpop_t h);
 
+/* ------------------------------------------------------------------------------------------
+ * DBA  (pydcop/algorithms/dba.py: Yokoo and Hirayama's distributed breakout, for ALL variables at
+ * once).  Same constraint-hypergraph arrays as MGM.  DBA reads a table only through
+ * `entry >= infinity` (:478), so fg_dba_init evaluates that predicate once, in the tables' precision,
+ * into VIOLATION BIT ROWS: slot s (variable v at scope position j of constraint f) owns
+ * table_size / dom(v) rows, indexed by the mixed-radix index of the OTHER scope variables' values in
+ * scope order; a row is ceil(dom(v) / 32) words and bit x of word x / 32 is entry(v = x) >= infinity.
+ * Slot s's rows start at word dev_bit_off[s].  Later writes to dev_tables are not seen.
+ * One round = two launches (phases: ok of round k = 2k, improve = 2k + 1, k from 1):
+ *   1. ok (:366-420): eval of every value = sum of the slot weights whose bit is set; best below
+ *      `infinity`, improve, consistency, the posted counter, the violated slots at the current value
+ *   2. improve (:504-562): counter minimum, the contest (larger improve, then smaller name), the stop
+ *      test (counter == max_distance), the move or the weight raise.
+ * End flood (:578-588): a variable finishes at phase p, and does nothing else, iff a neighbour's
+ * dev_finish_phase < p; a stopping variable finishes at its improve phase.  dev_status = {live,
+ * end_round}: live counts the unfinished variables with neighbours, end_round (INT32_MAX while live > 0)
+ * the round in which it reached 0; rounds after end_round change no state.  Variables without
+ * neighbours never evaluate, move or finish.
+ * Draws: Philox4x32-10 counter (canonical variable id, cycle, 0, 0); cycle 0xffffffff for the start
+ * value of EVERY variable (initial values are ignored), else the reference's cycle_count, k - 1.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t abi_version, precision;
+  int32_t n_vars, n_factors, n_edges, n_classes;
+  const fg_class_t *classes;      /* HOST [n_classes] */
+  const void *dev_tables;         /* T[...] read once, by fg_dba_init */
+  const int32_t *dev_dom_size;    /* [n_vars] */
+  const int32_t *dev_var_id;      /* [n_vars] canonical id = Philox counter */
+  const int32_t *dev_var_rank;    /* [n_vars] position of the variable's NAME in sorted order */
+  const int32_t *dev_edge_var;    /* [n_edges] */
+  const int32_t *dev_edge_class;  /* [n_edges] */
+  const int32_t *dev_var_ptr;     /* [n_vars+1] */
+  const int32_t *dev_slot_edge;   /* [n_edges] incident edges of v in node.constraints order */
+  const int32_t *dev_nbr_ptr;     /* [n_vars+1] distinct neighbours */
+  const int32_t *dev_nbr_idx;     /* [nbr_ptr[n_vars]] */
+  const int64_t *dev_bit_off;     /* [n_edges+1] first word of every slot's bit rows; [n_edges] = n_words */
+  uint32_t *dev_bits;             /* [n_words] violation bit rows (written by fg_dba_init) */
+  int32_t *dev_value[2];          /* [n_vars] each: round k reads dev_value[(k-1) % 2], writes dev_value[k % 2] */
+  int64_t *dev_cost;              /* [n_vars] current_cost: eval(current) after an ok phase, eval - improve after
+                                     a move (the reference assigns the field in both places, :385 and :558) */
+  uint8_t *dev_has_cost;          /* [n_vars] current_cost is not None (an ok phase has run) */
+  int64_t *dev_eval;              /* [n_vars] posted eval(current value) */
+  int64_t *dev_improve;           /* [n_vars] posted improve */
+  int32_t *dev_counter;           /* [n_vars] posted termination counter */
+  int32_t *dev_counter_own;       /* [n_vars] counter after the improve phase */
+  int32_t *dev_new_value;         /* [n_vars] value drawn among the best, -1 without a draw */
+  uint8_t *dev_can_move, *dev_qlm, *dev_consistent;   /* [n_vars] each */
+  int32_t *dev_finish_phase;      /* [n_vars] INT32_MAX while live */
+  int32_t *dev_weight;            /* [n_edges] per slot, from 1 */
+  uint8_t *dev_violated;          /* [n_edges] per slot: violated at the current value (last ok phase) */
+  int32_t *dev_status;            /* [2] live, end_round */
+  int32_t *dev_unresolved;        /* [1] improve > 0 with no value below infinity (the reference raises) */
+  int64_t n_words;                /* uint32 words of dev_bits */
+  int64_t infinity;
+  int32_t max_distance;           /* >= 0; 0 never stops */
+  int32_t stop_cycle;             /* 0 = never; a run ends when round + 1 >= stop_cycle (as fg_gdba_desc_t) */
+  int32_t n_live;                 /* variables with neighbours */
+  int32_t reserved0;
+  uint64_t seed;
+} fg_dba_desc_t;
+
+typedef struct fg_dba *fg_dba_t;
+
+int fg_dba_create(const fg_dba_desc_t *desc, fg_dba_t *out);
+int fg_dba_destroy(fg_dba_t h);
+const char *fg_dba_last_error(fg_dba_t h);
+/* bit rows from dev_tables, start values of every variable, weights 1, counters 0, status reset. */
+int fg_dba_init(fg_dba_t h, void *stream);
+/* up to n_cycles rounds; none once `finished` has been observed by fg_dba_current. */
+int fg_dba_step(fg_dba_t h, int32_t n_cycles, void *stream);
+/* waits for the work already enqueued; cycle = min(rounds enqueued, end_round), finished = every variable
+ * with neighbours finished, or stop_cycle reached.  The current values are in dev_value[cycle % 2]. */
+int fg_dba_current(fg_dba_t h, int64_t *cycle, int32_t *finished);
+int64_t fg_dba_launch_count(fg_dba_t h);
+
 /* Solution cost (next-tier row §8f.1; pydcop/dcop/dcop.py:319-367 `solution_cost`, called by the
  * orchestrator at the end of a run and at every metric tick, orchestrator.py:1229-1231): over the factors
  * of every non-ghost class the table entry at the assignment, over the first n_vars variables

@@ -138,6 +138,22 @@ class FgDpopDesc(C.Structure):
                 ("max_sep", C.c_int32), ("reserved0", C.c_int32)]
 
 
+class FgDbaDesc(C.Structure):
+    _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
+                ("n_vars", C.c_int32), ("n_factors", C.c_int32), ("n_edges", C.c_int32),
+                ("n_classes", C.c_int32), ("classes", C.POINTER(FgClass)),
+                ("dev_tables", P), ("dev_dom_size", P), ("dev_var_id", P), ("dev_var_rank", P),
+                ("dev_edge_var", P), ("dev_edge_class", P), ("dev_var_ptr", P), ("dev_slot_edge", P),
+                ("dev_nbr_ptr", P), ("dev_nbr_idx", P), ("dev_bit_off", P), ("dev_bits", P),
+                ("dev_value", P * 2), ("dev_cost", P), ("dev_has_cost", P), ("dev_eval", P), ("dev_improve", P),
+                ("dev_counter", P), ("dev_counter_own", P), ("dev_new_value", P),
+                ("dev_can_move", P), ("dev_qlm", P), ("dev_consistent", P), ("dev_finish_phase", P),
+                ("dev_weight", P), ("dev_violated", P), ("dev_status", P), ("dev_unresolved", P),
+                ("n_words", C.c_int64), ("infinity", C.c_int64),
+                ("max_distance", C.c_int32), ("stop_cycle", C.c_int32), ("n_live", C.c_int32),
+                ("reserved0", C.c_int32), ("seed", C.c_uint64)]
+
+
 GDBA_MODIFIERS = {"A": 0, "M": 1}
 GDBA_VIOLATIONS = {"NZ": 0, "NM": 1, "MX": 2}
 GDBA_INCREASE_MODES = {"E": 0, "R": 1, "C": 2, "T": 3}
@@ -225,6 +241,13 @@ SYMBOLS = {
     "fg_gdba_step": (C.c_int, [P, C.c_int32, P]),
     "fg_gdba_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "fg_gdba_launch_count": (C.c_int64, [P]),
+    "fg_dba_create": (C.c_int, [C.POINTER(FgDbaDesc), C.POINTER(P)]),
+    "fg_dba_destroy": (C.c_int, [P]),
+    "fg_dba_last_error": (C.c_char_p, [P]),
+    "fg_dba_init": (C.c_int, [P, P]),
+    "fg_dba_step": (C.c_int, [P, C.c_int32, P]),
+    "fg_dba_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "fg_dba_launch_count": (C.c_int64, [P]),
     "fg_dpop_create": (C.c_int, [C.POINTER(FgDpopDesc), C.POINTER(P)]),
     "fg_dpop_destroy": (C.c_int, [P]),
     "fg_dpop_last_error": (C.c_char_p, [P]),

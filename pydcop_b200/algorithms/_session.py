@@ -37,10 +37,12 @@ def tabulate(constraint, cache=None) -> np.ndarray:
 
 
 class Snapshot:
-    __slots__ = ("cycle", "values", "costs", "finished")
+    """`finished`: every proxy reports finished; `done`: the variables that finished on their own (DBA)."""
+    __slots__ = ("cycle", "values", "costs", "finished", "done")
 
-    def __init__(self, cycle, values, costs, finished):
+    def __init__(self, cycle, values, costs, finished, done=frozenset()):
         self.cycle, self.values, self.costs, self.finished = cycle, values, costs, finished
+        self.done = done
 
 
 class GpuSession:
@@ -272,6 +274,14 @@ class GpuSession:
                     break
                 engine.step(n)
                 cycle += n
+                if self.kind == "dba":   # each proxy finishes with its own variable; the rounds that changed state
+                    # the engine stops at stop_cycle - 1 rounds (gdba_gpu's convention): then every proxy finishes
+                    stopped = bool(stop_cycle and cycle + 1 >= stop_cycle)
+                    self._publish(engine, engine.cycle, stopped)
+                    if stopped or engine.finished:
+                        break
+                    time.sleep(0)
+                    continue
                 done = bool(stop_cycle and cycle >= stop_cycle) or bool(getattr(engine, "finished", False))
                 self._publish(engine, cycle, done)
                 if done:
@@ -297,7 +307,11 @@ class GpuSession:
         for i, n in enumerate(self.var_order):
             dom = domain_values(self.variables[n])
             vals[n] = (dom[int(idx[i])], float(costs[i]) if costs is not None else 0.0)
-        self.snapshot = Snapshot(cycle, vals, None, finished)
+        done = frozenset()
+        if self.kind == "dba":
+            fin = engine.finished_vars()
+            done = frozenset(n for i, n in enumerate(self.var_order) if fin[i])
+        self.snapshot = Snapshot(cycle, vals, None, finished, done)
 
     def _pseudo_tree(self, inst):
         """The orchestrator's pseudo-tree over the packed arrays; each node joins the constraints it owns

@@ -925,6 +925,123 @@ class GdbaEngine(_LocalSearchEngine):
                                    self.increase_mode)
 
 
+DBA_MODE_ERROR = "DBA is a constraint **satisfaction** algorithm and only support minimization objective"
+DBA_LIVE = 2 ** 31 - 1     # finish_phase of a variable that has not finished
+
+
+def canonical_slot(layout: FactorGraphLayout):
+    """Canonical slot (var_ptr / var_con order) of every internal slot."""
+    L = layout
+    pos = np.empty(L.n_edges, dtype=np.int64)
+    pos[L.canon_var_edge] = np.arange(L.n_edges)
+    return pos[L.slot_canon_edge] if L.n_edges else np.zeros(0, np.int64)
+
+
+def dba_bit_offsets(layout: FactorGraphLayout):
+    """First uint32 word of every internal slot's violation bit rows, and the total after the last: slot s of
+    variable v owns table_size / dom(v) rows of ceil(dom(v) / 32) words (csrc/dba_kernels.cuh)."""
+    L = layout
+    if not L.n_edges:
+        return np.zeros(1, dtype=np.int64)
+    tsize = np.array([c.table_size for c in L.classes], dtype=np.int64)
+    d = L.dom_size[L.slot_var].astype(np.int64)
+    words = tsize[L.edge_class[L.slot_edge]] // d * ((d + 31) // 32)
+    if int(words.max()) >= 2 ** 32:
+        raise ValueError("a constraint with 2^32 or more bit-row words per variable")
+    return np.concatenate([[0], np.cumsum(words)]).astype(np.int64)
+
+
+def dba_plan(layout: FactorGraphLayout, precision="f32", infinity=10000, max_distance=50, stop_cycle=0, seed=0,
+             var_rank=None):
+    """DbaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
+    buffer and `bits` the violation bit rows fg_dba_init fills from `tables`."""
+    L = layout
+    dt = PRECISIONS[precision][2]
+    h = mgm_host_arrays(L, "min", var_rank)
+    nb = _neighbourhood_inputs(L, dt, h)
+    nb.pop("init_value")                      # dba.py:341-349 ignores initial values
+    bit_off = dba_bit_offsets(L)
+    value0 = _per_var(L, np.zeros(L.n_vars), np.int32)
+    inputs = dict(**nb, bit_off=bit_off, value=[value0, value0.copy()])
+    n, E = L.n_vars, L.n_edges
+    state = dict(bits=(int(bit_off[-1]), np.int32, None), cost=(n, np.int64, 0), has_cost=(n, np.uint8, 0),
+                 eval=(n, np.int64, 0), improve=(n, np.int64, 0), counter=(n, np.int32, 0),
+                 counter_own=(n, np.int32, 0), new_value=(n, np.int32, -1), can_move=(n, np.uint8, 0),
+                 qlm=(n, np.uint8, 0), consistent=(n, np.uint8, 0), finish_phase=(n, np.int32, DBA_LIVE),
+                 weight=(E, np.int32, 1), violated=(E, np.uint8, 0), status=(2, np.int32, 0),
+                 unresolved=(1, np.int32, 0))
+    return inputs, state, dict(n_words=int(bit_off[-1]), infinity=int(infinity), max_distance=int(max_distance),
+                               stop_cycle=int(stop_cycle or 0), n_live=int(h["has_nbr"].sum()), seed=_seed(seed))
+
+
+class DbaEngine(_LocalSearchEngine):
+    """All-variables-at-once DBA (pydcop/algorithms/dba.py; parameters :265-268).
+
+    infinity      a constraint is violated where its entry is >= infinity (compared in the tables' precision)
+    max_distance  a variable stops when its termination counter reaches it (0: never)
+    stop_cycle    0 = run until every variable with neighbours has finished; else rounds also stop when
+                  round + 1 >= stop_cycle (gdba_gpu's convention)
+    var_rank      canonical order: position of each variable's NAME in sorted order, the tie break of
+                  dba.py:515 (default: the canonical index)
+    `cycle` is the number of rounds that changed the state, `finished` is true once every variable with
+    neighbours has finished (or at stop_cycle); `unresolved` counts the rounds in which a variable could improve
+    but had no value below infinity, where the reference raises on random.choice([]): it keeps its value.
+    """
+    FAMILY = "dba"
+
+    def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", infinity=10000,
+                 max_distance=50, stop_cycle=0, seed=0, var_rank=None):
+        if mode != "min":
+            raise ValueError(DBA_MODE_ERROR)
+        if int(max_distance) < 0:
+            raise ValueError(f"invalid max_distance {max_distance!r}: must be >= 0")
+        L = layout
+        self._open(layout, device, precision)
+        inputs, state, scalars = dba_plan(L, precision, infinity, max_distance, stop_cycle, seed, var_rank)
+        self.has_nbr_host = np.diff(inputs["nbr_ptr"]) > 0
+        self.bit_row_bytes = scalars["n_words"] * 4
+        t = self._upload(inputs, state)
+        self.__dict__.update({k: v for k, v in t.items() if k != "unresolved"})
+        self.unresolved_dev = t["unresolved"]
+        self._classes = _class_array(L)
+        self._create(fill_desc(fill_header(_cabi.FgDbaDesc(), precision, L, self._classes), t, scalars))
+
+    @functools.cached_property
+    def _canon_slot(self):
+        return canonical_slot(self.layout)
+
+    def _assignment(self):
+        return self.value[self.cycle % 2]
+
+    @property
+    def unresolved(self):
+        return int(self.unresolved_dev.item())
+
+    def finished_vars(self):
+        """Per variable, canonical order: it has finished (stopped, or reached by the End flood)."""
+        n = self.layout.n_vars
+        return self.layout.vars_to_canonical(self.finish_phase[:n].cpu().numpy() != DBA_LIVE)
+
+    def record(self):
+        """State after the last round, canonical order: per variable eval, improve, new_value (-1 without a draw),
+        can_move, qlm, consistent, counter (as posted with the improve message) and finish_phase (DBA_LIVE while
+        live; phases: ok of round k = 2k, improve = 2k + 1); per canonical slot violated and weight; and the
+        unresolved count and bit_row_bytes."""
+        L = self.layout
+        n, E = L.n_vars, L.n_edges
+        var = lambda t: L.vars_to_canonical(t[:n].cpu().numpy())  # noqa: E731
+
+        def slots(t):
+            out = np.zeros(E, dtype=t.cpu().numpy().dtype)
+            out[self._canon_slot] = t[:E].cpu().numpy()
+            return out
+        out = {k: var(self.__dict__[k]) for k in ("eval", "improve", "new_value", "can_move", "qlm", "consistent",
+                                                  "counter", "finish_phase")}
+        out.update(violated=slots(self.violated), weight=slots(self.weight), unresolved=self.unresolved,
+                   bit_row_bytes=self.bit_row_bytes)
+        return out
+
+
 def dpop_plan(layout: FactorGraphLayout, tree, sched, precision="f64", mode="min"):
     """DpopEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan, for the pseudo-tree
     `tree` and its pseudotree.schedule `sched`; the scalars carry the launch lists."""
@@ -1045,6 +1162,9 @@ def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precisio
     take them (var_rank None: the canonical index); tree: DPOP's pseudo-tree.  MaxSum records no sent flags."""
     from .solve import DEFAULTS
     p = dict(DEFAULTS[kind], **params)
+    if kind == "dba":
+        return DbaEngine(layout, device=device, precision=precision, mode=mode, infinity=p["infinity"],
+                         max_distance=p["max_distance"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank)
     if kind == "dpop":
         return DpopEngine(layout, tree=tree, device=device, precision=precision, mode=mode)
     if kind == "gdba":

@@ -1,5 +1,5 @@
 """Direct solve: a DCOP file (or arrays, or a pyDcop DCOP object) -> GPU engine -> result dict
-(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba, dpop).
+(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba, dpop, dba).
 
 The plugin modules (pydcop_b200/algorithms/) keep pyDcop's orchestrator, agents and one Python
 computation object per graph node around the engine — that is the drop-in path, and it is what
@@ -17,6 +17,9 @@ FINISHED when `stop_cycle` was reached and TIMEOUT otherwise, as in the referenc
 (orchestrator.py:1262, commands/solve.py:560-580).  DPOP is exact and not iterative: it needs neither,
 runs its UTIL and VALUE phases once on the pseudo-tree pydcop_b200.pseudotree builds, and is FINISHED at
 cycle 0.
+DBA (dba.py:265-268, plus `stop_cycle` with GDBA's convention) stops by itself once every variable with
+neighbours has finished (its termination counter reached `max_distance`, or an End message arrived): the loop
+then leaves early and reports the engine's cycle with status FINISHED.  DBA minimises only.
 
 No CPU path: the engines raise EngineError without a CUDA device.  `engine_factory` exists so
 the host logic can be tested without one.
@@ -38,8 +41,9 @@ ADSA_DEFAULTS = {"period": 0.5, "probability": 0.7, "variant": "B", "stop_cycle"
 MGM_DEFAULTS = {"break_mode": "lexic", "stop_cycle": 0}
 MGM2_DEFAULTS = {"threshold": 0.5, "favor": "unilateral", "stop_cycle": 0}
 GDBA_DEFAULTS = {"modifier": "A", "violation": "NZ", "increase_mode": "E", "stop_cycle": 0}
+DBA_DEFAULTS = {"infinity": 10000, "max_distance": 50, "stop_cycle": 0}
 DEFAULTS = {"maxsum": MAXSUM_DEFAULTS, "dsa": DSA_DEFAULTS, "mgm": MGM_DEFAULTS, "adsa": ADSA_DEFAULTS,
-            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS, "dpop": {}}
+            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS, "dpop": {}, "dba": DBA_DEFAULTS}
 _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "start_messages": ("leafs", "leafs_vars", "all"),
             "p_mode": ("fixed", "arity"), "variant": ("A", "B", "C"),
@@ -47,7 +51,7 @@ _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "modifier": ("A", "M"), "violation": ("NZ", "NM", "MX"), "increase_mode": ("E", "R", "C", "T")}
 ALGOS = {"maxsum": "maxsum", "maxsum_gpu": "maxsum", "dsa": "dsa", "dsa_gpu": "dsa",
          "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa", "mgm2": "mgm2", "mgm2_gpu": "mgm2",
-         "gdba": "gdba", "gdba_gpu": "gdba", "dpop": "dpop", "dpop_gpu": "dpop"}
+         "gdba": "gdba", "gdba_gpu": "gdba", "dpop": "dpop", "dpop_gpu": "dpop", "dba": "dba", "dba_gpu": "dba"}
 
 
 def check_params(kind: str, params: Optional[Dict[str, Any]]) -> Dict[str, Any]:
@@ -150,9 +154,9 @@ def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
         a = dcop.arrays
         tree = build_tree(a["dom_size"], a["factor_ptr"], a["edge_var"])
     else:
-        if kind != "mgm2":
+        if kind not in ("mgm2", "dba"):
             isolated_value = isolated_values(dcop, mode)
-        if kind in ("mgm", "mgm2", "gdba"):
+        if kind in ("mgm", "mgm2", "gdba", "dba"):
             var_rank = name_rank(dcop)
     return make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=seed or 0,
                        var_rank=var_rank, isolated_value=isolated_value, tree=tree)
@@ -167,7 +171,7 @@ def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, par
     from .multigpu import ShardedMaxSum, broadcast_owner
     from .multigpu_dsa import ShardedDsa
     rank, world = dist.get_rank(), dist.get_world_size()
-    if kind in ("mgm", "mgm2", "gdba", "dpop"):
+    if kind in ("mgm", "mgm2", "gdba", "dpop", "dba"):
         raise ValueError(f"{kind} is not sharded: run it on one GPU")
     kw = dict(sharded_kwargs or {})
     dev = device if device is not None else (torch.device("cuda", torch.cuda.current_device())
@@ -207,7 +211,7 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     noise).
 
     problem      see `load`
-    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba | dpop (the *_gpu spellings of the plugin modules are
+    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba | dpop | dba (the *_gpu spellings of the plugin modules are
                  accepted)
     algo_params  the reference's parameter names; `stop_cycle` bounds the run in cycles
     timeout      wall-clock bound in seconds (checked every `chunk` cycles)
@@ -233,6 +237,9 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     t0 = time.perf_counter()
     dcop = load(problem, seed)
     mode = dcop.objective
+    if kind == "dba" and mode != "min":
+        from .engine import DBA_MODE_ERROR
+        raise ValueError(DBA_MODE_ERROR)
     inst = dcop.instance()
     if kind == "maxsum":
         inst["unary"] = ingest.add_noise(inst["unary"], params["noise"], seed)
@@ -270,6 +277,10 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
         cycle += n
         if on_cycle is not None:
             on_cycle(cycle, _indices(engine))
+        if kind == "dba" and engine.finished:   # every variable with neighbours finished, or stop_cycle
+            break
+    if kind == "dba":                      # the rounds that changed the state
+        cycle = engine.cycle
     idx = _indices(engine)
     if hasattr(getattr(engine, "engine", engine), "_solution_cost"):   # reduced on the device(s); sharded engines all-reduce over NCCL
         cost, violation = engine.solution_cost(infinity, dcop.arrays["unary"])
