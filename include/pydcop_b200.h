@@ -14,7 +14,15 @@
  *     torch.Tensor.data_ptr()); the only device memory the library owns is the DSA handle's copy
  *     of the class table (a few hundred bytes) and a MaxSum handle's class table of the variable side
  *     (48 bytes per (domain, degree) class); a MaxSum handle also owns one side stream + 2 events;
- *   - `stream` is a cudaStream_t passed as void* (torch.cuda.current_stream().cuda_stream);
+ *   - a handle belongs to the device current when fg_*_create is called: every call on the handle
+ *     runs on that device (it is made current for the call, the caller's device restored on
+ *     return), and every non-NULL dev_* array of its descriptor must be device memory of that
+ *     device — create returns FG_ERR_ARG, naming the field, for host memory or another device's;
+ *     calls without a handle run on the current device and refuse a main array that lives
+ *     elsewhere; fg_enable_peer_access / fg_ipc_import / fg_halo_push take the current device as
+ *     the accessor by design;
+ *   - `stream` is a cudaStream_t passed as void* (torch.cuda.current_stream().cuda_stream), a stream
+ *     of the handle's device;
  *   - all calls are asynchronous on `stream`; the caller synchronises;
  *   - value type T is float (precision = FG_F32) or double (FG_F64) for every cost/message array;
  *   - there is NO CPU fallback: without a CUDA device every launch entry point returns

@@ -8,6 +8,8 @@
 #include <math_constants.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "../../include/pydcop_b200.h"
 
 #define FG_SAME_COUNT 4  // maxsum.py:106
@@ -58,6 +60,17 @@ struct MaxSumParams {
   // `next` buffer of the row this cycle produces, 0 for interior rows (fg_halo_plan_t::dev_edge_dst_r / dev_slot_dst_q)
   const int64_t *edge_dst, *slot_dst;
 };
+
+// The entry of `per_dev` for the current device, added on first use.  What a kernel's launch code works out once
+// (its dynamic shared-memory attribute, its occupancy, the SM count) holds for one device only: an attribute set with
+// cudaFuncSetAttribute belongs to the function in the current device's context.
+template <class S>
+inline S &fg_per_device(std::vector<S> &per_dev) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); dev = 0; }
+  if ((size_t)dev >= per_dev.size()) per_dev.resize((size_t)dev + 1);
+  return per_dev[(size_t)dev];
+}
 
 #define CUDA_TRY(h, expr)                                                          \
   do {                                                                             \

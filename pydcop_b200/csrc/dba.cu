@@ -64,6 +64,18 @@ extern "C" int fg_dba_create(const fg_dba_desc_t *desc, fg_dba_t *out) {
   }
   h->eval_dmax = dba_eval_dmax(h->classes.data(), (int)h->classes.size());
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  const fg_dba_desc_t &d = *desc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_var_id),
+                             FG_FIELD(d, dev_var_rank), FG_FIELD(d, dev_edge_var), FG_FIELD(d, dev_edge_class),
+                             FG_FIELD(d, dev_var_ptr), FG_FIELD(d, dev_slot_edge), FG_FIELD(d, dev_nbr_ptr),
+                             FG_FIELD(d, dev_nbr_idx), FG_FIELD(d, dev_bit_off), FG_FIELD(d, dev_bits),
+                             FG_FIELD(d, dev_value[0]), FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_cost),
+                             FG_FIELD(d, dev_has_cost), FG_FIELD(d, dev_eval), FG_FIELD(d, dev_improve),
+                             FG_FIELD(d, dev_counter), FG_FIELD(d, dev_counter_own), FG_FIELD(d, dev_new_value),
+                             FG_FIELD(d, dev_can_move), FG_FIELD(d, dev_qlm), FG_FIELD(d, dev_consistent),
+                             FG_FIELD(d, dev_finish_phase), FG_FIELD(d, dev_weight), FG_FIELD(d, dev_violated),
+                             FG_FIELD(d, dev_status), FG_FIELD(d, dev_unresolved)});
+  if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }
 
@@ -80,6 +92,7 @@ static void dba_bits_t(fg_dba *h, cudaStream_t st) {
 
 extern "C" int fg_dba_init(fg_dba_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   const fg_dba_desc_t &d = h->d;
   cudaStream_t st = (cudaStream_t)stream;
   if (d.n_edges) {
@@ -127,6 +140,7 @@ static int dba_round(fg_dba *h, cudaStream_t st) {
 
 extern "C" int fg_dba_step(fg_dba_t h, int32_t n_cycles, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_cycles; ++i) {
     if (dba_finished(h)) break;
@@ -143,6 +157,7 @@ extern "C" int fg_dba_step(fg_dba_t h, int32_t n_cycles, void *stream) {
 
 extern "C" int fg_dba_current(fg_dba_t h, int64_t *cycle, int32_t *finished) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (h->started && !h->ended) {
     int32_t status[2];
     CUDA_TRY(h, cudaMemcpyAsync(status, h->d.dev_status, sizeof(status), cudaMemcpyDeviceToHost, h->last_stream));

@@ -71,9 +71,17 @@ extern "C" int fg_dpop_create(const fg_dpop_desc_t *desc, fg_dpop_t *out) {
     return FG_ERR_ARG;
   int rc = fg_require_device(h);
   if (rc != FG_OK) return rc;
-  int dev = 0;
-  CUDA_TRY(h, cudaGetDevice(&dev));
-  CUDA_TRY(h, cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev));
+  const fg_dpop_desc_t &d = *desc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_unary), FG_FIELD(d, dev_tables), FG_FIELD(d, dev_arena),
+                             FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_unary_off), FG_FIELD(d, dev_util_off),
+                             FG_FIELD(d, dev_util_size), FG_FIELD(d, dev_sep_ptr), FG_FIELD(d, dev_sep_var),
+                             FG_FIELD(d, dev_term_ptr), FG_FIELD(d, dev_term_kind), FG_FIELD(d, dev_term_base),
+                             FG_FIELD(d, dev_term_own), FG_FIELD(d, dev_tdim_ptr), FG_FIELD(d, dev_tdim_pos),
+                             FG_FIELD(d, dev_tdim_stride), FG_FIELD(d, dev_util_nodes), FG_FIELD(d, dev_util_seg_ptr),
+                             FG_FIELD(d, dev_value_nodes), FG_FIELD(d, dev_value_seg_ptr), FG_FIELD(d, dev_value),
+                             FG_FIELD(d, dev_cost), FG_FIELD(d, dev_unresolved)});
+  if (rc != FG_OK) return rc;
+  CUDA_TRY(h, cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, h->device));
   return FG_OK;
 }
 
@@ -111,6 +119,7 @@ static int dpop_run_t(fg_dpop *h, cudaStream_t st) {
 
 extern "C" int fg_dpop_run(fg_dpop_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   if (h->d.n_vars == 0) return FG_OK;
   CUDA_TRY(h, cudaMemsetAsync(h->d.dev_unresolved, 0, sizeof(int32_t), st));

@@ -85,6 +85,17 @@ extern "C" int fg_maxsum_create(const fg_maxsum_desc_t *desc, fg_maxsum_t *out) 
     return FG_ERR_ARG;
   }
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  const fg_maxsum_desc_t &d = *desc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_unary), FG_FIELD(d, dev_dom_size),
+                             FG_FIELD(d, dev_unary_off), FG_FIELD(d, dev_var_ptr), FG_FIELD(d, dev_var_qbase),
+                             FG_FIELD(d, dev_slot_roff), FG_FIELD(d, dev_edge_qoff), FG_FIELD(d, dev_slot_roff32),
+                             FG_FIELD(d, dev_edge_qoff32), FG_FIELD(d, dev_slot_edge), FG_FIELD(d, dev_slot_var),
+                             FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_q[0]), FG_FIELD(d, dev_q[1]),
+                             FG_FIELD(d, dev_r[0]), FG_FIELD(d, dev_r[1]), FG_FIELD(d, dev_q_valid),
+                             FG_FIELD(d, dev_r_valid), FG_FIELD(d, dev_q_cnt), FG_FIELD(d, dev_r_cnt),
+                             FG_FIELD(d, dev_q_sent), FG_FIELD(d, dev_r_sent), FG_FIELD(d, dev_value),
+                             FG_FIELD(d, dev_value_cost)});
+  if (rc != FG_OK) return rc;
   maxsum_fast_plan(h->d, h->classes, h->varclasses, h->fast);
   if (maxsum_warp_plan(h->d, h->varclasses, h->fast, h->warp) != FG_OK) {
     snprintf(h->err, sizeof(h->err), "tile descriptors of the variable side: %s", cudaGetErrorString(cudaGetLastError()));
@@ -114,6 +125,7 @@ extern "C" int fg_maxsum_create(const fg_maxsum_desc_t *desc, fg_maxsum_t *out) 
 
 extern "C" int fg_maxsum_destroy(fg_maxsum_t h) {
   if (h) {
+    fg_device_scope on(h);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->ev_join) cudaEventDestroy(h->ev_join);
     if (h->ev_r) cudaEventDestroy(h->ev_r);
@@ -164,6 +176,7 @@ static int maxsum_init_t(fg_maxsum *h, cudaStream_t st) {
 
 extern "C" int fg_maxsum_init(fg_maxsum_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   return h->d.precision == FG_F64 ? maxsum_init_t<double>(h, st) : maxsum_init_t<float>(h, st);
 }
@@ -315,12 +328,14 @@ static int maxsum_compute_t(fg_maxsum *h, cudaStream_t st, bool push_split = fal
 
 extern "C" int fg_maxsum_cycle_compute(fg_maxsum_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   return h->d.precision == FG_F64 ? maxsum_compute_t<double>(h, st) : maxsum_compute_t<float>(h, st);
 }
 
 extern "C" int fg_maxsum_cycle_commit(fg_maxsum_t h) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   h->cur ^= 1;
   ++h->cycle;
   return FG_OK;
@@ -328,6 +343,7 @@ extern "C" int fg_maxsum_cycle_commit(fg_maxsum_t h) {
 
 extern "C" int fg_maxsum_step(fg_maxsum_t h, int32_t n_cycles, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   for (int i = 0; i < n_cycles; ++i) {
     int rc = fg_maxsum_cycle_compute(h, stream);
     if (rc != FG_OK) return rc;
@@ -338,6 +354,7 @@ extern "C" int fg_maxsum_step(fg_maxsum_t h, int32_t n_cycles, void *stream) {
 
 extern "C" int fg_maxsum_current(fg_maxsum_t h, int32_t *buf_index, int64_t *cycle) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (buf_index) *buf_index = h->cur;
   if (cycle) *cycle = h->cycle;
   return FG_OK;
@@ -347,6 +364,7 @@ extern "C" int64_t fg_maxsum_launch_count(fg_maxsum_t h) { return fg_launch_coun
 
 extern "C" int fg_maxsum_kernel_plan(fg_maxsum_t h, int32_t *family, int32_t n_classes) {
   if (!h || !family || n_classes != (int32_t)h->classes.size()) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   for (int32_t i = 0; i < n_classes; ++i) {
     const fg_class_t &c = h->classes[i];
     family[i] = (c.flags & FG_CLASS_GHOST) ? -1 : h->warp.f2v[i] ? FG_KERNEL_WARP : h->fast.f2v[i] ? FG_KERNEL_PIPE
@@ -357,6 +375,7 @@ extern "C" int fg_maxsum_kernel_plan(fg_maxsum_t h, int32_t *family, int32_t n_c
 
 extern "C" int fg_maxsum_table_width(fg_maxsum_t h, int32_t *bytes, int32_t n_classes) {
   if (!h || !bytes || n_classes != (int32_t)h->classes.size()) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   const int32_t full = (int32_t)prec_size(h->d.precision);
   for (int32_t i = 0; i < n_classes; ++i)
     bytes[i] = (!h->warp.tab8_base.empty() && h->warp.tab8_base[i] >= 0) ? 1 : full;
@@ -389,6 +408,7 @@ extern "C" int fg_peer_wait(const fg_peer_sync_t *ps, uint64_t epoch, void *stre
 
 extern "C" int fg_maxsum_shard_attach(fg_maxsum_t h, const fg_halo_plan_t *plan) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (halo_plan_check(plan) != FG_OK) { snprintf(h->err, sizeof(h->err), "invalid halo plan"); return FG_ERR_ARG; }
   if ((size_t)plan->elem_bytes != prec_size(h->d.precision)) { snprintf(h->err, sizeof(h->err), "halo plan element size"); return FG_ERR_ARG; }
   h->halo = *plan;
@@ -428,6 +448,7 @@ extern "C" int fg_maxsum_shard_fused(fg_maxsum_t h) { return (h && h->has_halo &
 
 extern "C" int fg_maxsum_shard_phase(fg_maxsum_t h, int32_t phase, void *stream) {
   if (!h || !h->has_halo) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   const int nxt = h->cur ^ 1;
   switch (phase) {
@@ -453,6 +474,7 @@ extern "C" int fg_maxsum_shard_phase(fg_maxsum_t h, int32_t phase, void *stream)
 //   out[3] push of the q rows (split mode)   out[4] join -> push (+ release) done   out[5] wait   out[6] whole cycle
 extern "C" int fg_maxsum_shard_profile(fg_maxsum_t h, int32_t n_cycles, void *stream, double *out_us) {
   if (!h || !h->has_halo || !out_us || n_cycles < 1) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   cudaEvent_t ev[8];
   for (auto &e : ev) CUDA_TRY(h, cudaEventCreate(&e));
@@ -484,6 +506,7 @@ extern "C" int fg_maxsum_shard_profile(fg_maxsum_t h, int32_t n_cycles, void *st
 
 extern "C" int fg_maxsum_shard_step(fg_maxsum_t h, int32_t n_cycles, void *stream) {
   if (!h || !h->has_halo) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   for (int i = 0; i < n_cycles; ++i)
     for (int ph = 0; ph < 4; ++ph) {
       int rc = fg_maxsum_shard_phase(h, ph, stream);
@@ -514,6 +537,7 @@ template <bool PACK>
 static int halo_rows(int32_t precision, void *arr, void *packed, const int64_t *row_off,
                      const int64_t *packed_off, const int32_t *row_len, int64_t n_rows, void *stream) {
   if (n_rows <= 0) return FG_OK;
+  if (!fg_on_current_device(arr) || !fg_on_current_device(packed)) return FG_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   unsigned blocks = blocks_for(n_rows * 32, 256);
   if (precision == FG_F64)
@@ -571,6 +595,7 @@ extern "C" int fg_halo_rows_uniform(int32_t precision, int32_t pack, void *dev_r
                                     const int64_t *peer_base, void *stream) {
   if (n_r + n_q <= 0) return FG_OK;
   if (n_peers < 1 || n_peers > 16 || dom < 1) return FG_ERR_ARG;
+  if (!fg_on_current_device(dev_packed)) return FG_ERR_ARG;
   HaloPeers hp;
   hp.n = n_peers;
   for (int i = 0; i <= n_peers; ++i) { hp.r_start[i] = peer_r_start[i]; hp.q_start[i] = peer_q_start[i]; }
@@ -681,6 +706,15 @@ extern "C" int fg_dsa_create(const fg_dsa_desc_t *desc, fg_dsa_t *out) {
   if (rc != FG_OK) return rc;
   fg_dsa *h = *out;
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  const fg_dsa_desc_t &d = *desc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_var_id),
+                             FG_FIELD(d, dev_edge_var), FG_FIELD(d, dev_edge_class), FG_FIELD(d, dev_var_ptr),
+                             FG_FIELD(d, dev_slot_edge), FG_FIELD(d, dev_has_nbr), FG_FIELD(d, dev_prob),
+                             FG_FIELD(d, dev_con_opt), FG_FIELD(d, dev_tables_or), FG_FIELD(d, dev_slot_nbr),
+                             FG_FIELD(d, dev_slot_tab), FG_FIELD(d, dev_slot_opt), FG_FIELD(d, dev_value[0]),
+                             FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_value_cost), FG_FIELD(d, dev_var_cost),
+                             FG_FIELD(d, dev_unary_off), FG_FIELD(d, dev_row_cache), FG_FIELD(d, dev_slot_last)});
+  if (rc != FG_OK) return rc;
   {  // experiment knob: L2 -> DRAM fetch granularity hint (32 | 64 | 128 bytes) for the sparse row reads
     const int g = fg_env_int("PYDCOP_B200_L2_FETCH", 0);
     if (g == 32 || g == 64 || g == 128) { cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)g); cudaGetLastError(); }
@@ -721,6 +755,7 @@ static int dsa_init_t(fg_dsa *h, cudaStream_t st) {
 
 extern "C" int fg_dsa_init(fg_dsa_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   return h->d.precision == FG_F64 ? dsa_init_t<double>(h, st) : dsa_init_t<float>(h, st);
 }
@@ -745,6 +780,7 @@ static int dsa_compute_t(fg_dsa *h, cudaStream_t st) {
 
 extern "C" int fg_dsa_cycle_compute(fg_dsa_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (h->d.stop_cycle && h->cycle >= h->d.stop_cycle) return FG_OK;
   cudaStream_t st = (cudaStream_t)stream;
   return h->d.precision == FG_F64 ? dsa_compute_t<double>(h, st) : dsa_compute_t<float>(h, st);
@@ -752,6 +788,7 @@ extern "C" int fg_dsa_cycle_compute(fg_dsa_t h, void *stream) {
 
 extern "C" int fg_dsa_cycle_commit(fg_dsa_t h) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (h->d.stop_cycle && h->cycle >= h->d.stop_cycle) return FG_OK;
   h->cur ^= 1;
   ++h->cycle;
@@ -760,6 +797,7 @@ extern "C" int fg_dsa_cycle_commit(fg_dsa_t h) {
 
 extern "C" int fg_dsa_step(fg_dsa_t h, int32_t n_cycles, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   for (int i = 0; i < n_cycles; ++i) {
     if (h->d.stop_cycle && h->cycle >= h->d.stop_cycle) break;
     int rc = fg_dsa_cycle_compute(h, stream);
@@ -771,6 +809,7 @@ extern "C" int fg_dsa_step(fg_dsa_t h, int32_t n_cycles, void *stream) {
 
 extern "C" int fg_dsa_current(fg_dsa_t h, int32_t *buf_index, int64_t *cycle) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (buf_index) *buf_index = h->cur;
   if (cycle) *cycle = h->cycle;
   return FG_OK;
@@ -780,6 +819,7 @@ extern "C" int64_t fg_dsa_launch_count(fg_dsa_t h) { return fg_launch_count(h); 
 
 extern "C" int fg_dsa_shard_attach(fg_dsa_t h, const fg_halo_plan_t *plan) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (halo_plan_check(plan) != FG_OK || plan->elem_bytes != 4 || plan->dom != 1 || plan->n_q != 0) {
     snprintf(h->err, sizeof(h->err), "invalid halo plan (DSA pushes single 4-byte values, list r only)");
     return FG_ERR_ARG;
@@ -794,6 +834,7 @@ extern "C" int fg_dsa_shard_attach(fg_dsa_t h, const fg_halo_plan_t *plan) {
 // entries of `next` (+ release) -> wait -> commit.  Ghost (frozen) variables are never written locally.
 extern "C" int fg_dsa_shard_step(fg_dsa_t h, int32_t n_cycles, void *stream) {
   if (!h || !h->has_halo) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_cycles; ++i) {
     if (h->d.stop_cycle && h->cycle >= h->d.stop_cycle) break;
@@ -849,6 +890,7 @@ extern "C" int fg_solution_cost(int32_t precision, int32_t n_classes, const fg_c
                                 const int32_t *dev_edge_var, const int32_t *dev_value, const void *dev_unary,
                                 const int64_t *dev_unary_off, int32_t n_vars, const uint8_t *dev_factor_skip,
                                 const uint8_t *dev_var_skip, double infinity, double *dev_out, void *stream) {
+  if (!fg_on_current_device(dev_out) || (dev_value && !fg_on_current_device(dev_value))) return FG_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   if (cudaMemsetAsync(dev_out, 0, 2 * sizeof(double), st) != cudaSuccess) return FG_ERR_CUDA;
   for (int i = 0; i < n_classes; ++i) {
@@ -879,6 +921,7 @@ __global__ void k_selftest_match(int64_t n, const T *__restrict__ c, const T *__
 extern "C" int fg_selftest_approx_match(int32_t precision, int64_t n, const void *dev_c, const void *dev_prev,
                                         double stability, uint8_t *dev_out_fast, uint8_t *dev_out_exact, void *stream) {
   if (n <= 0) return FG_OK;
+  if (!fg_on_current_device(dev_c)) return FG_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   if (precision == FG_F64)
     k_selftest_match<double><<<blocks_for(n, 256), 256, 0, st>>>(n, (const double *)dev_c, (const double *)dev_prev, stability, dev_out_fast, dev_out_exact);
@@ -892,6 +935,7 @@ extern "C" int fg_selftest_gather(const void *dev_base, int64_t region_bytes, in
   if (!dev_base || !dev_out || row_bytes <= 0 || row_bytes % 16 || stride_bytes < row_bytes || stride_bytes % 16 ||
       region_bytes < stride_bytes || n_threads <= 0)
     return FG_ERR_ARG;
+  if (!fg_on_current_device(dev_base)) return FG_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   const uint64_t n_slots = (uint64_t)(region_bytes / stride_bytes);
   const unsigned blocks = blocks_for(n_threads, 128);

@@ -57,6 +57,16 @@ extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
     return FG_ERR_ARG;
   }
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  const fg_gdba_desc_t &d = *desc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_unary), FG_FIELD(d, dev_unary_off),
+                             FG_FIELD(d, dev_viol_ref), FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_var_id),
+                             FG_FIELD(d, dev_var_rank), FG_FIELD(d, dev_edge_var), FG_FIELD(d, dev_edge_class),
+                             FG_FIELD(d, dev_var_ptr), FG_FIELD(d, dev_slot_edge), FG_FIELD(d, dev_nbr_ptr),
+                             FG_FIELD(d, dev_nbr_idx), FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_value[0]),
+                             FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_cost), FG_FIELD(d, dev_has_cost),
+                             FG_FIELD(d, dev_improve), FG_FIELD(d, dev_new_value), FG_FIELD(d, dev_violated),
+                             FG_FIELD(d, dev_breakout), FG_FIELD(d, dev_mod), FG_FIELD(d, dev_mod_off)});
+  if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }
 
@@ -66,6 +76,7 @@ extern "C" const char *fg_gdba_last_error(fg_gdba_t h) { return fg_last_error(h)
 
 extern "C" int fg_gdba_init(fg_gdba_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   const fg_gdba_desc_t &d = h->d;
   cudaStream_t st = (cudaStream_t)stream;
   if (d.mod_size > 0) CUDA_TRY(h, cudaMemsetAsync(d.dev_mod, 0, sizeof(int32_t) * (size_t)d.mod_size, st));

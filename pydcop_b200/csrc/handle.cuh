@@ -1,9 +1,10 @@
 // Host-side scaffolding shared by the fg_<family>_* handles (engine.cu, mgm.cu, mgm2.cu, gdba.cu, dpop.cu): opening a
-// handle over a copy of its descriptor, the class-table checks and upload, closing, and the step loop of the
-// families that stop at cycle + 1 >= stop_cycle.  No device code.
+// handle over a copy of its descriptor, the class-table checks and upload, the device a handle belongs to, closing,
+// and the step loop of the families that stop at cycle + 1 >= stop_cycle.  No device code.
 #pragma once
 
 #include <cstdio>
+#include <initializer_list>
 #include <new>
 #include <vector>
 
@@ -12,10 +13,89 @@
 struct fg_handle_base {
   std::vector<fg_class_t> classes;      // the descriptor's class table, copied (d.classes points here)
   fg_class_t *dev_classes = nullptr;    // its device copy (fg_upload_classes)
+  int device = -1;                      // the device current at create (fg_require_device); -1 before
   int64_t cycle = 0;
   int64_t launches = 0;
-  char err[512] = {0};
+  mutable char err[512] = {0};        // written by const readers too (fg_device_scope)
 };
+
+// Runs the rest of an entry point on the handle's device and gives the caller's device back on exit, so a handle
+// works whichever device the calling thread has current.  No-op for a null handle or one without a device yet.
+// A failed switch leaves ok false and its reason in the handle's err.
+struct fg_device_scope {
+  int prev = -1;
+  bool ok = true;
+  explicit fg_device_scope(const fg_handle_base *h) {
+    if (!h || h->device < 0) return;
+    int cur = 0;
+    cudaError_t e = cudaGetDevice(&cur);
+    if (e == cudaSuccess && cur == h->device) return;
+    if (e == cudaSuccess) e = cudaSetDevice(h->device);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      snprintf(h->err, sizeof(h->err), "cannot make the handle's device %d current: %s", h->device,
+               cudaGetErrorString(e));
+      ok = false;
+      return;
+    }
+    prev = cur;
+  }
+  ~fg_device_scope() {
+    if (prev >= 0) cudaSetDevice(prev);
+  }
+  fg_device_scope(const fg_device_scope &) = delete;
+  fg_device_scope &operator=(const fg_device_scope &) = delete;
+};
+
+#define FG_ON_DEVICE(h)                      \
+  fg_device_scope fg_device_scope_(h);       \
+  if (!fg_device_scope_.ok) return FG_ERR_CUDA
+
+// Where `p` lives, for messages: "device memory of device N", "pinned host memory", ...; *dev = the device of
+// device memory, else -1
+static inline const char *fg_memory_kind(const void *p, int *dev) {
+  cudaPointerAttributes a;
+  *dev = -1;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return "pageable host memory"; }
+  switch (a.type) {
+    case cudaMemoryTypeDevice: *dev = a.device; return "device memory";
+    case cudaMemoryTypeHost: return "pinned host memory";
+    case cudaMemoryTypeManaged: return "managed memory";
+    default: return "pageable host memory";
+  }
+}
+
+// true when `p` is device memory of the current device (the handle-less entry points' check of their main array)
+static inline bool fg_on_current_device(const void *p) {
+  int cur = 0, dev = -1;
+  if (cudaGetDevice(&cur) != cudaSuccess) { cudaGetLastError(); return false; }
+  fg_memory_kind(p, &dev);
+  return dev == cur;
+}
+
+struct fg_field {
+  const char *name;
+  const void *ptr;
+};
+#define FG_FIELD(d, x) fg_field{#x, (const void *)(d).x}
+
+// Every non-null array of a descriptor must be device memory of the handle's device: FG_ERR_ARG naming the first one
+// that is not, and where it lives.  After fg_require_device.
+static inline int fg_check_resident(fg_handle_base *h, std::initializer_list<fg_field> fields) {
+  for (const fg_field &f : fields) {
+    if (!f.ptr) continue;
+    int dev = -1;
+    const char *kind = fg_memory_kind(f.ptr, &dev);
+    if (dev == h->device) continue;
+    if (dev >= 0)
+      snprintf(h->err, sizeof(h->err), "%s is device memory of device %d, the handle belongs to device %d", f.name, dev,
+               h->device);
+    else
+      snprintf(h->err, sizeof(h->err), "%s is %s, not device memory of the handle's device %d", f.name, kind, h->device);
+    return FG_ERR_ARG;
+  }
+  return FG_OK;
+}
 
 static inline int check_class(const fg_class_t &c, char *err, size_t n) {
   if (c.arity < 1 || c.arity > FG_MAX_ARITY) { snprintf(err, n, "class arity %d out of range", c.arity); return FG_ERR_ARG; }
@@ -67,6 +147,7 @@ static inline int fg_require_device(fg_handle_base *h) {
     snprintf(h->err, sizeof(h->err), "no CUDA device visible: pydcop_b200 has no CPU fallback");
     return FG_ERR_CUDA;
   }
+  CUDA_TRY(h, cudaGetDevice(&h->device));   // the handle belongs to this device from now on
   return FG_OK;
 }
 
@@ -81,7 +162,10 @@ static inline int fg_upload_classes(fg_handle_base *h) {
 
 template <class H>
 static inline int fg_close(H *h) {
-  if (h && h->dev_classes) cudaFree(h->dev_classes);
+  {
+    fg_device_scope on(h);
+    if (h && h->dev_classes) cudaFree(h->dev_classes);
+  }
   delete h;
   return FG_OK;
 }
@@ -97,6 +181,7 @@ static inline bool fg_finished(const H *h) { return h->d.stop_cycle && h->cycle 
 template <class H>
 static inline int fg_current(const H *h, int64_t *cycle, int32_t *finished) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   if (cycle) *cycle = h->cycle;
   if (finished) *finished = fg_finished(h) ? 1 : 0;
   return FG_OK;
@@ -107,6 +192,7 @@ template <class H>
 static inline int fg_step(H *h, int32_t n_cycles, void *stream, int (*cycle_f32)(H *, cudaStream_t),
                           int (*cycle_f64)(H *, cudaStream_t)) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_cycles; ++i) {
     if (fg_finished(h)) break;

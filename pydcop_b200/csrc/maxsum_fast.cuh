@@ -841,20 +841,22 @@ inline void launch_f2v_tile(const fg_class_t &c, const fg_maxsum_desc_t &d, cons
   using C = F2VCfg<T, A, D>;
   auto kern = k_f2v_pipe<T, A, D, uint32_t>;
   using PP = F2VPipe<T, A, D>;
-  static int ctas_per_sm = 0, n_sm = 0;  // one per instantiation
-  if (!ctas_per_sm) {
+  struct Launch { int ctas_per_sm = 0, n_sm = 0; };
+  static std::vector<Launch> per_dev;  // one per instantiation and device
+  Launch &L = fg_per_device(per_dev);
+  if (!L.ctas_per_sm) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PP::SMEM);
     int dev = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, C::NT, PP::SMEM);
-    if (ctas_per_sm < 1) ctas_per_sm = 1;
+    cudaDeviceGetAttribute(&L.n_sm, cudaDevAttrMultiProcessorCount, dev);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&L.ctas_per_sm, kern, C::NT, PP::SMEM);
+    if (L.ctas_per_sm < 1) L.ctas_per_sm = 1;
     // the two sides of a cycle run concurrently on two streams: leave room for the other kernel
     const int cap = fg_env_int("PYDCOP_B200_F2V_CPS", 2);
-    if (ctas_per_sm > cap) ctas_per_sm = cap;
+    if (L.ctas_per_sm > cap) L.ctas_per_sm = cap;
   }
   const int n_tiles = (c.n_factors + C::NF - 1) / C::NF;
-  const unsigned blocks = (unsigned)min(n_tiles, n_sm * ctas_per_sm);
+  const unsigned blocks = (unsigned)min(n_tiles, L.n_sm * L.ctas_per_sm);
   kern<<<blocks, C::NT, PP::SMEM, st>>>(c, (const T *)d.dev_tables, q_cur, r_cur, r_next, d.dev_edge_qoff32, d.dev_r_cnt,
                                        d.dev_r_sent, p);
 }
@@ -966,23 +968,24 @@ template <typename T, int D>
 inline void launch_v2f_classes(const V2FLaunch &L, const fg_maxsum_desc_t &d, const T *r_cur, const T *q_cur, T *q_next,
                                const MaxSumParams &p, cudaStream_t st) {
   auto kern = k_v2f_pipe<T, D, uint32_t>;
-  static size_t attr_smem = 0;
-  static int n_sm = 0;
-  if (L.smem > attr_smem) {
+  struct Attr { size_t smem = 0; int n_sm = 0; };
+  static std::vector<Attr> per_dev;  // one per instantiation and device
+  Attr &A = fg_per_device(per_dev);
+  if (L.smem > A.smem) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem);
-    attr_smem = L.smem;
+    A.smem = L.smem;
   }
-  if (!n_sm) {
+  if (!A.n_sm) {
     int dev = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    cudaDeviceGetAttribute(&A.n_sm, cudaDevAttrMultiProcessorCount, dev);
   }
   int per_sm = 1;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, FG_V2F_NT, L.smem);
   if (per_sm < 1) per_sm = 1;
   static const int cap = fg_env_int("PYDCOP_B200_V2F_CPS", 3);
   if (per_sm > cap) per_sm = cap;
-  const unsigned blocks = (unsigned)std::min(L.tab.total_tiles, n_sm * per_sm);
+  const unsigned blocks = (unsigned)std::min(L.tab.total_tiles, A.n_sm * per_sm);
   kern<<<blocks, FG_V2F_NT, L.smem, st>>>(L.tab, d.dev_slot_roff32, (const T *)d.dev_unary, r_cur, q_cur, q_next,
                                           d.dev_q_cnt, d.dev_q_sent, d.dev_value, (T *)d.dev_value_cost, p);
 }

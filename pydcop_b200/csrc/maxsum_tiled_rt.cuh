@@ -48,9 +48,10 @@ inline int tiled_rt_pow2_ge(int d) { int g = 1; while (g < d && g < 32) g *= 2; 
 // costs more in index arithmetic and shuffles than the bank conflicts of a small table)
 constexpr int64_t FG_TILED_RT_WIDE = 2048;
 
-// SMs of the current device (queried once): the tile size spreads a class over about 6 tiles per SM
+// SMs of the current device (queried once per device): the tile size spreads a class over about 6 tiles per SM
 inline int tiled_rt_n_sm() {
-  static int n_sm = 0;
+  static std::vector<int> per_dev;
+  int &n_sm = fg_per_device(per_dev);
   if (!n_sm) {
     int dev = 0;
     cudaGetDevice(&dev);
@@ -340,11 +341,12 @@ k_f2v_tiled_rt(const fg_class_t *__restrict__ classes, const RtTile *__restrict_
 template <typename T, int A>
 inline int launch_f2v_tiled_rt(const TiledRtPlan &plan, const fg_maxsum_desc_t &d, const T *q_cur, const T *r_cur, T *r_next,
                                const MaxSumParams &p, cudaStream_t st) {
-  static bool attr_done = false;   // per instantiation
+  static std::vector<uint8_t> per_dev;   // per instantiation and device: the attribute is set
   int n = 0;
   for (int g = 0; g < 2; ++g) {
     const int t0 = plan.first_tile[2 * A + g], t1 = plan.first_tile[2 * A + g + 1];
     if (t1 <= t0) continue;
+    uint8_t &attr_done = fg_per_device(per_dev);
     if (!attr_done) {
       cudaFuncSetAttribute(k_f2v_tiled_rt<T, A>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FG_TILED_RT_SMEM_BIG);
       attr_done = true;

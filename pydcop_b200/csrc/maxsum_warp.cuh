@@ -441,24 +441,28 @@ inline bool launch_v2f_warp_ns(const WClassEntry *dev_classes, const WTileRange 
     return false;
   } else {
     auto kern = k_v2f_warp<T, D, NS_, MX, uint32_t>;
-    static int per_sm = 0, n_sm = 0;  // one per instantiation
-    if (!per_sm) {
+    struct Launch { int per_sm = 0, n_sm = 0; bool peer_attr = false; };
+    static std::vector<Launch> per_dev;  // one per instantiation and device
+    Launch &L = fg_per_device(per_dev);
+    if (!L.per_sm) {
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
       int dev = 0;
       cudaGetDevice(&dev);
-      cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, FG_V2FW_WARPS * 32, C::SMEM);
-      if (per_sm < 1) per_sm = 1;
+      cudaDeviceGetAttribute(&L.n_sm, cudaDevAttrMultiProcessorCount, dev);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&L.per_sm, kern, FG_V2FW_WARPS * 32, C::SMEM);
+      if (L.per_sm < 1) L.per_sm = 1;
       const int cap = fg_env_int("PYDCOP_B200_V2FW_CPS", 3);  // leaves room for the factor side (runs concurrently)
-      if (per_sm > cap) per_sm = cap;
+      if (L.per_sm > cap) L.per_sm = cap;
     }
     const int need = (rg.n_tiles + FG_V2FW_WARPS - 1) / FG_V2FW_WARPS;
-    const unsigned blocks = (unsigned)std::min(need, n_sm * per_sm);
+    const unsigned blocks = (unsigned)std::min(need, L.n_sm * L.per_sm);
     if constexpr (NS_ == 2) {   // fused halo: same kernel with the peer stores compiled in (default depth only)
       if (p.slot_dst != nullptr) {
         auto kp = k_v2f_warp<T, D, NS_, MX, uint32_t, true>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM); attr = true; }
+        if (!L.peer_attr) {
+          cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+          L.peer_attr = true;
+        }
         kp<<<blocks, FG_V2FW_WARPS * 32, C::SMEM, st>>>(dev_classes + rg.first, rg.count, rg.n_tiles, d.dev_slot_roff32,
                                                         (const T *)d.dev_unary, r_cur, q_cur, q_next, d.dev_q_cnt, d.dev_q_sent,
                                                         d.dev_value, (T *)d.dev_value_cost, p);
@@ -920,26 +924,30 @@ inline bool launch_f2v_warp_ns(bool probe, const fg_class_t &c, const TT *tables
   } else {
     if (probe) return true;
     auto kern = k_f2v_warp<T, TT, D, NS_, MX, uint32_t>;
-    static int per_sm = 0, n_sm = 0;  // one per instantiation
-    if (!per_sm) {
+    struct Launch { int per_sm = 0, n_sm = 0; bool peer_attr = false; };
+    static std::vector<Launch> per_dev;  // one per instantiation and device
+    Launch &L = fg_per_device(per_dev);
+    if (!L.per_sm) {
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
       int dev = 0;
       cudaGetDevice(&dev);
-      cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, C::WARPS * 32, C::SMEM);
-      if (per_sm < 1) per_sm = 1;
+      cudaDeviceGetAttribute(&L.n_sm, cudaDevAttrMultiProcessorCount, dev);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&L.per_sm, kern, C::WARPS * 32, C::SMEM);
+      if (L.per_sm < 1) L.per_sm = 1;
       // CTAs of 2 warps; the variable side shares the SMs
       const int cap = fg_env_int("PYDCOP_B200_F2VW_CPS", C::NARROW ? FG_F2VW8_CPS : 3);
-      if (per_sm > cap) per_sm = cap;
+      if (L.per_sm > cap) L.per_sm = cap;
     }
     const int n_tiles = (c.n_factors + C::NF - 1) / C::NF;
     const int need = (n_tiles + C::WARPS - 1) / C::WARPS;
-    const unsigned blocks = (unsigned)std::min(need, n_sm * per_sm);
+    const unsigned blocks = (unsigned)std::min(need, L.n_sm * L.per_sm);
     if (p.edge_dst != nullptr) {   // fused halo: only the PEER instantiation stores the boundary rows
       if constexpr (NS_ == FG_F2VW_PEER_NS(T, TT)) {
         auto kp = k_f2v_warp<T, TT, D, NS_, MX, uint32_t, true>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM); attr = true; }
+        if (!L.peer_attr) {
+          cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+          L.peer_attr = true;
+        }
         kp<<<blocks, C::WARPS * 32, C::SMEM, st>>>(c, tables, q_cur, r_cur, r_next, d.dev_edge_qoff32,
                                                   d.dev_r_cnt, d.dev_r_sent, p);
         return true;

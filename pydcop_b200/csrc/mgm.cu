@@ -34,6 +34,16 @@ extern "C" int fg_mgm_create(const fg_mgm_desc_t *desc, fg_mgm_t *out) {
     return FG_ERR_ARG;
   }
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  const fg_mgm_desc_t &d = *desc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_unary), FG_FIELD(d, dev_unary_off),
+                             FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_var_id), FG_FIELD(d, dev_var_rank),
+                             FG_FIELD(d, dev_edge_var), FG_FIELD(d, dev_edge_class), FG_FIELD(d, dev_var_ptr),
+                             FG_FIELD(d, dev_slot_edge), FG_FIELD(d, dev_nbr_ptr), FG_FIELD(d, dev_nbr_idx),
+                             FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_value), FG_FIELD(d, dev_cost),
+                             FG_FIELD(d, dev_has_cost), FG_FIELD(d, dev_gain), FG_FIELD(d, dev_new_value),
+                             FG_FIELD(d, dev_tables_or), FG_FIELD(d, dev_slot_nbr), FG_FIELD(d, dev_slot_tab),
+                             FG_FIELD(d, dev_row_cache), FG_FIELD(d, dev_slot_last)});
+  if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }
 
@@ -43,6 +53,7 @@ extern "C" const char *fg_mgm_last_error(fg_mgm_t h) { return fg_last_error(h); 
 
 extern "C" int fg_mgm_init(fg_mgm_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   const fg_mgm_desc_t &d = h->d;
   cudaStream_t st = (cudaStream_t)stream;
   if (d.n_vars) {

@@ -53,6 +53,17 @@ extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
     return FG_ERR_ARG;
   }
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  const fg_mgm2_desc_t &d = *desc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_var_id),
+                             FG_FIELD(d, dev_var_rank), FG_FIELD(d, dev_edge_var), FG_FIELD(d, dev_edge_class),
+                             FG_FIELD(d, dev_var_ptr), FG_FIELD(d, dev_slot_edge), FG_FIELD(d, dev_nbr_ptr),
+                             FG_FIELD(d, dev_nbr_idx), FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_value),
+                             FG_FIELD(d, dev_cost), FG_FIELD(d, dev_has_cost), FG_FIELD(d, dev_gain),
+                             FG_FIELD(d, dev_potential_value), FG_FIELD(d, dev_local_cost), FG_FIELD(d, dev_offerer),
+                             FG_FIELD(d, dev_partner), FG_FIELD(d, dev_committed), FG_FIELD(d, dev_go),
+                             FG_FIELD(d, dev_answer), FG_FIELD(d, dev_answer_value), FG_FIELD(d, dev_answer_gain),
+                             FG_FIELD(d, dev_offer_off), FG_FIELD(d, dev_offer)});
+  if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }
 
@@ -70,6 +81,7 @@ static void mgm2_init_t(fg_mgm2 *h, cudaStream_t st) {
 
 extern "C" int fg_mgm2_init(fg_mgm2_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
   const fg_mgm2_desc_t &d = h->d;
   cudaStream_t st = (cudaStream_t)stream;
   if (d.n_vars) {

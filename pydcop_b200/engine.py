@@ -123,8 +123,10 @@ class _EngineBase:
         return getattr(self.lib, f"fg_{self.FAMILY}_{name}")
 
     def _create(self, d):
+        """The handle over descriptor `d`; it belongs to self.device, which every later call makes current."""
         self._desc, self._h = d, C.c_void_p()
-        self._check(self._fn("create")(C.byref(d), C.byref(self._h)), f"fg_{self.FAMILY}_create")
+        with torch.cuda.device(self.device):
+            self._check(self._fn("create")(C.byref(d), C.byref(self._h)), f"fg_{self.FAMILY}_create")
 
     def _upload(self, inputs, state):
         """Every input of a host-array plan through _dev, in order (None stays None), then the state allocated on the
@@ -147,7 +149,8 @@ class _EngineBase:
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
-            self._fn("destroy")(self._h)
+            with torch.cuda.device(self.device):   # __del__ may run with any device current
+                self._fn("destroy")(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -237,11 +240,13 @@ class _CycleEngine(_EngineBase):
             self._check(self._fn("cycle_compute")(self._h, self._stream()), f"fg_{self.FAMILY}_cycle_compute")
 
     def cycle_commit(self):
-        self._check(self._fn("cycle_commit")(self._h), f"fg_{self.FAMILY}_cycle_commit")
+        with torch.cuda.device(self.device):
+            self._check(self._fn("cycle_commit")(self._h), f"fg_{self.FAMILY}_cycle_commit")
 
     def _current(self):
         b, c = C.c_int32(), C.c_int64()
-        self._fn("current")(self._h, C.byref(b), C.byref(c))
+        with torch.cuda.device(self.device):
+            self._fn("current")(self._h, C.byref(b), C.byref(c))
         return b.value, c.value
 
     @property
@@ -323,7 +328,8 @@ class MaxSumEngine(_CycleEngine):
         """Kernel family of every factor class (fg_maxsum_kernel_plan), as a list of names."""
         n = len(self.layout.classes)
         out = (C.c_int32 * max(n, 1))()
-        rc = self.lib.fg_maxsum_kernel_plan(self._h, out, n)
+        with torch.cuda.device(self.device):
+            rc = self.lib.fg_maxsum_kernel_plan(self._h, out, n)
         if rc != 0:
             raise EngineError(f"fg_maxsum_kernel_plan rc={rc}")
         return [self.KERNEL_FAMILIES[int(out[i])] for i in range(n)]
@@ -333,7 +339,8 @@ class MaxSumEngine(_CycleEngine):
         1 where the warp kernel reads the engine's 8-bit copy of integer tables, else 4 (f32) or 8 (f64)."""
         n = len(self.layout.classes)
         out = (C.c_int32 * max(n, 1))()
-        rc = self.lib.fg_maxsum_table_width(self._h, out, n)
+        with torch.cuda.device(self.device):
+            rc = self.lib.fg_maxsum_table_width(self._h, out, n)
         if rc != 0:
             raise EngineError(f"fg_maxsum_table_width rc={rc}")
         return [int(out[i]) for i in range(n)]
@@ -612,7 +619,8 @@ class _LocalSearchEngine(_EngineBase):
 
     def _current(self):
         c, f = C.c_int64(), C.c_int32()
-        self._fn("current")(self._h, C.byref(c), C.byref(f))
+        with torch.cuda.device(self.device):
+            self._fn("current")(self._h, C.byref(c), C.byref(f))
         return c.value, bool(f.value)
 
     @property

@@ -582,28 +582,32 @@ class ShardedMaxSum:
         def stream():
             return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
+        # the halo kernels run on the current device: make it the shard's (shards of one process may be on several)
         def pack(src, packed, row_off, packed_off, row_len, n):
-            rc = lib.fg_halo_pack(prec, C.c_void_p(src.data_ptr()), C.c_void_p(packed.data_ptr()),
-                                  C.c_void_p(row_off.data_ptr()), C.c_void_p(packed_off.data_ptr()),
-                                  C.c_void_p(row_len.data_ptr()), n, stream())
+            with torch.cuda.device(self.device):
+                rc = lib.fg_halo_pack(prec, C.c_void_p(src.data_ptr()), C.c_void_p(packed.data_ptr()),
+                                      C.c_void_p(row_off.data_ptr()), C.c_void_p(packed_off.data_ptr()),
+                                      C.c_void_p(row_len.data_ptr()), n, stream())
             if rc != _cabi.FG_OK:
                 raise _cabi.EngineError(f"fg_halo_pack failed rc={rc}")
 
         def unpack(dst, packed, row_off, packed_off, row_len, n):
-            rc = lib.fg_halo_unpack(prec, C.c_void_p(dst.data_ptr()), C.c_void_p(packed.data_ptr()),
-                                    C.c_void_p(row_off.data_ptr()), C.c_void_p(packed_off.data_ptr()),
-                                    C.c_void_p(row_len.data_ptr()), n, stream())
+            with torch.cuda.device(self.device):
+                rc = lib.fg_halo_unpack(prec, C.c_void_p(dst.data_ptr()), C.c_void_p(packed.data_ptr()),
+                                        C.c_void_p(row_off.data_ptr()), C.c_void_p(packed_off.data_ptr()),
+                                        C.c_void_p(row_len.data_ptr()), n, stream())
             if rc != _cabi.FG_OK:
                 raise _cabi.EngineError(f"fg_halo_unpack failed rc={rc}")
 
         self.halo = HaloExchange(self.plan, tdt, self.device, pack, unpack, group)
 
         def fused(is_pack, r, q, packed, off_r, off_q, n_r, n_q, dom, n_peers, pr, pq, pb):
-            rc = lib.fg_halo_rows_uniform(prec, is_pack, C.c_void_p(r.data_ptr()), C.c_void_p(q.data_ptr()),
-                                          C.c_void_p(packed.data_ptr()), C.c_void_p(off_r.data_ptr()),
-                                          C.c_void_p(off_q.data_ptr()), n_r, n_q, dom, n_peers,
-                                          C.cast(pr, C.c_void_p), C.cast(pq, C.c_void_p),
-                                          C.cast(pb, C.c_void_p), stream())
+            with torch.cuda.device(self.device):
+                rc = lib.fg_halo_rows_uniform(prec, is_pack, C.c_void_p(r.data_ptr()), C.c_void_p(q.data_ptr()),
+                                              C.c_void_p(packed.data_ptr()), C.c_void_p(off_r.data_ptr()),
+                                              C.c_void_p(off_q.data_ptr()), n_r, n_q, dom, n_peers,
+                                              C.cast(pr, C.c_void_p), C.cast(pq, C.c_void_p),
+                                              C.cast(pb, C.c_void_p), stream())
             if rc != _cabi.FG_OK:
                 raise _cabi.EngineError(f"fg_halo_rows_uniform failed rc={rc}")
 

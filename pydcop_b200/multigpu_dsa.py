@@ -308,11 +308,13 @@ class ShardedDsa:
             def stream():
                 return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
+            # the halo kernels run on the current device: make it the shard's (shards of one process may be on several)
             def mover(fn, name):
                 def move(buf, packed, row_off, packed_off, row_len, n):
-                    rc = fn(_cabi.FG_F32, C.c_void_p(buf.data_ptr()), C.c_void_p(packed.data_ptr()),
-                            C.c_void_p(row_off.data_ptr()), C.c_void_p(packed_off.data_ptr()),
-                            C.c_void_p(row_len.data_ptr()), n, stream())
+                    with torch.cuda.device(self.device):
+                        rc = fn(_cabi.FG_F32, C.c_void_p(buf.data_ptr()), C.c_void_p(packed.data_ptr()),
+                                C.c_void_p(row_off.data_ptr()), C.c_void_p(packed_off.data_ptr()),
+                                C.c_void_p(row_len.data_ptr()), n, stream())
                     if rc != _cabi.FG_OK:
                         raise _cabi.EngineError(f"{name} failed rc={rc}")
                 return move
