@@ -698,6 +698,65 @@ int fg_dba_step(fg_dba_t h, int32_t n_cycles, void *stream);
 int fg_dba_current(fg_dba_t h, int64_t *cycle, int32_t *finished);
 int64_t fg_dba_launch_count(fg_dba_t h);
 
+/* ------------------------------------------------------------------------------------------
+ * SyncBB  (pydcop/algorithms/syncbb.py: synchronous branch and bound over the variables sorted by
+ * name, ordered_graph.py:173).  The search is a token walk: one message is in flight at any time.
+ * ONE CTA runs the whole search, message after message, and leaves every piece of state in the
+ * caller's arrays, so a run may be split into launches anywhere with the same result.
+ * Everything is indexed by CHAIN POSITION p (the variable's rank in name order).  The path is always
+ * a prefix of the chain: path element q is (chain variable q, dev_path_val[q], dev_path_cost[q]).
+ * Per step, threads cover the candidates of the receiver; each sums its candidate's path elements
+ * sequentially in path order (get_next_assignment, :415-473):
+ *   ass(q) = dev_pair[dev_elt_tab[k] + val_q * dom(p) + x] for the earlier neighbour at q (slot k),
+ *            0 for any other element
+ *   min mode: element q fails when cc + ass >= ub(p) or ass + path_cost(q) >= ub(p); a candidate
+ *            is rejected iff its FIRST element fails, else accepted with cc up to the last passing
+ *            element.  Max mode accepts every candidate with its full sum.
+ * A block reduction picks the first accepted candidate, or at the last variable the first strict
+ * best of psum + cost (psum = the path's costs summed as CPython's sum() does, Neumaier-compensated,
+ * kept per prefix in dev_path_sum / dev_path_comp).  Unary constraints and variable costs are not
+ * part of the plan (SyncBB never reads them); constraints of arity > 2 are refused by the host.
+ * dev_msg = {type (0 forward, 1 backward, 2 terminate), receiver, path length, finished}.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t abi_version, precision;
+  int32_t n_vars;                 /* chain length, >= 2 */
+  int32_t mode_max;
+  const int32_t *dev_dom;         /* [n_vars] domain size per chain position, 1..FG_MAX_DOM; the kernel covers
+                                     FG_MAX_DOM candidates per step and cannot check these device values, so a
+                                     larger domain is undefined behaviour (SyncbbEngine's layout refuses it) */
+  const int32_t *dev_elt_ptr;     /* [n_vars+1] earlier neighbours of chain position p */
+  const int32_t *dev_elt_pos;     /* [n_elts] their chain positions, ascending within p */
+  const int64_t *dev_elt_tab;     /* [n_elts] first entry of the pair table [val_u][x] in dev_pair */
+  const void *dev_pair;           /* T[n_pair] every binary constraint between p and u summed from 0 in
+                                     node.constraints order */
+  void *dev_ub;                   /* T[n_vars] per-variable upper_bound */
+  int32_t *dev_sel;               /* [n_vars] last value_selection, -1 before any */
+  int32_t *dev_path_val;          /* [n_vars] */
+  void *dev_path_cost;            /* T[n_vars] */
+  void *dev_path_sum;             /* T[n_vars] compensated prefix sum of path_cost[0..q] */
+  void *dev_path_comp;            /* T[n_vars] its compensation */
+  int32_t *dev_msg;               /* [4] */
+  void *dev_msg_ub;               /* T[1] bound carried by the message in flight */
+  int64_t *dev_count;             /* [2] steps (messages delivered), messages posted */
+  int64_t *dev_cycles;            /* [n_vars] the reference's new_cycle count per variable: messages received,
+                                     plus one for the first variable's start (syncbb.py:211) */
+  int64_t n_elts, n_pair;
+} fg_syncbb_desc_t;
+
+typedef struct fg_syncbb *fg_syncbb_t;
+
+int fg_syncbb_create(const fg_syncbb_desc_t *desc, fg_syncbb_t *out);
+int fg_syncbb_destroy(fg_syncbb_t h);
+const char *fg_syncbb_last_error(fg_syncbb_t h);
+/* bounds +-inf, no selection, the first variable's start message [(x0, 0, 0)] to chain position 1. */
+int fg_syncbb_init(fg_syncbb_t h, void *stream);
+/* one launch delivering up to n_steps messages; none once the last terminate message is delivered. */
+int fg_syncbb_step(fg_syncbb_t h, int64_t n_steps, void *stream);
+/* waits for the work already enqueued. */
+int fg_syncbb_current(fg_syncbb_t h, int64_t *steps, int64_t *messages, int32_t *finished);
+int64_t fg_syncbb_launch_count(fg_syncbb_t h);
+
 /* Solution cost (next-tier row §8f.1; pydcop/dcop/dcop.py:319-367 `solution_cost`, called by the
  * orchestrator at the end of a run and at every metric tick, orchestrator.py:1229-1231): over the factors
  * of every non-ghost class the table entry at the assignment, over the first n_vars variables

@@ -154,6 +154,14 @@ class FgDbaDesc(C.Structure):
                 ("reserved0", C.c_int32), ("seed", C.c_uint64)]
 
 
+class FgSyncbbDesc(C.Structure):
+    _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32), ("n_vars", C.c_int32), ("mode_max", C.c_int32),
+                ("dev_dom", P), ("dev_elt_ptr", P), ("dev_elt_pos", P), ("dev_elt_tab", P), ("dev_pair", P),
+                ("dev_ub", P), ("dev_sel", P), ("dev_path_val", P), ("dev_path_cost", P), ("dev_path_sum", P),
+                ("dev_path_comp", P), ("dev_msg", P), ("dev_msg_ub", P), ("dev_count", P),
+                ("dev_cycles", P), ("n_elts", C.c_int64), ("n_pair", C.c_int64)]
+
+
 GDBA_MODIFIERS = {"A": 0, "M": 1}
 GDBA_VIOLATIONS = {"NZ": 0, "NM": 1, "MX": 2}
 GDBA_INCREASE_MODES = {"E": 0, "R": 1, "C": 2, "T": 3}
@@ -248,6 +256,13 @@ SYMBOLS = {
     "fg_dba_step": (C.c_int, [P, C.c_int32, P]),
     "fg_dba_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "fg_dba_launch_count": (C.c_int64, [P]),
+    "fg_syncbb_create": (C.c_int, [C.POINTER(FgSyncbbDesc), C.POINTER(P)]),
+    "fg_syncbb_destroy": (C.c_int, [P]),
+    "fg_syncbb_last_error": (C.c_char_p, [P]),
+    "fg_syncbb_init": (C.c_int, [P, P]),
+    "fg_syncbb_step": (C.c_int, [P, C.c_int64, P]),
+    "fg_syncbb_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "fg_syncbb_launch_count": (C.c_int64, [P]),
     "fg_dpop_create": (C.c_int, [C.POINTER(FgDpopDesc), C.POINTER(P)]),
     "fg_dpop_destroy": (C.c_int, [P]),
     "fg_dpop_last_error": (C.c_char_p, [P]),

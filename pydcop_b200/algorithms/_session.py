@@ -37,12 +37,13 @@ def tabulate(constraint, cache=None) -> np.ndarray:
 
 
 class Snapshot:
-    """`finished`: every proxy reports finished; `done`: the variables that finished on their own (DBA)."""
-    __slots__ = ("cycle", "values", "costs", "finished", "done")
+    """`finished`: every proxy reports finished; `done`: the variables that finished on their own (DBA);
+    `cycles`: name -> the variable's own cycle count (SyncBB)."""
+    __slots__ = ("cycle", "values", "costs", "finished", "done", "cycles")
 
-    def __init__(self, cycle, values, costs, finished, done=frozenset()):
+    def __init__(self, cycle, values, costs, finished, done=frozenset(), cycles=None):
         self.cycle, self.values, self.costs, self.finished = cycle, values, costs, finished
-        self.done = done
+        self.done, self.cycles = done, cycles
 
 
 class GpuSession:
@@ -258,6 +259,8 @@ class GpuSession:
                         [rnd.uniform(0, noise) for _ in range(len(inst["unary"]))])
             elif self.kind == "dpop":
                 inst["tree"] = self._pseudo_tree(inst)
+            elif self.kind == "syncbb":   # name order is the chain: no start values to work out
+                pass
             else:
                 inst["isolated_value"] = self._isolated_values(inst)
             layout = build_layout(**{k: v for k, v in inst.items() if k not in ("isolated_value", "tree")})
@@ -267,6 +270,15 @@ class GpuSession:
             cycle = 0
             self._publish(engine, cycle, False)
             while not self.closed and not self.all_stopped():
+                if self.kind == "syncbb":   # a message per step: launches of SYNCBB_CHUNK until the search ends
+                    from ..solve import SYNCBB_CHUNK
+                    engine.step(SYNCBB_CHUNK)
+                    done = bool(engine.finished)
+                    self._publish(engine, engine.cycle, done)
+                    if done:
+                        break
+                    time.sleep(0)
+                    continue
                 n = self.cycles_per_poll
                 if stop_cycle:
                     n = min(n, stop_cycle - cycle)
@@ -304,14 +316,22 @@ class GpuSession:
         else:
             idx, costs = out, None
         vals = {}
+        if self.kind == "syncbb":      # last value selection and the bound it came with; (None, None): never selected
+            costs = engine.bounds()
         for i, n in enumerate(self.var_order):
             dom = domain_values(self.variables[n])
+            if idx[i] < 0:
+                vals[n] = (None, None)
+                continue
             vals[n] = (dom[int(idx[i])], float(costs[i]) if costs is not None else 0.0)
         done = frozenset()
         if self.kind == "dba":
             fin = engine.finished_vars()
             done = frozenset(n for i, n in enumerate(self.var_order) if fin[i])
-        self.snapshot = Snapshot(cycle, vals, None, finished, done)
+        cycles = None
+        if self.kind == "syncbb":
+            cycles = dict(zip(self.var_order, (int(c) for c in engine.cycle_counts())))
+        self.snapshot = Snapshot(cycle, vals, None, finished, done, cycles)
 
     def _pseudo_tree(self, inst):
         """The orchestrator's pseudo-tree over the packed arrays; each node joins the constraints it owns

@@ -1163,6 +1163,163 @@ class DpopEngine(_EngineBase):
                 .contiguous() if L.n_vars else self.value)
 
 
+def syncbb_plan(layout: FactorGraphLayout, precision="f64", mode="min", var_rank=None, factor_names=None):
+    """SyncbbEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan, in CHAIN order (the
+    variables sorted by name, `var_rank`; default: the canonical index).  Per chain position p: its earlier
+    neighbours sorted by chain position, and per (p, neighbour u) one pair table laid out [val_u][x], every binary
+    constraint of p on u added from 0 in node.constraints order in the tables' precision (relations.py:1513-1530 sums
+    the same terms in that order).  Unary constraints and variable costs are not part of the plan (syncbb.py reads
+    neither); a constraint of arity > 2 raises ValueError naming it (`factor_names`: canonical factor names)."""
+    L = layout
+    dt = PRECISIONS[precision][2]
+    V = L.n_vars
+    if V < 2:
+        raise ValueError(f"SyncBB needs at least two variables, got {V}: with one, the reference's first variable "
+                         "posts its start message to no next variable (syncbb.py:210) and never finishes")
+    if mode not in ("min", "max"):
+        raise ValueError(f"invalid mode {mode!r}")
+    rank = np.arange(V) if var_rank is None else np.asarray(var_rank, dtype=np.int64)
+    chain = np.argsort(rank, kind="stable")
+    pos = np.empty(V, dtype=np.int64)
+    pos[chain] = np.arange(V)
+    inv_factor = np.empty(L.n_factors, dtype=np.int64)
+    inv_factor[L.factor_perm] = np.arange(L.n_factors)
+    for c in L.classes:
+        if c.arity > 2:
+            f = int(inv_factor[c.first_factor])
+            name = factor_names[f] if factor_names is not None else f"#{f}"
+            raise ValueError(f"constraint {name} has arity {c.arity}: SyncBB supports binary constraints only "
+                             "(syncbb.py:456)")
+    edge_class = np.asarray(L.edge_class)
+    pair = {}                                   # (p, q) -> [val_u][x] table
+    for v in range(V):
+        p = int(pos[v])
+        for e in L.canon_var_edge[L.canon_var_ptr[v]:L.canon_var_ptr[v + 1]]:   # node.constraints order
+            ie = int(L.edge_perm[e])
+            c = L.classes[int(edge_class[ie])]
+            if c.arity != 2:
+                continue
+            fl, j = divmod(ie - c.first_edge, 2)
+            u = int(L.var_order[L.edge_var[c.first_edge + 2 * fl + 1 - j]])
+            q = int(pos[u])
+            if q >= p:
+                continue
+            t = np.asarray(L.tables[c.table_base + fl * c.table_size:c.table_base + (fl + 1) * c.table_size],
+                           dtype=dt).reshape(c.dom[0], c.dom[1])
+            t = t.T if j == 0 else t            # [val_u][x]
+            pair[(p, q)] = (pair.get((p, q), dt(0)) + t).astype(dt)
+    keys = sorted(pair)
+    elt_ptr = np.zeros(V + 1, dtype=np.int32)
+    np.add.at(elt_ptr, np.array([k[0] + 1 for k in keys], dtype=np.int64), 1)
+    elt_ptr = np.cumsum(elt_ptr).astype(np.int32)
+    sizes = np.array([pair[k].size for k in keys], dtype=np.int64)
+    elt_tab = np.concatenate([[0], np.cumsum(sizes)])[:-1].astype(np.int64)
+    tabs = np.concatenate([pair[k].reshape(-1) for k in keys]).astype(dt) if keys else np.zeros(0, dt)
+    dom = np.asarray(L.canon_dom_size, dtype=np.int32)[chain]
+    inputs = dict(dom=dom, elt_ptr=elt_ptr, elt_pos=np.array([k[1] for k in keys], dtype=np.int32),
+                  elt_tab=elt_tab, pair=tabs)
+    state = dict(ub=(V, dt, None), sel=(V, np.int32, None), path_val=(V, np.int32, None),
+                 path_cost=(V, dt, None), path_sum=(V, dt, None), path_comp=(V, dt, None),
+                 msg=(4, np.int32, 0), msg_ub=(1, dt, None), count=(2, np.int64, 0), cycles=(V, np.int64, None))
+    return inputs, state, dict(n_vars=V, mode_max=int(mode == "max"), n_elts=len(keys), n_pair=int(tabs.size))
+
+
+SYNCBB_TYPES = ("forward", "backward", "terminate")
+
+
+class SyncbbEngine(_EngineBase):
+    """SyncBB (pydcop/algorithms/syncbb.py): the whole branch-and-bound search in one resident CTA, one message per
+    step (forward, backward or terminate).  `step(n)` enqueues one launch that delivers up to n messages; the state
+    stays on the device, so a run may be split anywhere.  `finished` once the last variable received its terminate
+    message; `values()` is each variable's last value selection (-1 for one that never selected).
+
+    var_rank      position of each variable's NAME in sorted order: the chain (default: the canonical index)
+    factor_names  canonical constraint names, for the arity error
+    """
+    FAMILY = "syncbb"
+
+    def __init__(self, layout: FactorGraphLayout, device=None, precision="f64", mode="min", var_rank=None,
+                 factor_names=None):
+        L = layout
+        inputs, state, scalars = syncbb_plan(L, precision, mode, var_rank, factor_names)
+        self._open(layout, device, precision)
+        self.mode = mode
+        self.chain = np.argsort(np.arange(L.n_vars) if var_rank is None else np.asarray(var_rank), kind="stable")
+        self.dev = self._upload(inputs, state)
+        self._classes = _class_array(L)
+        d = _cabi.FgSyncbbDesc()
+        d.abi_version, d.precision = _cabi.FG_ABI_VERSION, PRECISIONS[precision][0]
+        self._create(fill_desc(d, self.dev, scalars))
+
+    def step(self, n_steps=1):
+        with torch.cuda.device(self.device):
+            self._check(self.lib.fg_syncbb_step(self._h, int(n_steps), self._stream()), "fg_syncbb_step")
+        return self
+
+    def _current(self):
+        s, m, f = C.c_int64(), C.c_int64(), C.c_int32()
+        with torch.cuda.device(self.device):
+            self._check(self.lib.fg_syncbb_current(self._h, C.byref(s), C.byref(m), C.byref(f)), "fg_syncbb_current")
+        return s.value, m.value, bool(f.value)
+
+    @property
+    def steps(self):
+        """Messages delivered."""
+        return self._current()[0]
+
+    @property
+    def messages(self):
+        """Messages posted: forward, backward and terminate, the first variable's start message included."""
+        return self._current()[1]
+
+    @property
+    def finished(self):
+        return self._current()[2]
+
+    @property
+    def cycle(self):
+        """What the reference's orchestrated run reports as `cycle`: the largest per-variable new_cycle count
+        (orchestrator.py:1243-1258 over agents.py:733)."""
+        return int(self.dev["cycles"][:self.layout.n_vars].max().item())
+
+    def cycle_counts(self):
+        """Each variable's new_cycle count (messages it received, plus one for the first variable's start),
+        canonical order."""
+        return self._canonical(self.dev["cycles"][:self.layout.n_vars].cpu().numpy())
+
+    def _canonical(self, a):
+        out = np.empty_like(a)
+        out[self.chain] = a
+        return out
+
+    def values(self):
+        """Each variable's last value selection (domain index, -1: none), canonical order."""
+        return self._canonical(self.dev["sel"][:self.layout.n_vars].cpu().numpy())
+
+    def bounds(self):
+        """Each variable's upper_bound, canonical order."""
+        return self._canonical(self.dev["ub"][:self.layout.n_vars].cpu().numpy())
+
+    def message(self):
+        """The message in flight: (type 0 forward / 1 backward / 2 terminate, receiver as canonical index, path
+        length, bound carried, finished)."""
+        m = self.dev["msg"].cpu().numpy()
+        return int(m[0]), int(self.chain[m[1]]), int(m[2]), self.dev["msg_ub"][0].item(), bool(m[3])
+
+    def _assignment(self):
+        """The canonical-order values in the layout's internal order (a variable without a value reads 0)."""
+        L = self.layout
+        canon = torch.as_tensor(np.maximum(self.values(), 0).astype(np.int32), device=self.device)
+        return canon[torch.as_tensor(L.var_order.astype(np.int64), device=self.device)].contiguous()
+
+    @property
+    def tables(self):
+        """The full tables, uploaded on first use: only the solution cost reads them."""
+        if not hasattr(self, "_tables"):
+            self._tables = self._dev(self.layout.tables, PRECISIONS[self.precision][1])
+        return self._tables
+
+
 def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precision="f32", device=None, seed=0,
                 var_rank=None, isolated_value=None, tree=None):
     """The single-GPU engine of algorithm `kind` (a value of solve.ALGOS) over `layout`.  `params`: its algorithm
@@ -1170,6 +1327,8 @@ def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precisio
     take them (var_rank None: the canonical index); tree: DPOP's pseudo-tree.  MaxSum records no sent flags."""
     from .solve import DEFAULTS
     p = dict(DEFAULTS[kind], **params)
+    if kind == "syncbb":
+        return SyncbbEngine(layout, device=device, precision=precision, mode=mode, var_rank=var_rank)
     if kind == "dba":
         return DbaEngine(layout, device=device, precision=precision, mode=mode, infinity=p["infinity"],
                          max_distance=p["max_distance"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank)

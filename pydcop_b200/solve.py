@@ -1,5 +1,5 @@
 """Direct solve: a DCOP file (or arrays, or a pyDcop DCOP object) -> GPU engine -> result dict
-(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba, dpop, dba).
+(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba, dpop, dba, syncbb).
 
 The plugin modules (pydcop_b200/algorithms/) keep pyDcop's orchestrator, agents and one Python
 computation object per graph node around the engine — that is the drop-in path, and it is what
@@ -20,6 +20,14 @@ cycle 0.
 DBA (dba.py:265-268, plus `stop_cycle` with GDBA's convention) stops by itself once every variable with
 neighbours has finished (its termination counter reached `max_distance`, or an End message arrived): the loop
 then leaves early and reports the engine's cycle with status FINISHED.  DBA minimises only.
+SyncBB (syncbb.py) takes no parameters and stops by itself: the loop enqueues launches of SYNCBB_CHUNK messages until
+the last terminate message is delivered (FINISHED), or until the timeout (TIMEOUT, with the bounds and selections
+reached so far).  `cycle` is the largest per-variable new_cycle count (messages a variable handled, plus one for the
+first variable's start), which is what the reference's orchestrated run reports; `msg_count` is the number of SyncBB
+messages posted (forward, backward, terminate and the start message).  The orchestrated run's msg_count also counts
+the orchestrator's own traffic, which a direct run has none of.  A
+variable that never selected a value is left out of the assignment and cost / violation are then None, as the
+orchestrator reports an incomplete assignment (orchestrator.py:1226-1240).
 
 No CPU path: the engines raise EngineError without a CUDA device.  `engine_factory` exists so
 the host logic can be tested without one.
@@ -43,7 +51,7 @@ MGM2_DEFAULTS = {"threshold": 0.5, "favor": "unilateral", "stop_cycle": 0}
 GDBA_DEFAULTS = {"modifier": "A", "violation": "NZ", "increase_mode": "E", "stop_cycle": 0}
 DBA_DEFAULTS = {"infinity": 10000, "max_distance": 50, "stop_cycle": 0}
 DEFAULTS = {"maxsum": MAXSUM_DEFAULTS, "dsa": DSA_DEFAULTS, "mgm": MGM_DEFAULTS, "adsa": ADSA_DEFAULTS,
-            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS, "dpop": {}, "dba": DBA_DEFAULTS}
+            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS, "dpop": {}, "dba": DBA_DEFAULTS, "syncbb": {}}
 _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "start_messages": ("leafs", "leafs_vars", "all"),
             "p_mode": ("fixed", "arity"), "variant": ("A", "B", "C"),
@@ -51,7 +59,9 @@ _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "modifier": ("A", "M"), "violation": ("NZ", "NM", "MX"), "increase_mode": ("E", "R", "C", "T")}
 ALGOS = {"maxsum": "maxsum", "maxsum_gpu": "maxsum", "dsa": "dsa", "dsa_gpu": "dsa",
          "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa", "mgm2": "mgm2", "mgm2_gpu": "mgm2",
-         "gdba": "gdba", "gdba_gpu": "gdba", "dpop": "dpop", "dpop_gpu": "dpop", "dba": "dba", "dba_gpu": "dba"}
+         "gdba": "gdba", "gdba_gpu": "gdba", "dpop": "dpop", "dpop_gpu": "dpop", "dba": "dba", "dba_gpu": "dba",
+         "syncbb": "syncbb", "syncbb_gpu": "syncbb"}
+SYNCBB_CHUNK = 1 << 16   # SyncBB messages per launch: the timeout is checked between launches
 
 
 def check_params(kind: str, params: Optional[Dict[str, Any]]) -> Dict[str, Any]:
@@ -156,7 +166,7 @@ def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
     else:
         if kind not in ("mgm2", "dba"):
             isolated_value = isolated_values(dcop, mode)
-        if kind in ("mgm", "mgm2", "gdba", "dba"):
+        if kind in ("mgm", "mgm2", "gdba", "dba", "syncbb"):
             var_rank = name_rank(dcop)
     return make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=seed or 0,
                        var_rank=var_rank, isolated_value=isolated_value, tree=tree)
@@ -170,9 +180,9 @@ def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, par
     import torch.distributed as dist
     from .multigpu import ShardedMaxSum, broadcast_owner
     from .multigpu_dsa import ShardedDsa
-    rank, world = dist.get_rank(), dist.get_world_size()
-    if kind in ("mgm", "mgm2", "gdba", "dpop", "dba"):
+    if kind in ("mgm", "mgm2", "gdba", "dpop", "dba", "syncbb"):
         raise ValueError(f"{kind} is not sharded: run it on one GPU")
+    rank, world = dist.get_rank(), dist.get_world_size()
     kw = dict(sharded_kwargs or {})
     dev = device if device is not None else (torch.device("cuda", torch.cuda.current_device())
                                              if torch.cuda.is_available() and "engine_factory" not in kw
@@ -211,20 +221,23 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     noise).
 
     problem      see `load`
-    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba | dpop | dba (the *_gpu spellings of the plugin modules are
+    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba | dpop | dba | syncbb (the *_gpu spellings of the plugin modules are
                  accepted)
     algo_params  the reference's parameter names; `stop_cycle` bounds the run in cycles
-    timeout      wall-clock bound in seconds (checked every `chunk` cycles)
+    timeout      wall-clock bound in seconds (checked every `chunk` cycles; SyncBB: between launches of
+                 SYNCBB_CHUNK messages)
     precision    f32 | f64 (f64 reproduces the reference's double arithmetic bit for bit)
     seed         MaxSum: the U(0, noise) draws; DSA: the Philox stream of the random choices
     on_cycle     callback(cycle, value_index) after every chunk (metrics collection)
+    SyncBB has no cycles to chunk: it ignores `chunk` and never calls `on_cycle` (a variable may have no value
+    until the search ends).
     """
     if algo not in ALGOS:
         raise ValueError(f"unknown algorithm {algo!r}: expected one of {sorted(ALGOS)}")
     kind = ALGOS[algo]
     params = check_params(kind, algo_params)
-    stop_cycle = 1 if kind == "dpop" else int(params["stop_cycle"])   # DPOP: both phases in one step
-    if not stop_cycle and timeout is None:
+    stop_cycle = 1 if kind == "dpop" else 0 if kind == "syncbb" else int(params["stop_cycle"])   # DPOP: both phases in one step
+    if not stop_cycle and timeout is None and kind != "syncbb":
         raise ValueError(f"{kind} does not stop by itself: give algo_params['stop_cycle'] or a timeout")
     if distributed is None:
         try:
@@ -240,6 +253,12 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     if kind == "dba" and mode != "min":
         from .engine import DBA_MODE_ERROR
         raise ValueError(DBA_MODE_ERROR)
+    if kind == "syncbb":                   # before any device work: assignment_cost raises on such a constraint
+        arity = np.diff(np.asarray(dcop.arrays["factor_ptr"], dtype=np.int64))
+        big = np.nonzero(arity > 2)[0]
+        if len(big):
+            raise ValueError(f"constraint {dcop.con_names[int(big[0])]} has arity {int(arity[big[0]])}: SyncBB "
+                             "supports binary constraints only (syncbb.py:456)")
     inst = dcop.instance()
     if kind == "maxsum":
         inst["unary"] = ingest.add_noise(inst["unary"], params["noise"], seed)
@@ -260,6 +279,8 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     engine.init()
     cycle, status = 0, "FINISHED"
     deadline = None if timeout is None else t0 + float(timeout)
+    if kind == "syncbb":
+        return _finish_syncbb(engine, dcop, deadline, infinity, precision, t0, t_packed)
     while True:
         n = chunk if not stop_cycle else min(chunk, stop_cycle - cycle)
         if n <= 0:
@@ -294,6 +315,31 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
             # bytes this process moved host -> device (problem arrays) and device -> host (assignment, costs)
             "h2d_bytes": int(getattr(getattr(engine, "engine", engine), "h2d_bytes", 0)),
             "d2h_bytes": int(len(idx) * 12 + 16)}
+
+
+def _finish_syncbb(engine, dcop, deadline, infinity, precision, t0, t_packed):
+    status = "FINISHED"
+    while not engine.finished:
+        if deadline is not None and time.perf_counter() >= deadline:
+            status = "TIMEOUT"
+            break
+        engine.step(SYNCBB_CHUNK)
+    idx = _indices(engine)
+    has = idx >= 0
+    if has.all():
+        if hasattr(engine, "_solution_cost"):
+            cost, violation = engine.solution_cost(infinity, dcop.arrays["unary"])
+        else:                              # engine seam of the CPU tests
+            violation, cost = solution_cost(dcop, idx, infinity)
+    else:                                  # incomplete assignment (orchestrator.py:1226-1240)
+        cost = violation = None
+    full = dcop.assignment(np.maximum(idx, 0))
+    names = list(full)
+    assignment = {names[i]: full[names[i]] for i in range(len(names)) if has[i]}
+    return {"status": status, "assignment": assignment, "cost": cost, "violation": violation,
+            "time": time.perf_counter() - t0, "cycle": engine.cycle, "msg_count": int(engine.messages),
+            "msg_size": 0, "algo": "syncbb", "precision": precision, "n_gpus": 1, "ingest_time": t_packed - t0,
+            "h2d_bytes": int(getattr(engine, "h2d_bytes", 0)), "d2h_bytes": int(len(idx) * 12 + 16)}
 
 
 def _indices(engine) -> np.ndarray:
