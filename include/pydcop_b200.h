@@ -773,6 +773,13 @@ int fg_solution_cost(int32_t precision, int32_t n_classes, const fg_class_t *cla
                      const int64_t *dev_unary_off, int32_t n_vars, const uint8_t *dev_factor_skip,
                      const uint8_t *dev_var_skip, double infinity, double *dev_out, void *stream);
 
+/* Row permutation on the device (engine creation): dev_dst[i * row_elems + k] = dev_src[dev_rows[i] * row_elems + k]
+ * for i < n_rows, k < row_elems, elements of the given precision.  MaxSumEngine packs a one-class layout's tables with it
+ * when the factor order permutes them (layout.FactorGraphLayout.table_rows): the caller's array is uploaded as it is and
+ * the host makes no copy. */
+int fg_gather_rows(int32_t precision, void *dev_dst, const void *dev_src, const int64_t *dev_rows, int64_t n_rows,
+                   int64_t row_elems, void *stream);
+
 /* Diagnostic: evaluates the send-gate predicate approx_match (maxsum.py:688-710) on n pairs with
  * the division-free fast form used by the tiled kernels (out_fast) and the literal form
  * (out_exact); the two must agree on every input.  T arrays of n elements, uint8 outputs. */

@@ -270,6 +270,7 @@ SYMBOLS = {
     "fg_dpop_launch_count": (C.c_int64, [P]),
     "fg_solution_cost": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
                                    C.c_int32, P, P, C.c_double, P, P]),
+    "fg_gather_rows": (C.c_int, [C.c_int32, P, P, P, C.c_int64, C.c_int64, P]),
 }
 
 _lib = None

@@ -906,6 +906,35 @@ extern "C" int fg_solution_cost(int32_t precision, int32_t n_classes, const fg_c
   return cudaGetLastError() == cudaSuccess ? FG_OK : FG_ERR_CUDA;
 }
 
+// one 16-, 8- or 4-byte word per thread and step: rows of C2's f32 tables (400 bytes) move as 25 16-byte words
+template <typename W>
+__global__ void k_gather_rows(W *__restrict__ dst, const W *__restrict__ src, const int64_t *__restrict__ rows,
+                              int64_t n_rows, int64_t row_words) {
+  const int64_t n = n_rows * row_words;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / row_words;
+    dst[i] = src[rows[r] * row_words + (i - r * row_words)];
+  }
+}
+
+extern "C" int fg_gather_rows(int32_t precision, void *dev_dst, const void *dev_src, const int64_t *dev_rows,
+                              int64_t n_rows, int64_t row_elems, void *stream) {
+  if (n_rows <= 0 || row_elems <= 0) return FG_OK;
+  if (!dev_dst || !dev_src || !dev_rows || !fg_on_current_device(dev_dst) || !fg_on_current_device(dev_src))
+    return FG_ERR_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t row_bytes = row_elems * (precision == FG_F64 ? 8 : 4);
+  const uintptr_t al = (uintptr_t)dev_dst | (uintptr_t)dev_src | (uintptr_t)row_bytes;
+  const unsigned blocks = (unsigned)std::min<int64_t>((n_rows * row_bytes / 4 + 255) / 256, 8192);
+  if (al % 16 == 0)
+    k_gather_rows<int4><<<blocks, 256, 0, st>>>((int4 *)dev_dst, (const int4 *)dev_src, dev_rows, n_rows, row_bytes / 16);
+  else if (al % 8 == 0)
+    k_gather_rows<int2><<<blocks, 256, 0, st>>>((int2 *)dev_dst, (const int2 *)dev_src, dev_rows, n_rows, row_bytes / 8);
+  else
+    k_gather_rows<int32_t><<<blocks, 256, 0, st>>>((int32_t *)dev_dst, (const int32_t *)dev_src, dev_rows, n_rows, row_bytes / 4);
+  return cudaGetLastError() == cudaSuccess ? FG_OK : FG_ERR_CUDA;
+}
+
 // ---------------------------------------------------------------------------------------------
 // diagnostics
 // ---------------------------------------------------------------------------------------------

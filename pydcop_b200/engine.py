@@ -189,6 +189,21 @@ class _EngineBase:
         self.h2d_bytes = getattr(self, "h2d_bytes", 0) + t.numel() * t.element_size()   # what crossed PCIe / C2C
         return t
 
+    def _dev_tables(self, L, dtype):
+        """L.tables on the device.  A layout that deferred its table permutation (one class; FactorGraphLayout.table_rows)
+        and was not read on the host yet is permuted on the device by fg_gather_rows: the caller's array is uploaded as
+        it is, without a host copy."""
+        if L.table_rows is None or L._tables is not None:
+            return self._dev(L.tables, dtype)
+        src = self._dev(L.table_src, dtype)
+        rows = self._dev(L.table_rows, torch.int64)
+        out = torch.zeros(max(int(L.table_total), 1), dtype=dtype, device=self.device)
+        n = len(L.table_rows)
+        rc = self.lib.fg_gather_rows(PRECISIONS[self.precision][0], _ptr(out), _ptr(src), _ptr(rows), n,
+                                     int(L.table_src.size // n), self._stream())
+        self._check(rc, "fg_gather_rows")
+        return out
+
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
@@ -280,7 +295,7 @@ class MaxSumEngine(_CycleEngine):
         if mode not in ("min", "max"):
             raise ValueError(f"invalid mode {mode!r}")
         with torch.cuda.device(self.device):
-            self.tables = self._dev(L.tables, tdt)
+            self.tables = self._dev_tables(L, tdt)
             self.unary = self._dev(L.unary, tdt)
             self.dom_size = self._dev(L.dom_size, torch.int32)
             self.unary_off = self._dev(L.unary_off, torch.int64)

@@ -119,6 +119,11 @@ class FactorGraphLayout:
     init_value: np.ndarray     # int32 [V] (-1 = none), internal order
     msg_gather: Optional[np.ndarray] = field(default=None, repr=False)
     msg_gather_q: Optional[np.ndarray] = field(default=None, repr=False)
+    # deferred table permutation (one class only): internal tables = rows table_rows of table_src viewed as
+    # (n_rows, table_size), then zeros up to table_total elements; `tables` is None until first read
+    table_src: Optional[np.ndarray] = field(default=None, repr=False)
+    table_rows: Optional[np.ndarray] = field(default=None, repr=False)
+    table_total: int = 0
 
     # -- canonical <-> internal helpers (used by tests / readback, not by the hot path) ---------
     def message_gather_index(self):
@@ -157,6 +162,22 @@ class FactorGraphLayout:
         idx = np.repeat(start, d) + (np.arange(int(d.sum()), dtype=np.int64)
                                      - np.repeat(np.cumsum(d) - d, d))
         return self.unary[idx]
+
+
+def _layout_tables(self):
+    if self._tables is None and self.table_rows is not None:
+        self._tables = _take_rows(self.table_src, self.table_rows, self.table_src.size // len(self.table_rows),
+                                  self.table_total)
+    return self._tables
+
+
+def _set_layout_tables(self, value):
+    self._tables = value
+
+
+FactorGraphLayout.tables = property(_layout_tables, _set_layout_tables,
+                                    doc="tables in internal (class-major) order; a deferred permutation is applied on "
+                                        "first read")
 
 
 def _as(a, dt):
@@ -204,8 +225,23 @@ def _gather_tables(tables, starts, size):
         bounds = np.concatenate([[0], brk, [n]])
         return np.concatenate([tables[starts[a]:starts[a] + (b - a) * size]
                                for a, b in zip(bounds[:-1], bounds[1:])])
+    if tables.flags.writeable and tables.size % size == 0 and not (starts % size).any():
+        return _take_rows(tables, starts // size, size, n * size)      # one table shape tiles the array: a row gather
     idx = starts[:, None] + np.arange(size, dtype=np.int64)[None, :]
     return tables[idx.reshape(-1)]
+
+
+def _take_rows(src, rows, size, total):
+    """Rows `rows` of src viewed as (-1, size), flattened, then zeros up to `total` elements: a row gather on torch's CPU
+    threads (4-5x faster than numpy's single-threaded take at 10^5 rows)."""
+    out = np.zeros(total, dtype=src.dtype)
+    if not src.flags.writeable:     # torch wants writable memory (e.g. not a read-only memory map): numpy's take
+        out[:len(rows) * size] = src.reshape(-1, size)[rows].reshape(-1)
+        return out
+    import torch
+    torch.index_select(torch.from_numpy(src.reshape(-1, size)), 0, torch.from_numpy(np.asarray(rows, dtype=np.int64)),
+                       out=torch.from_numpy(out[:len(rows) * size].reshape(-1, size)))
+    return out
 
 
 def stable_group_order(keys, n_groups=None):
@@ -287,50 +323,7 @@ def build_layout(dom_size, factor_ptr, edge_var, tables, table_off=None, unary=N
         uniq, cls_of_factor = _unique_rows(key)
     else:
         uniq, cls_of_factor = np.zeros((0, MAX_ARITY + 1), np.int32), np.zeros(0, np.int64)
-    order = stable_group_order(cls_of_factor, len(uniq))[0].astype(np.int64)   # internal factor -> canonical factor
-    factor_perm = np.empty(F, dtype=np.int32)
-    factor_perm[order] = np.arange(F, dtype=np.int32)          # canonical -> internal
     counts = np.bincount(cls_of_factor, minlength=len(uniq)) if F else np.zeros(0, np.int64)
-
-    classes: List[FactorClass] = []
-    edge_perm = np.zeros(E, dtype=np.int32)
-    edge_msg_off = np.zeros(E, dtype=np.int64)
-    edge_class = np.zeros(E, dtype=np.int32)
-    int_edge_var = np.zeros(E, dtype=np.int32)
-    tab_parts = []
-    first_factor = first_edge = table_base = msg_base = 0
-    for ci in range(len(uniq)):
-        dom = tuple(int(x) for x in uniq[ci][:MAX_ARITY] if x > 0)
-        a, n = len(dom), int(counts[ci])
-        S = int(np.prod(dom, dtype=np.int64))
-        fc = FactorClass(a, dom, n, first_factor, first_edge, S, table_base, msg_base,
-                         tag=int(uniq[ci][MAX_ARITY]))
-        R = fc.row_total
-        classes.append(fc)
-        fs = order[first_factor:first_factor + n]               # canonical factor ids, in order
-        # tables
-        t = _gather_tables(tables, table_off[fs], S)
-        pad = (-t.size) % ALIGN
-        tab_parts.append(t)
-        if pad:
-            tab_parts.append(np.zeros(pad, dtype=tables.dtype))
-        # edges
-        ce = (factor_ptr[fs][:, None] + np.arange(a, dtype=np.int64)[None, :]).reshape(-1)
-        ie = first_edge + np.arange(n * a, dtype=np.int64)
-        edge_perm[ce] = ie
-        int_edge_var[ie] = edge_var[ce]
-        edge_class[ie] = ci
-        row_off = np.array(fc.row_off, dtype=np.int64)
-        edge_msg_off[ie] = (msg_base + (np.arange(n, dtype=np.int64) * R)[:, None]
-                            + row_off[None, :]).reshape(-1)
-        first_factor += n
-        first_edge += n * a
-        table_base += t.size + pad
-        msg_base += n * R
-        msg_base += (-msg_base) % ALIGN
-    n_msg = msg_base
-    tables_int = (tab_parts[0] if len(tab_parts) == 1 else np.concatenate(tab_parts)) if tab_parts \
-        else np.zeros(0, dtype=tables.dtype)
 
     canon_msg_off = np.zeros(E + 1, dtype=np.int64)
     np.cumsum(edge_dom, out=canon_msg_off[1:])
@@ -373,9 +366,6 @@ def build_layout(dom_size, factor_ptr, edge_var, tables, table_off=None, unary=N
                 + (np.arange(E, dtype=np.int64) - i_var_ptr[:-1].astype(np.int64)[slot_var])) \
         if E else np.zeros(0, np.int64)
     slot_canon_edge = c_var_edge[src_slot].astype(np.int32) if E else np.zeros(0, np.int32)
-    slot_edge = edge_perm[slot_canon_edge].astype(np.int32)
-    slot_roff = edge_msg_off[slot_edge]
-
     var_classes: List[VarClass] = []
     i_unary_off = np.zeros(V + 1, dtype=np.int64)
     var_qbase = np.zeros(V + 1, dtype=np.int64)
@@ -409,6 +399,76 @@ def build_layout(dom_size, factor_ptr, edge_var, tables, table_off=None, unary=N
     slot_qoff = (var_qbase[:-1][slot_var]
                  + (np.arange(E, dtype=np.int64) - i_var_ptr[:-1].astype(np.int64)[slot_var])
                  * i_dom.astype(np.int64)[slot_var]) if E else np.zeros(0, np.int64)
+
+    # ---------------- factor order ----------------
+    # Inside a class with tag 0, factors follow the q row of their position-0 edge: the internal index of the
+    # first variable, then the factor's place in that variable's `links`.  The position-0 rows a tile of factors
+    # gathers then lie within a window of about a kilobyte, and so do the r rows a tile of variables reads at
+    # its position-0 slots; the warp kernels load that window with one bulk copy (DESIGN.md §3).  Tagged classes
+    # (the multi-GPU ghost stubs) keep the caller's order.  Two stable counting sorts: key, then class.
+    slot_of_edge = np.empty(E, dtype=np.int64)
+    slot_of_edge[slot_canon_edge] = np.arange(E, dtype=np.int64)
+    tag0 = (uniq[:, MAX_ARITY] == 0)[cls_of_factor] if F else np.zeros(0, dtype=bool)
+    fkey = np.where(tag0, slot_of_edge[factor_ptr[:-1]], np.arange(F, dtype=np.int64))
+    by_key = stable_group_order(fkey, max(E, F))[0]
+    order = by_key[stable_group_order(cls_of_factor[by_key], len(uniq))[0]].astype(np.int64)   # internal -> canonical
+    factor_perm = np.empty(F, dtype=np.int32)
+    factor_perm[order] = np.arange(F, dtype=np.int32)          # canonical -> internal
+
+    classes: List[FactorClass] = []
+    table_rows = None
+    edge_perm = np.zeros(E, dtype=np.int32)
+    edge_msg_off = np.zeros(E, dtype=np.int64)
+    edge_class = np.zeros(E, dtype=np.int32)
+    int_edge_var = np.zeros(E, dtype=np.int32)
+    tab_parts = []
+    first_factor = first_edge = table_base = msg_base = 0
+    for ci in range(len(uniq)):
+        dom = tuple(int(x) for x in uniq[ci][:MAX_ARITY] if x > 0)
+        a, n = len(dom), int(counts[ci])
+        S = int(np.prod(dom, dtype=np.int64))
+        fc = FactorClass(a, dom, n, first_factor, first_edge, S, table_base, msg_base,
+                         tag=int(uniq[ci][MAX_ARITY]))
+        R = fc.row_total
+        classes.append(fc)
+        fs = order[first_factor:first_factor + n]               # canonical factor ids, in order
+        # tables.  One class whose tables tile the caller's array in another order (C2 after the factor order of
+        # DESIGN.md §3): the permutation is recorded, not applied: MaxSumEngine uploads the caller's array and permutes
+        # the rows on the device, every other reader gets the host copy on first access of `tables`
+        if len(uniq) == 1 and tables.size == n * S and n > 1 and (table_off[fs] != np.arange(n) * S).any():
+            table_rows = np.ascontiguousarray(table_off[fs] // S)
+            t = tables[:0]
+            t_size = n * S
+        else:
+            t = _gather_tables(tables, table_off[fs], S)
+            t_size = t.size
+        pad = (-t_size) % ALIGN
+        tab_parts.append(t)
+        if pad:
+            tab_parts.append(np.zeros(pad, dtype=tables.dtype))
+        # edges
+        ce = (factor_ptr[fs][:, None] + np.arange(a, dtype=np.int64)[None, :]).reshape(-1)
+        ie = first_edge + np.arange(n * a, dtype=np.int64)
+        edge_perm[ce] = ie
+        int_edge_var[ie] = edge_var[ce]
+        edge_class[ie] = ci
+        row_off = np.array(fc.row_off, dtype=np.int64)
+        edge_msg_off[ie] = (msg_base + (np.arange(n, dtype=np.int64) * R)[:, None]
+                            + row_off[None, :]).reshape(-1)
+        first_factor += n
+        first_edge += n * a
+        table_base += t_size + pad
+        msg_base += n * R
+        msg_base += (-msg_base) % ALIGN
+    n_msg = msg_base
+    tables_int = (tab_parts[0] if len(tab_parts) == 1 else np.concatenate(tab_parts)) if tab_parts \
+        else np.zeros(0, dtype=tables.dtype)
+    table_src = None
+    if table_rows is not None:      # deferred: the rows of `tables` in internal order, then the class padding
+        table_src, tables_int = tables, None
+
+    slot_edge = edge_perm[slot_canon_edge].astype(np.int32)
+    slot_roff = edge_msg_off[slot_edge]
     edge_qoff = np.zeros(E, dtype=np.int64)
     edge_qoff[slot_edge] = slot_qoff
     uniform_dom = int(dom_size[0]) if V and (dom_size == dom_size[0]).all() else 0
@@ -425,7 +485,8 @@ def build_layout(dom_size, factor_ptr, edge_var, tables, table_off=None, unary=N
         factor_perm=factor_perm, var_perm=var_perm, var_order=var_order,
         canon_edge_var=edge_var, canon_msg_off=canon_msg_off, canon_var_ptr=c_var_ptr,
         canon_var_edge=c_var_edge, canon_dom_size=dom_size, slot_canon_edge=slot_canon_edge,
-        init_value=c_init[var_order].astype(np.int32))
+        init_value=c_init[var_order].astype(np.int32), table_src=table_src, table_rows=table_rows,
+        table_total=int(table_base))
 
 
 def layout_from_instance(inst) -> FactorGraphLayout:
