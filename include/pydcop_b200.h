@@ -757,6 +757,70 @@ int fg_syncbb_step(fg_syncbb_t h, int64_t n_steps, void *stream);
 int fg_syncbb_current(fg_syncbb_t h, int64_t *steps, int64_t *messages, int32_t *finished);
 int64_t fg_syncbb_launch_count(fg_syncbb_t h);
 
+/* ------------------------------------------------------------------------------------------
+ * MixedDSA  (pydcop/algorithms/mixeddsa.py, MixedDsaComputation: DSA for problems that mix hard
+ * constraints, a table with a +inf or -inf entry, with soft ones; for ALL variables at once).  Same
+ * constraint-hypergraph arrays as MGM, except that dev_slot_edge lists each variable's SOFT slots first and
+ * its HARD slots after dev_soft_end[v], each group in node.constraints order (the host classifies the
+ * constraints in the tables' precision).  One round = one launch, one thread per variable:
+ *   C(x) = (((0 + soft slots) + own cost at x) + neighbours' costs) + hard entries that are not +inf
+ *   H(x) = hard entries equal to +inf
+ * then the lexicographic best (H, then C strictly, ties in domain order) and the five-way decision of
+ * mixeddsa.py:300-358 (csrc/mixeddsa_kernels.cuh).  Values are double-buffered: round k reads
+ * dev_value[(k-1) % 2] and writes dev_value[k % 2].  A variable without neighbours evaluates in round 1
+ * only.  dev_con_opt is written by fg_mixeddsa_init (the whole-table optimum of every constraint).
+ * Draws: Philox4x32-10 counter (canonical variable id, cycle, 0, 0): cycle 0xffffffff for the start value
+ * of EVERY variable without an initial value, else the 1-based round; u (philox_u53) for the probability
+ * test and the choice among the best values from the same block.
+ * ------------------------------------------------------------------------------------------ */
+enum { FG_MIXEDDSA_BRANCH_NONE = 0, FG_MIXEDDSA_BRANCH_HARD = 1, FG_MIXEDDSA_BRANCH_SOFT = 2,
+       FG_MIXEDDSA_BRANCH_STUCK_HARD = 3, FG_MIXEDDSA_BRANCH_STUCK_SOFT = 4, FG_MIXEDDSA_BRANCH_IDLE = 5,
+       FG_MIXEDDSA_MOVED = 8 };
+
+typedef struct {
+  int32_t abi_version, precision;
+  int32_t n_vars, n_factors, n_edges, n_classes;
+  const fg_class_t *classes;      /* HOST [n_classes] */
+  const void *dev_tables;         /* T[...] */
+  const void *dev_unary;          /* T[...] variable costs (cost_for_val) */
+  const int64_t *dev_unary_off;   /* [n_vars+1] */
+  const int32_t *dev_dom_size;    /* [n_vars] */
+  const int32_t *dev_var_id;      /* [n_vars] canonical id = Philox counter */
+  const int32_t *dev_edge_var;    /* [n_edges] */
+  const int32_t *dev_edge_class;  /* [n_edges] */
+  const int32_t *dev_var_ptr;     /* [n_vars+1] */
+  const int32_t *dev_slot_edge;   /* [n_edges] v's soft slots, then its hard slots */
+  const int32_t *dev_soft_end;    /* [n_vars] end of v's soft slots: var_ptr[v] <= soft_end[v] <= var_ptr[v+1] */
+  const int32_t *dev_nbr_ptr;     /* [n_vars+1] distinct neighbours, first-appearance order */
+  const int32_t *dev_nbr_idx;     /* [nbr_ptr[n_vars]] */
+  const int32_t *dev_init_value;  /* [n_vars] value index or -1 (random), may be NULL */
+  void *dev_con_opt;              /* T[n_factors] internal factor order (written by init) */
+  int32_t *dev_value[2];          /* [n_vars] each */
+  void *dev_cost;                 /* T[n_vars] current_cost: the eff_cost of the last move */
+  uint8_t *dev_has_cost;          /* [n_vars] current_cost is not None (the variable has moved) */
+  int32_t *dev_h_best;            /* [n_vars] H of the best values in the last round, -1 without an evaluation */
+  uint8_t *dev_branch;            /* [n_vars] FG_MIXEDDSA_BRANCH_* of the last round, | FG_MIXEDDSA_MOVED */
+  double proba_hard, proba_soft;
+  int32_t mode_max;
+  int32_t variant;                /* FG_DSA_A | FG_DSA_B | FG_DSA_C (C acts as B, mixeddsa.py:342) */
+  int32_t stop_cycle;             /* 0 = never; a run ends after stop_cycle rounds (as fg_dsa_desc_t) */
+  int32_t reserved0;
+  uint64_t seed;
+} fg_mixeddsa_desc_t;
+
+typedef struct fg_mixeddsa *fg_mixeddsa_t;
+
+int fg_mixeddsa_create(const fg_mixeddsa_desc_t *desc, fg_mixeddsa_t *out);
+int fg_mixeddsa_destroy(fg_mixeddsa_t h);
+const char *fg_mixeddsa_last_error(fg_mixeddsa_t h);
+/* constraint optima, start value of every variable (initial_value or a draw), no cost yet. */
+int fg_mixeddsa_init(fg_mixeddsa_t h, void *stream);
+/* up to n_cycles rounds (none once stop_cycle rounds have run). */
+int fg_mixeddsa_step(fg_mixeddsa_t h, int32_t n_cycles, void *stream);
+/* rounds run; the current values are in dev_value[cycle % 2]. */
+int fg_mixeddsa_current(fg_mixeddsa_t h, int64_t *cycle, int32_t *finished);
+int64_t fg_mixeddsa_launch_count(fg_mixeddsa_t h);
+
 /* Solution cost (next-tier row §8f.1; pydcop/dcop/dcop.py:319-367 `solution_cost`, called by the
  * orchestrator at the end of a run and at every metric tick, orchestrator.py:1229-1231): over the factors
  * of every non-ghost class the table entry at the assignment, over the first n_vars variables

@@ -162,6 +162,26 @@ class FgSyncbbDesc(C.Structure):
                 ("dev_cycles", P), ("n_elts", C.c_int64), ("n_pair", C.c_int64)]
 
 
+class FgMixedDsaDesc(C.Structure):
+    _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
+                ("n_vars", C.c_int32), ("n_factors", C.c_int32), ("n_edges", C.c_int32),
+                ("n_classes", C.c_int32), ("classes", C.POINTER(FgClass)),
+                ("dev_tables", P), ("dev_unary", P), ("dev_unary_off", P), ("dev_dom_size", P), ("dev_var_id", P),
+                ("dev_edge_var", P), ("dev_edge_class", P), ("dev_var_ptr", P), ("dev_slot_edge", P),
+                ("dev_soft_end", P), ("dev_nbr_ptr", P), ("dev_nbr_idx", P), ("dev_init_value", P),
+                ("dev_con_opt", P), ("dev_value", P * 2), ("dev_cost", P), ("dev_has_cost", P),
+                ("dev_h_best", P), ("dev_branch", P),
+                ("proba_hard", C.c_double), ("proba_soft", C.c_double),
+                ("mode_max", C.c_int32), ("variant", C.c_int32), ("stop_cycle", C.c_int32),
+                ("reserved0", C.c_int32), ("seed", C.c_uint64)]
+
+
+MIXEDDSA_VARIANTS = {"A": 0, "B": 1, "C": 2}
+# fg_mixeddsa_desc_t dev_branch: the case of mixeddsa.py:300-358 that applied, | MIXEDDSA_MOVED
+MIXEDDSA_BRANCH_NONE, MIXEDDSA_BRANCH_HARD, MIXEDDSA_BRANCH_SOFT = 0, 1, 2
+MIXEDDSA_BRANCH_STUCK_HARD, MIXEDDSA_BRANCH_STUCK_SOFT, MIXEDDSA_BRANCH_IDLE = 3, 4, 5
+MIXEDDSA_MOVED = 8
+
 GDBA_MODIFIERS = {"A": 0, "M": 1}
 GDBA_VIOLATIONS = {"NZ": 0, "NM": 1, "MX": 2}
 GDBA_INCREASE_MODES = {"E": 0, "R": 1, "C": 2, "T": 3}
@@ -268,6 +288,13 @@ SYMBOLS = {
     "fg_dpop_last_error": (C.c_char_p, [P]),
     "fg_dpop_run": (C.c_int, [P, P]),
     "fg_dpop_launch_count": (C.c_int64, [P]),
+    "fg_mixeddsa_create": (C.c_int, [C.POINTER(FgMixedDsaDesc), C.POINTER(P)]),
+    "fg_mixeddsa_destroy": (C.c_int, [P]),
+    "fg_mixeddsa_last_error": (C.c_char_p, [P]),
+    "fg_mixeddsa_init": (C.c_int, [P, P]),
+    "fg_mixeddsa_step": (C.c_int, [P, C.c_int32, P]),
+    "fg_mixeddsa_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "fg_mixeddsa_launch_count": (C.c_int64, [P]),
     "fg_solution_cost": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
                                    C.c_int32, P, P, C.c_double, P, P]),
     "fg_gather_rows": (C.c_int, [C.c_int32, P, P, P, C.c_int64, C.c_int64, P]),

@@ -48,9 +48,9 @@ def build(force=False, verbose=False):
         raise RuntimeError("nvcc not found: cannot build libpydcop_b200.so")
     os.makedirs(LIB_DIR, exist_ok=True)
     # one translation unit per family: engine.cu (MaxSum, DSA, halo, cost), mgm.cu (MGM), mgm2.cu (MGM-2),
-    # gdba.cu (GDBA), dpop.cu (DPOP), dba.cu (DBA), syncbb.cu (SyncBB)
+    # gdba.cu (GDBA), dpop.cu (DPOP), dba.cu (DBA), syncbb.cu (SyncBB), mixeddsa.cu (MixedDSA)
     units = [os.path.join(CSRC, f) for f in ("engine.cu", "mgm.cu", "mgm2.cu", "gdba.cu", "dpop.cu", "dba.cu",
-                                              "syncbb.cu")]
+                                              "syncbb.cu", "mixeddsa.cu")]
     cmd = [nvcc, *NVCC_FLAGS, "-o", LIB_PATH, *units, "-ldl"]
     if verbose:
         cmd.insert(1, "-Xptxas")

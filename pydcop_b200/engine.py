@@ -1065,6 +1065,105 @@ class DbaEngine(_LocalSearchEngine):
         return out
 
 
+def mixeddsa_hard_factors(layout: FactorGraphLayout, tables):
+    """Per internal factor: its table holds a +inf or -inf entry (mixeddsa.py:219), tested on `tables`, the layout's
+    tables in the run's precision (an f64 entry above the f32 range is therefore hard in f32 only)."""
+    L = layout
+    hard = np.zeros(L.n_factors, dtype=bool)
+    for c in L.classes:
+        if c.n_factors:
+            t = tables[c.table_base:c.table_base + c.n_factors * c.table_size].reshape(c.n_factors, c.table_size)
+            hard[c.first_factor:c.first_factor + c.n_factors] = np.isinf(t).any(1)
+    return hard
+
+
+def mixeddsa_slots(layout: FactorGraphLayout, hard):
+    """(slot_edge, soft_end): every variable's slots reordered to its soft constraints, then its hard ones, each in
+    node.constraints order, and where its soft slots end (csrc/mixeddsa_kernels.cuh sums them in that order)."""
+    L = layout
+    V, E = L.n_vars, L.n_edges
+    soft_end = np.asarray(L.var_ptr[:-1], dtype=np.int32).copy()
+    if not E:
+        return np.zeros(1, dtype=np.int32), soft_end
+    arity = np.array([c.arity for c in L.classes], dtype=np.int64)
+    first_edge = np.array([c.first_edge for c in L.classes], dtype=np.int64)
+    first_factor = np.array([c.first_factor for c in L.classes], dtype=np.int64)
+    e = L.slot_edge.astype(np.int64)
+    cl = L.edge_class[e].astype(np.int64)
+    slot_hard = hard[first_factor[cl] + (e - first_edge[cl]) // arity[cl]]
+    order = np.lexsort((np.arange(E), slot_hard, L.slot_var))
+    soft_end += np.bincount(L.slot_var[~slot_hard], minlength=V).astype(np.int32)
+    return np.ascontiguousarray(L.slot_edge[order], np.int32), soft_end
+
+
+def mixeddsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", proba_hard=0.7, proba_soft=0.5, variant="B",
+                  stop_cycle=0, seed=0):
+    """MixedDsaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
+    buffer, `slot_edge` the soft-then-hard slot order of mixeddsa_slots, `con_opt` written by fg_mixeddsa_init."""
+    L = layout
+    dt = PRECISIONS[precision][2]
+    with np.errstate(over="ignore"):     # an f64 entry above the f32 range becomes inf: hard in f32 (mixeddsa.py:219)
+        tables = np.ascontiguousarray(L.tables, dt)
+    slot_edge, soft_end = mixeddsa_slots(L, mixeddsa_hard_factors(L, tables))
+    nbr_ptr, nbr_idx = distinct_neighbours(L)
+    i32 = lambda a: np.ascontiguousarray(a, np.int32)  # noqa: E731
+    value0 = _per_var(L, np.zeros(L.n_vars), np.int32)
+    inputs = dict(tables=tables, unary=np.ascontiguousarray(L.unary, dt),
+                  unary_off=np.ascontiguousarray(L.unary_off, np.int64), dom_size=i32(L.dom_size),
+                  var_id=i32(L.var_order), edge_var=i32(L.edge_var), edge_class=i32(L.edge_class),
+                  var_ptr=i32(L.var_ptr), slot_edge=slot_edge, soft_end=_per_var(L, soft_end, np.int32),
+                  nbr_ptr=i32(nbr_ptr), nbr_idx=i32(nbr_idx), init_value=i32(L.init_value),
+                  value=[value0, value0.copy()])
+    n = L.n_vars
+    state = dict(con_opt=(L.n_factors, dt, 0), cost=(n, dt, 0), has_cost=(n, np.uint8, 0),
+                 h_best=(n, np.int32, -1), branch=(n, np.uint8, 0))
+    return inputs, state, dict(proba_hard=float(proba_hard), proba_soft=float(proba_soft), mode_max=int(mode == "max"),
+                               variant=_cabi.MIXEDDSA_VARIANTS[variant], stop_cycle=int(stop_cycle or 0),
+                               seed=_seed(seed))
+
+
+class MixedDsaEngine(_LocalSearchEngine):
+    """All-variables-at-once MixedDSA (pydcop/algorithms/mixeddsa.py, MixedDsaComputation; parameters :119-124).
+
+    proba_hard  probability of a move that lowers the number of violated hard constraints, or of a sideways move
+                while some remain violated
+    proba_soft  probability of a move that only improves the soft cost, or of a sideways move away from a violated
+                soft constraint (variants B and C)
+    variant     A | B | C; C behaves as B (its own branch in the reference is unreachable)
+    stop_cycle  0 = run forever; else the run ends after stop_cycle rounds (dsa_gpu's convention, dsa.py:352)
+    `values()` reports the cost of the last move (inf while a hard constraint stays violated), NaN before the first
+    one; `record()` the best H and the branch of the last round.
+    """
+    FAMILY = "mixeddsa"
+
+    def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", proba_hard=0.7,
+                 proba_soft=0.5, variant="B", stop_cycle=0, seed=0):
+        L = layout
+        self._open(layout, device, precision)
+        if mode not in ("min", "max"):
+            raise ValueError(f"invalid mode {mode!r}")
+        if variant not in _cabi.MIXEDDSA_VARIANTS:
+            raise ValueError(f"invalid variant {variant!r}: expected one of {sorted(_cabi.MIXEDDSA_VARIANTS)}")
+        if int(stop_cycle or 0) < 0:
+            raise ValueError(f"invalid stop_cycle {stop_cycle!r}: must be >= 0")
+        inputs, state, scalars = mixeddsa_plan(L, precision, mode, proba_hard, proba_soft, variant, stop_cycle, seed)
+        t = self._upload(inputs, state)
+        self.__dict__.update(t)
+        self._classes = _class_array(L)
+        self._create(fill_desc(fill_header(_cabi.FgMixedDsaDesc(), precision, L, self._classes), t, scalars))
+
+    def _assignment(self):
+        return self.value[self.cycle % 2]
+
+    def record(self):
+        """State of the last round, canonical order: h_best (-1 where the variable did not evaluate) and branch
+        (MIXEDDSA_BRANCH_* | MIXEDDSA_MOVED)."""
+        L = self.layout
+        n = L.n_vars
+        return dict(h_best=L.vars_to_canonical(self.h_best[:n].cpu().numpy()),
+                    branch=L.vars_to_canonical(self.branch[:n].cpu().numpy()))
+
+
 def dpop_plan(layout: FactorGraphLayout, tree, sched, precision="f64", mode="min"):
     """DpopEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan, for the pseudo-tree
     `tree` and its pseudotree.schedule `sched`; the scalars carry the launch lists."""
@@ -1349,6 +1448,9 @@ def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precisio
                          max_distance=p["max_distance"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank)
     if kind == "dpop":
         return DpopEngine(layout, tree=tree, device=device, precision=precision, mode=mode)
+    if kind == "mixeddsa":
+        return MixedDsaEngine(layout, device=device, precision=precision, mode=mode, proba_hard=p["proba_hard"],
+                              proba_soft=p["proba_soft"], variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed)
     if kind == "gdba":
         return GdbaEngine(layout, device=device, precision=precision, mode=mode, modifier=p["modifier"],
                           violation=p["violation"], increase_mode=p["increase_mode"], stop_cycle=p["stop_cycle"],

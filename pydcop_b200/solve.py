@@ -1,5 +1,5 @@
 """Direct solve: a DCOP file (or arrays, or a pyDcop DCOP object) -> GPU engine -> result dict
-(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba, dpop, dba, syncbb).
+(algorithms: maxsum, dsa, adsa, mgm, mgm2, gdba, dpop, dba, syncbb, mixeddsa).
 
 The plugin modules (pydcop_b200/algorithms/) keep pyDcop's orchestrator, agents and one Python
 computation object per graph node around the engine — that is the drop-in path, and it is what
@@ -28,6 +28,9 @@ messages posted (forward, backward, terminate and the start message).  The orche
 the orchestrator's own traffic, which a direct run has none of.  A
 variable that never selected a value is left out of the assignment and cost / violation are then None, as the
 orchestrator reports an incomplete assignment (orchestrator.py:1226-1240).
+MixedDSA (mixeddsa.py:119-124) runs `stop_cycle` rounds, DSA's convention (dsa.py:352); its cost and violation
+count come from the same device reduction as every other algorithm's, so runs on a hard-constrained problem compare
+directly with DBA's and GDBA's.
 
 No CPU path: the engines raise EngineError without a CUDA device.  `engine_factory` exists so
 the host logic can be tested without one.
@@ -50,8 +53,10 @@ MGM_DEFAULTS = {"break_mode": "lexic", "stop_cycle": 0}
 MGM2_DEFAULTS = {"threshold": 0.5, "favor": "unilateral", "stop_cycle": 0}
 GDBA_DEFAULTS = {"modifier": "A", "violation": "NZ", "increase_mode": "E", "stop_cycle": 0}
 DBA_DEFAULTS = {"infinity": 10000, "max_distance": 50, "stop_cycle": 0}
+MIXEDDSA_DEFAULTS = {"proba_hard": 0.7, "proba_soft": 0.5, "variant": "B", "stop_cycle": 0}   # mixeddsa.py:119-124
 DEFAULTS = {"maxsum": MAXSUM_DEFAULTS, "dsa": DSA_DEFAULTS, "mgm": MGM_DEFAULTS, "adsa": ADSA_DEFAULTS,
-            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS, "dpop": {}, "dba": DBA_DEFAULTS, "syncbb": {}}
+            "mgm2": MGM2_DEFAULTS, "gdba": GDBA_DEFAULTS, "dpop": {}, "dba": DBA_DEFAULTS, "syncbb": {},
+            "mixeddsa": MIXEDDSA_DEFAULTS}
 _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
             "start_messages": ("leafs", "leafs_vars", "all"),
             "p_mode": ("fixed", "arity"), "variant": ("A", "B", "C"),
@@ -60,7 +65,7 @@ _CHOICES = {"damping_nodes": ("vars", "factors", "both", "none"),
 ALGOS = {"maxsum": "maxsum", "maxsum_gpu": "maxsum", "dsa": "dsa", "dsa_gpu": "dsa",
          "mgm": "mgm", "mgm_gpu": "mgm", "adsa": "adsa", "adsa_gpu": "adsa", "mgm2": "mgm2", "mgm2_gpu": "mgm2",
          "gdba": "gdba", "gdba_gpu": "gdba", "dpop": "dpop", "dpop_gpu": "dpop", "dba": "dba", "dba_gpu": "dba",
-         "syncbb": "syncbb", "syncbb_gpu": "syncbb"}
+         "syncbb": "syncbb", "syncbb_gpu": "syncbb", "mixeddsa": "mixeddsa", "mixeddsa_gpu": "mixeddsa"}
 SYNCBB_CHUNK = 1 << 16   # SyncBB messages per launch: the timeout is checked between launches
 
 
@@ -164,7 +169,7 @@ def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
         a = dcop.arrays
         tree = build_tree(a["dom_size"], a["factor_ptr"], a["edge_var"])
     else:
-        if kind not in ("mgm2", "dba"):
+        if kind not in ("mgm2", "dba", "mixeddsa"):
             isolated_value = isolated_values(dcop, mode)
         if kind in ("mgm", "mgm2", "gdba", "dba", "syncbb"):
             var_rank = name_rank(dcop)
@@ -180,7 +185,7 @@ def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, par
     import torch.distributed as dist
     from .multigpu import ShardedMaxSum, broadcast_owner
     from .multigpu_dsa import ShardedDsa
-    if kind in ("mgm", "mgm2", "gdba", "dpop", "dba", "syncbb"):
+    if kind in ("mgm", "mgm2", "gdba", "dpop", "dba", "syncbb", "mixeddsa"):
         raise ValueError(f"{kind} is not sharded: run it on one GPU")
     rank, world = dist.get_rank(), dist.get_world_size()
     kw = dict(sharded_kwargs or {})
@@ -221,8 +226,8 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     noise).
 
     problem      see `load`
-    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba | dpop | dba | syncbb (the *_gpu spellings of the plugin modules are
-                 accepted)
+    algo         maxsum | dsa | adsa | mgm | mgm2 | gdba | dpop | dba | syncbb | mixeddsa (the *_gpu spellings of the plugin
+                 modules are accepted)
     algo_params  the reference's parameter names; `stop_cycle` bounds the run in cycles
     timeout      wall-clock bound in seconds (checked every `chunk` cycles; SyncBB: between launches of
                  SYNCBB_CHUNK messages)
