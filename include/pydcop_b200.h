@@ -490,6 +490,58 @@ int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream);
 int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished);
 int64_t fg_mgm2_launch_count(fg_mgm2_t h);
 
+/* Sharded MGM-2 (multi-GPU; pydcop_b200/multigpu_mgm2.py).  The handle's problem is one rank's closed local
+ * problem: its own variables with all their constraints plus a GHOST for every remote variable in their scopes
+ * (dev_var_id = GLOBAL ids, so the draws equal the single-GPU run's).  The phase kernels run on the owned variables
+ * only; a cycle has five exchanges, each one pack -> transport -> unpack over per-exchange buffers of T elements:
+ *   0 offers  owner -> holders (offerer, partner as the receiver's id or -1, the first len - 1 offer entries)
+ *   1 answers holder -> owner (accepted value or -1, the receiver's global gain), merged into the owner's flags
+ *   2 gains, 3 GO flags, 4 values: owner -> holders (one element each).
+ * Entry i of a list moves variable var[i] in record buf[off[i] .. off[i+1]); the lists of one transport peer are
+ * consecutive, so a peer's block is one contiguous run of each buffer. */
+typedef struct {
+  int64_t n_send, n_recv;
+  const int32_t *dev_send_var, *dev_recv_var;   /* internal local ids */
+  const int64_t *dev_send_off, *dev_recv_off;   /* [n + 1] record starts, elements of the run's precision */
+  void *dev_send_buf, *dev_recv_buf;            /* T[send_off[n_send]], T[recv_off[n_recv]] */
+} fg_mgm2_xfer_t;
+
+#define FG_MGM2_EXCHANGES 5
+typedef struct {
+  fg_mgm2_xfer_t x[FG_MGM2_EXCHANGES];
+  const uint8_t *dev_ghost;        /* [n_vars] 1 = another rank's variable: never computed here */
+  const int32_t *dev_send_peer;    /* [x[0].n_send] rank each offer record goes to */
+  const int32_t *dev_owner_rank;   /* [n_vars] rank owning the variable */
+  const int32_t *dev_owner_local;  /* [n_vars] the variable's internal id on that rank */
+} fg_mgm2_shard_plan_t;
+
+/* Transport over NVLink peer memory: for exchange x, block b copies n_elems[x][b] elements from send_buf + src[x][b]
+ * to the absolute (peer-mapped) address dst[x][b]; the last block of the copy kernel releases the next epoch to every
+ * peer of `sync` (csrc/peer_sync.cuh), then the rank waits for the same epoch from every peer and unpacks. */
+typedef struct {
+  int32_t n_blocks[FG_MGM2_EXCHANGES];
+  int32_t reserved0;
+  int64_t src[FG_MGM2_EXCHANGES][FG_MAX_PEERS];
+  int64_t n_elems[FG_MGM2_EXCHANGES][FG_MAX_PEERS];
+  uint64_t dst[FG_MGM2_EXCHANGES][FG_MAX_PEERS];
+  uint32_t *dev_counter;           /* one zeroed uint32 */
+  fg_peer_sync_t sync;
+} fg_mgm2_peer_plan_t;
+
+/* Attach the shard plan (copied) and, when `peer` is not NULL, the NVLink transport (copied); attaching again
+ * replaces both.  The epoch counter starts at 0 and only grows: every rank runs the same number of cycles. */
+int fg_mgm2_shard_attach(fg_mgm2_t h, const fg_mgm2_shard_plan_t *plan, const fg_mgm2_peer_plan_t *peer);
+/* init on the owned variables, then pack exchange 4 (values); the caller transports and calls unpack(4). */
+int fg_mgm2_shard_init(fg_mgm2_t h, void *stream);
+/* Host-transported cycles (NCCL): phase x runs the kernel that produces exchange x (0 value, 1 answer, 2 commit,
+ * 3 gain, 4 go) and packs it; phase 4 ends the cycle.  unpack(x) after the transport.  A cycle is phases 0..4 in
+ * order, each followed by its transport and unpack; check fg_mgm2_current's `finished` before starting one. */
+int fg_mgm2_shard_phase(fg_mgm2_t h, int32_t x, void *stream);
+int fg_mgm2_shard_unpack(fg_mgm2_t h, int32_t x, void *stream);
+/* Up to n_cycles whole cycles on the device with the NVLink transport (stops at stop_cycle as fg_mgm2_step):
+ * per exchange kernel -> pack -> copy + release -> wait -> unpack; five epochs per cycle. */
+int fg_mgm2_shard_step(fg_mgm2_t h, int32_t n_cycles, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * GDBA  (pydcop/algorithms/gdba.py: distributed breakout with constraint modifiers, for ALL
  * variables at once).  Same constraint-hypergraph arrays as MGM.  One round = two launches:

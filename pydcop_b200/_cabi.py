@@ -204,6 +204,26 @@ class FgHaloPlan(C.Structure):
                 ("dev_edge_dst_r", P * 2), ("dev_slot_dst_q", P * 2)]
 
 
+FG_MGM2_EXCHANGES = 5
+
+
+class FgMgm2Xfer(C.Structure):
+    _fields_ = [("n_send", C.c_int64), ("n_recv", C.c_int64), ("dev_send_var", P), ("dev_recv_var", P),
+                ("dev_send_off", P), ("dev_recv_off", P), ("dev_send_buf", P), ("dev_recv_buf", P)]
+
+
+class FgMgm2ShardPlan(C.Structure):
+    _fields_ = [("x", FgMgm2Xfer * FG_MGM2_EXCHANGES), ("dev_ghost", P), ("dev_send_peer", P),
+                ("dev_owner_rank", P), ("dev_owner_local", P)]
+
+
+class FgMgm2PeerPlan(C.Structure):
+    _fields_ = [("n_blocks", C.c_int32 * FG_MGM2_EXCHANGES), ("reserved0", C.c_int32),
+                ("src", (C.c_int64 * FG_MAX_PEERS) * FG_MGM2_EXCHANGES),
+                ("n_elems", (C.c_int64 * FG_MAX_PEERS) * FG_MGM2_EXCHANGES),
+                ("dst", (C.c_uint64 * FG_MAX_PEERS) * FG_MGM2_EXCHANGES),
+                ("dev_counter", P), ("sync", FgPeerSync)]
+
 # every symbol include/pydcop_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "fg_abi_version": (C.c_int, []),
@@ -262,6 +282,11 @@ SYMBOLS = {
     "fg_mgm2_step": (C.c_int, [P, C.c_int32, P]),
     "fg_mgm2_current": (C.c_int, [P, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "fg_mgm2_launch_count": (C.c_int64, [P]),
+    "fg_mgm2_shard_attach": (C.c_int, [P, C.POINTER(FgMgm2ShardPlan), C.POINTER(FgMgm2PeerPlan)]),
+    "fg_mgm2_shard_init": (C.c_int, [P, P]),
+    "fg_mgm2_shard_phase": (C.c_int, [P, C.c_int32, P]),
+    "fg_mgm2_shard_unpack": (C.c_int, [P, C.c_int32, P]),
+    "fg_mgm2_shard_step": (C.c_int, [P, C.c_int32, P]),
     "fg_gdba_create": (C.c_int, [C.POINTER(FgGdbaDesc), C.POINTER(P)]),
     "fg_gdba_destroy": (C.c_int, [P]),
     "fg_gdba_last_error": (C.c_char_p, [P]),

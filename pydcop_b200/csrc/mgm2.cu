@@ -8,11 +8,23 @@
 //   offer gain            = current_cost - cost                                   (:553)
 //   global gain           = (current_cost - cost over the other constraints) + offer gain (:593)
 //   cost after a move     = current_cost - potential_gain                         (:941, :986)
+#include <type_traits>
+
 #include "handle.cuh"
-#include "mgm2_kernels.cuh"
+#include "mgm2_shard_kernels.cuh"
+
+// engine.cu defines the barrier kernels of peer_sync.cuh; here they get internal linkage (no duplicate host stubs at
+// link time).  Its includes (<cuda_runtime.h>, <stdint.h>, <type_traits>, pydcop_b200.h) come before the namespace.
+namespace {
+#include "peer_sync.cuh"
+}
+
+struct fg_mgm2_shard;
 
 struct fg_mgm2 : fg_handle_base {
   fg_mgm2_desc_t d;
+  fg_mgm2_shard *shard = nullptr;   // fg_mgm2_shard_attach: this handle runs one rank of a sharded problem
+  ~fg_mgm2();
 };
 
 static inline unsigned mgm2_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
@@ -131,3 +143,274 @@ extern "C" int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream) {
 extern "C" int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished) { return fg_current(h, cycle, finished); }
 
 extern "C" int64_t fg_mgm2_launch_count(fg_mgm2_t h) { return fg_launch_count(h); }
+
+// ---------------------------------------------------------------------------------------------
+// Sharded MGM-2 (include/pydcop_b200.h: fg_mgm2_shard_*; kernels in csrc/mgm2_shard_kernels.cuh)
+// ---------------------------------------------------------------------------------------------
+
+struct fg_mgm2_shard {
+  fg_mgm2_shard_plan_t plan;
+  fg_mgm2_peer_plan_t peer;
+  bool has_peer = false;
+  uint64_t epoch = 0;
+};
+
+fg_mgm2::~fg_mgm2() { delete shard; }
+
+template <typename T>
+static Mgm2State<T> mgm2_state(const fg_mgm2 *h) {
+  const fg_mgm2_desc_t &d = h->d;
+  return Mgm2State<T>{d.dev_value, d.dev_offerer, d.dev_partner, d.dev_answer, d.dev_answer_value,
+                      (T *)d.dev_answer_gain, (T *)d.dev_gain, d.dev_go, d.dev_offer_off, (T *)d.dev_offer};
+}
+
+template <typename T>
+static Mgm2List<T> mgm2_list(const fg_mgm2_xfer_t &x, bool send) {
+  return send ? Mgm2List<T>{x.n_send, x.dev_send_var, x.dev_send_off, (T *)x.dev_send_buf}
+              : Mgm2List<T>{x.n_recv, x.dev_recv_var, x.dev_recv_off, (T *)x.dev_recv_buf};
+}
+
+template <typename T>
+static void mgm2_pack_t(fg_mgm2 *h, int x, cudaStream_t st) {
+  const fg_mgm2_shard_plan_t &p = h->shard->plan;
+  const Mgm2List<T> l = mgm2_list<T>(p.x[x], true);
+  if (!l.n) return;
+  k_mgm2x_pack<T><<<mgm2_blocks(l.n, 256), 256, 0, st>>>(x, l, mgm2_state<T>(h),
+                                                         Mgm2Xlat{p.dev_send_peer, p.dev_owner_rank, p.dev_owner_local});
+  ++h->launches;
+}
+
+template <typename T>
+static void mgm2_unpack_t(fg_mgm2 *h, int x, cudaStream_t st) {
+  const Mgm2List<T> l = mgm2_list<T>(h->shard->plan.x[x], false);
+  if (!l.n) return;
+  k_mgm2x_unpack<T><<<mgm2_blocks(l.n, 256), 256, 0, st>>>(x, l, mgm2_state<T>(h));
+  ++h->launches;
+}
+
+// the phase kernel that produces exchange x, on the owned variables, then the pack of x
+template <typename T>
+static int mgm2_phase_t(fg_mgm2 *h, int x, cudaStream_t st) {
+  const fg_mgm2_desc_t &d = h->d;
+  const uint8_t *gh = h->shard->plan.dev_ghost;
+  const int n = d.n_vars;
+  if (n) {
+    const MgmSide g = mgm2_side(h);
+    const uint32_t cyc = (uint32_t)(h->cycle + 1);
+    T *cost = (T *)d.dev_cost, *local = (T *)d.dev_local_cost, *gain = (T *)d.dev_gain;
+    switch (x) {
+      case MGM2X_OFFERS:
+        k_mgm2s_value<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
+            g, n, gh, (const T *)d.dev_tables, d.dev_value, cost, d.dev_has_cost, local, gain, d.dev_potential_value,
+            d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_offer_off, (T *)d.dev_offer, d.mode_max,
+            d.threshold, d.seed, cyc);
+        break;
+      case MGM2X_ANSWERS:
+        k_mgm2s_answer<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
+            g, n, gh, (const T *)d.dev_tables, d.dev_value, local, gain, d.dev_potential_value, d.dev_offerer,
+            d.dev_partner, d.dev_committed, d.dev_answer, d.dev_answer_value, (T *)d.dev_answer_gain, d.dev_offer_off,
+            (const T *)d.dev_offer, d.mode_max, d.favor, d.seed, cyc);
+        break;
+      case MGM2X_GAINS:
+        k_mgm2s_commit<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, gh, d.dev_offerer, d.dev_answer, d.dev_answer_value,
+                                                               (const T *)d.dev_answer_gain, gain,
+                                                               d.dev_potential_value, d.dev_committed);
+        break;
+      case MGM2X_GO:
+        k_mgm2s_gain<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(g, n, gh, gain, d.dev_potential_value, d.dev_committed,
+                                                             d.dev_partner, d.dev_go, d.dev_value, cost);
+        break;
+      default:
+        k_mgm2s_go<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, gh, d.dev_committed, d.dev_partner, d.dev_go, gain,
+                                                           d.dev_potential_value, d.dev_value, cost);
+        break;
+    }
+    ++h->launches;
+  }
+  mgm2_pack_t<T>(h, x, st);
+  CUDA_TRY(h, cudaGetLastError());
+  if (x == MGM2X_VALUES) ++h->cycle;
+  return FG_OK;
+}
+
+// NVLink transport of one exchange: every thread stores one 4-byte word of a peer's block into the peer's receive
+// buffer; the last block to finish releases `epoch` to every peer (the ordering argument of csrc/peer_sync.cuh)
+struct Mgm2Blocks {
+  int n;
+  int64_t word0[FG_MAX_PEERS + 1];      // prefix sums of the blocks' words
+  const uint32_t *src[FG_MAX_PEERS];
+  uint32_t *dst[FG_MAX_PEERS];
+};
+
+__global__ void __launch_bounds__(256) k_mgm2x_push(Mgm2Blocks b, uint32_t *__restrict__ counter, PeerSlots ps,
+                                                    uint64_t epoch) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < b.word0[b.n]) {
+    int k = 0;
+    while (b.word0[k + 1] <= t) ++k;
+    const int64_t w = t - b.word0[k];
+    b.dst[k][w] = b.src[k][w];
+  }
+  __threadfence_system();   // my stores are ordered before the release below
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned prev = atomicAdd(counter, 1u);
+    if (prev == gridDim.x - 1) {
+      *counter = 0;          // ready for the next launch (stream-ordered)
+      peer_release_all(ps, epoch);
+    }
+  }
+}
+
+template <typename T>
+static int mgm2_push(fg_mgm2 *h, int x, cudaStream_t st) {
+  fg_mgm2_shard *s = h->shard;
+  const fg_mgm2_peer_plan_t &pp = s->peer;
+  const int wpe = (int)(sizeof(T) / 4);
+  Mgm2Blocks b;
+  b.n = pp.n_blocks[x];
+  b.word0[0] = 0;
+  for (int k = 0; k < b.n; ++k) {
+    b.src[k] = (const uint32_t *)((const T *)s->plan.x[x].dev_send_buf + pp.src[x][k]);
+    b.dst[k] = (uint32_t *)(uintptr_t)pp.dst[x][k];
+    b.word0[k + 1] = b.word0[k] + pp.n_elems[x][k] * wpe;
+  }
+  const int64_t words = b.word0[b.n];
+  const unsigned blocks = (unsigned)(words > 0 ? (words + 255) / 256 : 1);
+  k_mgm2x_push<<<blocks, 256, 0, st>>>(b, pp.dev_counter, peer_slots_of(pp.sync), s->epoch + 1);
+  ++h->launches;
+  return cudaGetLastError() == cudaSuccess ? FG_OK : FG_ERR_CUDA;
+}
+
+template <typename T>
+static int mgm2_shard_cycle_t(fg_mgm2 *h, cudaStream_t st) {
+  fg_mgm2_shard *s = h->shard;
+  for (int x = 0; x < MGM2X_N; ++x) {
+    int rc = mgm2_phase_t<T>(h, x, st);
+    if (rc != FG_OK) return rc;
+    if (s->peer.sync.n_peers) {
+      rc = mgm2_push<T>(h, x, st);
+      if (rc == FG_OK) rc = peer_wait_launch(s->peer.sync, s->epoch + 1, st, h->launches);
+      if (rc != FG_OK) { snprintf(h->err, sizeof(h->err), "peer push / wait launch failed"); return rc; }
+      ++s->epoch;
+    }
+    mgm2_unpack_t<T>(h, x, st);
+  }
+  CUDA_TRY(h, cudaGetLastError());
+  return FG_OK;
+}
+
+template <typename T>
+static int mgm2_preload() {
+  cudaFuncAttributes a;
+  const void *fns[] = {(const void *)k_mgm2s_value<T>, (const void *)k_mgm2s_answer<T>, (const void *)k_mgm2s_commit<T>,
+                       (const void *)k_mgm2s_gain<T>,  (const void *)k_mgm2s_go<T>,     (const void *)k_mgm2x_pack<T>,
+                       (const void *)k_mgm2x_unpack<T>, (const void *)k_mgm2x_push,     (const void *)k_peer_wait};
+  for (const void *f : fns)
+    if (cudaFuncGetAttributes(&a, f) != cudaSuccess) { cudaGetLastError(); return FG_ERR_CUDA; }
+  return FG_OK;
+}
+
+static int mgm2_xfer_check(const fg_mgm2_xfer_t &x) {
+  if (x.n_send < 0 || x.n_recv < 0) return FG_ERR_ARG;
+  if (x.n_send && (!x.dev_send_var || !x.dev_send_off || !x.dev_send_buf)) return FG_ERR_ARG;
+  if (x.n_recv && (!x.dev_recv_var || !x.dev_recv_off || !x.dev_recv_buf)) return FG_ERR_ARG;
+  return FG_OK;
+}
+
+extern "C" int fg_mgm2_shard_attach(fg_mgm2_t h, const fg_mgm2_shard_plan_t *plan, const fg_mgm2_peer_plan_t *peer) {
+  if (!h || !plan) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
+  if (h->d.n_vars && (!plan->dev_ghost || !plan->dev_owner_rank || !plan->dev_owner_local)) {
+    snprintf(h->err, sizeof(h->err), "shard plan: missing ghost mask or owner arrays");
+    return FG_ERR_ARG;
+  }
+  for (int x = 0; x < MGM2X_N; ++x) {
+    if (mgm2_xfer_check(plan->x[x]) != FG_OK) {
+      snprintf(h->err, sizeof(h->err), "shard plan: exchange %d has a missing array or a negative count", x);
+      return FG_ERR_ARG;
+    }
+  }
+  if (plan->x[MGM2X_OFFERS].n_send && !plan->dev_send_peer) {
+    snprintf(h->err, sizeof(h->err), "shard plan: missing dev_send_peer");
+    return FG_ERR_ARG;
+  }
+  if (peer) {
+    if (peer_sync_check(&peer->sync) != FG_OK || (peer->sync.n_peers && !peer->dev_counter)) {
+      snprintf(h->err, sizeof(h->err), "invalid peer plan");
+      return FG_ERR_ARG;
+    }
+    const int64_t es = h->d.precision == FG_F64 ? 8 : 4;
+    for (int x = 0; x < MGM2X_N; ++x) {
+      if (peer->n_blocks[x] < 0 || peer->n_blocks[x] > FG_MAX_PEERS) {
+        snprintf(h->err, sizeof(h->err), "peer plan: exchange %d has %d blocks", x, peer->n_blocks[x]);
+        return FG_ERR_ARG;
+      }
+      for (int k = 0; k < peer->n_blocks[x]; ++k) {
+        if (peer->src[x][k] < 0 || peer->n_elems[x][k] < 0 || (peer->n_elems[x][k] && !peer->dst[x][k]) ||
+            peer->dst[x][k] % (uint64_t)es) {
+          snprintf(h->err, sizeof(h->err), "peer plan: exchange %d block %d is malformed", x, k);
+          return FG_ERR_ARG;
+        }
+      }
+    }
+  }
+  if (peer) {
+    // Load every kernel of the device-side cycle now: with lazy module loading, the first launch of a kernel may wait
+    // for the device to go idle, which never happens while this rank's barrier wait spins for a peer driven by the same
+    // host thread (several shards in one process).
+    const int rc = h->d.precision == FG_F64 ? mgm2_preload<double>() : mgm2_preload<float>();
+    if (rc != FG_OK) { snprintf(h->err, sizeof(h->err), "cannot load the sharded MGM-2 kernels"); return rc; }
+  }
+  if (!h->shard) h->shard = new (std::nothrow) fg_mgm2_shard();
+  if (!h->shard) { snprintf(h->err, sizeof(h->err), "out of host memory"); return FG_ERR_ARG; }
+  h->shard->plan = *plan;
+  h->shard->has_peer = peer != nullptr;
+  if (peer) h->shard->peer = *peer;
+  else h->shard->peer = fg_mgm2_peer_plan_t{};
+  return FG_OK;
+}
+
+template <typename T>
+static int mgm2_shard_init_t(fg_mgm2 *h, cudaStream_t st) {
+  const fg_mgm2_desc_t &d = h->d;
+  if (d.n_vars) {
+    k_mgm2s_init<T><<<mgm2_blocks(d.n_vars, 128), 128, 0, st>>>(mgm2_side(h), d.n_vars, h->shard->plan.dev_ghost,
+                                                                (const T *)d.dev_tables, d.dev_init_value, d.mode_max,
+                                                                d.seed, d.dev_value, (T *)d.dev_cost, d.dev_has_cost);
+    ++h->launches;
+  }
+  mgm2_pack_t<T>(h, MGM2X_VALUES, st);
+  CUDA_TRY(h, cudaGetLastError());
+  h->cycle = 0;
+  return FG_OK;
+}
+
+extern "C" int fg_mgm2_shard_init(fg_mgm2_t h, void *stream) {
+  if (!h || !h->shard) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
+  cudaStream_t st = (cudaStream_t)stream;
+  return h->d.precision == FG_F64 ? mgm2_shard_init_t<double>(h, st) : mgm2_shard_init_t<float>(h, st);
+}
+
+extern "C" int fg_mgm2_shard_phase(fg_mgm2_t h, int32_t x, void *stream) {
+  if (!h || !h->shard || x < 0 || x >= MGM2X_N) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
+  cudaStream_t st = (cudaStream_t)stream;
+  return h->d.precision == FG_F64 ? mgm2_phase_t<double>(h, x, st) : mgm2_phase_t<float>(h, x, st);
+}
+
+extern "C" int fg_mgm2_shard_unpack(fg_mgm2_t h, int32_t x, void *stream) {
+  if (!h || !h->shard || x < 0 || x >= MGM2X_N) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (h->d.precision == FG_F64) mgm2_unpack_t<double>(h, x, st);
+  else mgm2_unpack_t<float>(h, x, st);
+  CUDA_TRY(h, cudaGetLastError());
+  return FG_OK;
+}
+
+extern "C" int fg_mgm2_shard_step(fg_mgm2_t h, int32_t n_cycles, void *stream) {
+  if (!h || !h->shard || !h->shard->has_peer) return FG_ERR_ARG;
+  return fg_step(h, n_cycles, stream, mgm2_shard_cycle_t<float>, mgm2_shard_cycle_t<double>);
+}

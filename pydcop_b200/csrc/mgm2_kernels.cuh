@@ -93,13 +93,15 @@ __device__ __forceinline__ int mgm2_nth_best(const T *rel, int d, T best, int pi
   return 0;
 }
 
+// Each phase is a per-variable device function (mgm2_<phase>_at) behind its kernel, so the sharded kernels
+// (csrc/mgm2_shard_kernels.cuh) run the same code on the variables a rank owns.
+
 // on_start (mgm2.py:459-493)
 template <typename T>
-__global__ void k_mgm2_init(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ init_value,
-                            int mode_max, uint64_t seed, int32_t *__restrict__ value, T *__restrict__ cost,
-                            uint8_t *__restrict__ has_cost) {
-  int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n_vars) return;
+__device__ __forceinline__ void mgm2_init_at(int v, const MgmSide &g, const T *__restrict__ tables,
+                                             const int32_t *__restrict__ init_value, int mode_max, uint64_t seed,
+                                             int32_t *__restrict__ value, T *__restrict__ cost,
+                                             uint8_t *__restrict__ has_cost) {
   const int d = g.dom_size[v];
   uint32_t b[4];
   philox_draw((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, MGM2_PURPOSE_INIT, seed, b);
@@ -119,17 +121,25 @@ __global__ void k_mgm2_init(MgmSide g, int n_vars, const T *__restrict__ tables,
   has_cost[v] = 1;
 }
 
-// 1. value phase (mgm2.py:742-785)
 template <typename T>
-__global__ void __launch_bounds__(128, 8)
-k_mgm2_value(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ val,
-             T *__restrict__ cost, uint8_t *__restrict__ has_cost, T *__restrict__ local_cost,
-             T *__restrict__ gain, int32_t *__restrict__ pvalue, uint8_t *__restrict__ offerer,
-             int32_t *__restrict__ partner, uint8_t *__restrict__ committed, uint8_t *__restrict__ answer,
-             const int64_t *__restrict__ offer_off, T *__restrict__ offer, int mode_max, double threshold,
-             uint64_t seed, uint32_t cycle) {
+__global__ void k_mgm2_init(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ init_value,
+                            int mode_max, uint64_t seed, int32_t *__restrict__ value, T *__restrict__ cost,
+                            uint8_t *__restrict__ has_cost) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= n_vars) return;
+  mgm2_init_at<T>(v, g, tables, init_value, mode_max, seed, value, cost, has_cost);
+}
+
+// 1. value phase (mgm2.py:742-785)
+template <typename T>
+__device__ __forceinline__ void mgm2_value_at(int v, const MgmSide &g, const T *__restrict__ tables,
+                                              const int32_t *__restrict__ val, T *__restrict__ cost,
+                                              uint8_t *__restrict__ has_cost, T *__restrict__ local_cost,
+                                              T *__restrict__ gain, int32_t *__restrict__ pvalue,
+                                              uint8_t *__restrict__ offerer, int32_t *__restrict__ partner,
+                                              uint8_t *__restrict__ committed, uint8_t *__restrict__ answer,
+                                              const int64_t *__restrict__ offer_off, T *__restrict__ offer,
+                                              int mode_max, double threshold, uint64_t seed, uint32_t cycle) {
   const int n0 = g.nbr_ptr[v], n1 = g.nbr_ptr[v + 1];
   if (n0 == n1) return;
   const int cur = val[v];
@@ -187,19 +197,32 @@ k_mgm2_value(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t 
   }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(128, 8)
+k_mgm2_value(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ val,
+             T *__restrict__ cost, uint8_t *__restrict__ has_cost, T *__restrict__ local_cost,
+             T *__restrict__ gain, int32_t *__restrict__ pvalue, uint8_t *__restrict__ offerer,
+             int32_t *__restrict__ partner, uint8_t *__restrict__ committed, uint8_t *__restrict__ answer,
+             const int64_t *__restrict__ offer_off, T *__restrict__ offer, int mode_max, double threshold,
+             uint64_t seed, uint32_t cycle) {
+  int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n_vars) return;
+  mgm2_value_at<T>(v, g, tables, val, cost, has_cost, local_cost, gain, pvalue, offerer, partner, committed, answer,
+                   offer_off, offer, mode_max, threshold, seed, cycle);
+}
+
 // 2. answers of the non-offerers (mgm2.py:787-856, _find_best_offer :556-603).  The offers are read
 // in canonical order (offerer's neighbour position, offerer value, own value); only variable v
 // writes its own state and the answer slot of the one offerer it accepts.
 template <typename T>
-__global__ void __launch_bounds__(128)
-k_mgm2_answer(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ val,
-              const T *__restrict__ local_cost, T *__restrict__ gain, int32_t *__restrict__ pvalue,
-              const uint8_t *__restrict__ offerer, int32_t *__restrict__ partner, uint8_t *__restrict__ committed,
-              uint8_t *__restrict__ answer, int32_t *__restrict__ answer_value, T *__restrict__ answer_gain,
-              const int64_t *__restrict__ offer_off, const T *__restrict__ offer, int mode_max, int favor,
-              uint64_t seed, uint32_t cycle) {
-  int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n_vars) return;
+__device__ __forceinline__ void mgm2_answer_at(int v, const MgmSide &g, const T *__restrict__ tables,
+                                               const int32_t *__restrict__ val, const T *__restrict__ local_cost,
+                                               T *__restrict__ gain, int32_t *__restrict__ pvalue,
+                                               const uint8_t *__restrict__ offerer, int32_t *__restrict__ partner,
+                                               uint8_t *__restrict__ committed, uint8_t *__restrict__ answer,
+                                               int32_t *__restrict__ answer_value, T *__restrict__ answer_gain,
+                                               const int64_t *__restrict__ offer_off, const T *__restrict__ offer,
+                                               int mode_max, int favor, uint64_t seed, uint32_t cycle) {
   const int n0 = g.nbr_ptr[v], n1 = g.nbr_ptr[v + 1];
   if (n0 == n1 || offerer[v]) return;
   const int d = g.dom_size[v];
@@ -267,28 +290,50 @@ k_mgm2_answer(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t
   answer_gain[acc_u] = best;
 }
 
+template <typename T>
+__global__ void __launch_bounds__(128)
+k_mgm2_answer(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ val,
+              const T *__restrict__ local_cost, T *__restrict__ gain, int32_t *__restrict__ pvalue,
+              const uint8_t *__restrict__ offerer, int32_t *__restrict__ partner, uint8_t *__restrict__ committed,
+              uint8_t *__restrict__ answer, int32_t *__restrict__ answer_value, T *__restrict__ answer_gain,
+              const int64_t *__restrict__ offer_off, const T *__restrict__ offer, int mode_max, int favor,
+              uint64_t seed, uint32_t cycle) {
+  int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n_vars) return;
+  mgm2_answer_at<T>(v, g, tables, val, local_cost, gain, pvalue, offerer, partner, committed, answer, answer_value,
+                    answer_gain, offer_off, offer, mode_max, favor, seed, cycle);
+}
+
 // 3. an accepted offerer commits to the joint move (mgm2.py:858-890)
+template <typename T>
+__device__ __forceinline__ void mgm2_commit_at(int v, const uint8_t *__restrict__ offerer,
+                                               const uint8_t *__restrict__ answer,
+                                               const int32_t *__restrict__ answer_value,
+                                               const T *__restrict__ answer_gain, T *__restrict__ gain,
+                                               int32_t *__restrict__ pvalue, uint8_t *__restrict__ committed) {
+  if (!offerer[v] || !answer[v]) return;
+  pvalue[v] = answer_value[v];
+  gain[v] = answer_gain[v];
+  committed[v] = 1;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_mgm2_commit(int n_vars, const uint8_t *__restrict__ offerer, const uint8_t *__restrict__ answer,
               const int32_t *__restrict__ answer_value, const T *__restrict__ answer_gain, T *__restrict__ gain,
               int32_t *__restrict__ pvalue, uint8_t *__restrict__ committed) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n_vars || !offerer[v] || !answer[v]) return;
-  pvalue[v] = answer_value[v];
-  gain[v] = answer_gain[v];
-  committed[v] = 1;
+  if (v >= n_vars) return;
+  mgm2_commit_at<T>(v, offerer, answer, answer_value, answer_gain, gain, pvalue, committed);
 }
 
 // 4. gain phase (mgm2.py:892-972): a committed variable sends GO when its gain beats every other
 // neighbour's; the others move on MGM's rule (strict maximum, or tie and smallest name)
 template <typename T>
-__global__ void __launch_bounds__(256)
-k_mgm2_gain(MgmSide g, int n_vars, const T *__restrict__ gain, const int32_t *__restrict__ pvalue,
-            const uint8_t *__restrict__ committed, const int32_t *__restrict__ partner, uint8_t *__restrict__ go,
-            int32_t *__restrict__ val, T *__restrict__ cost) {
-  int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n_vars) return;
+__device__ __forceinline__ void mgm2_gain_at(int v, const MgmSide &g, const T *__restrict__ gain,
+                                             const int32_t *__restrict__ pvalue, const uint8_t *__restrict__ committed,
+                                             const int32_t *__restrict__ partner, uint8_t *__restrict__ go,
+                                             int32_t *__restrict__ val, T *__restrict__ cost) {
   const int n0 = g.nbr_ptr[v], n1 = g.nbr_ptr[v + 1];
   if (n0 == n1) return;
   go[v] = 0;
@@ -329,14 +374,33 @@ k_mgm2_gain(MgmSide g, int n_vars, const T *__restrict__ gain, const int32_t *__
   }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_mgm2_gain(MgmSide g, int n_vars, const T *__restrict__ gain, const int32_t *__restrict__ pvalue,
+            const uint8_t *__restrict__ committed, const int32_t *__restrict__ partner, uint8_t *__restrict__ go,
+            int32_t *__restrict__ val, T *__restrict__ cost) {
+  int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n_vars) return;
+  mgm2_gain_at<T>(v, g, gain, pvalue, committed, partner, go, val, cost);
+}
+
 // 5. coordinated moves (mgm2.py:974-1001)
+template <typename T>
+__device__ __forceinline__ void mgm2_go_at(int v, const uint8_t *__restrict__ committed,
+                                           const int32_t *__restrict__ partner, const uint8_t *__restrict__ go,
+                                           const T *__restrict__ gain, const int32_t *__restrict__ pvalue,
+                                           int32_t *__restrict__ val, T *__restrict__ cost) {
+  if (!committed[v] || !go[v] || !go[partner[v]]) return;
+  val[v] = pvalue[v];
+  cost[v] = cost[v] - gain[v];
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_mgm2_go(int n_vars, const uint8_t *__restrict__ committed, const int32_t *__restrict__ partner,
           const uint8_t *__restrict__ go, const T *__restrict__ gain, const int32_t *__restrict__ pvalue,
           int32_t *__restrict__ val, T *__restrict__ cost) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n_vars || !committed[v] || !go[v] || !go[partner[v]]) return;
-  val[v] = pvalue[v];
-  cost[v] = cost[v] - gain[v];
+  if (v >= n_vars) return;
+  mgm2_go_at<T>(v, committed, partner, go, gain, pvalue, val, cost);
 }

@@ -732,13 +732,16 @@ def mgm2_offer_offsets(layout: FactorGraphLayout, nbr_ptr, nbr_idx):
 
 
 def mgm2_plan(layout: FactorGraphLayout, precision="f32", mode="min", threshold=0.5, favor="unilateral",
-              stop_cycle=0, seed=0, var_rank=None):
-    """Mgm2Engine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan."""
+              stop_cycle=0, seed=0, var_rank=None, var_global_id=None):
+    """Mgm2Engine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan.  var_global_id (canonical
+    order): the Philox counter of every variable when the layout is a shard of a larger problem."""
     L = layout
     dt = PRECISIONS[precision][2]
     h = mgm_host_arrays(L, mode, var_rank)
     offer_off, offer_size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
     inputs = dict(**_neighbourhood_inputs(L, dt, h), offer_off=_per_var(L, offer_off, np.int64))
+    if var_global_id is not None:
+        inputs["var_id"] = _per_var(L, np.asarray(var_global_id, dtype=np.int32)[L.var_order], np.int32)
     n = L.n_vars
     state = dict(value=(n, np.int32, 0), potential_value=(n, np.int32, 0), answer_value=(n, np.int32, 0),
                  partner=(n, np.int32, -1), cost=(n, dt, 0), gain=(n, dt, 0), local_cost=(n, dt, 0),
@@ -757,20 +760,23 @@ class Mgm2Engine(_LocalSearchEngine):
                EQUALS its best unilateral gain (mgm2.py:818-822)
     var_rank   canonical order: position of each variable's NAME in sorted order, the lexicographic
                tie break of mgm2.py:944-949 (default: the canonical index)
+    var_global_id  canonical order: the Philox counter of each variable when the layout is one rank's shard
+               of a larger problem (pydcop_b200/multigpu_mgm2.py; default: the canonical index)
     Variable costs are not part of MGM-2's costs (assignment_cost without them); a variable without
     neighbours takes a drawn value among its best over its unary constraints on the device.
     """
     FAMILY = "mgm2"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
-                 threshold=0.5, favor="unilateral", stop_cycle=0, seed=0, var_rank=None):
+                 threshold=0.5, favor="unilateral", stop_cycle=0, seed=0, var_rank=None, var_global_id=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
             raise ValueError(f"invalid mode {mode!r}")
         if favor not in _cabi.MGM2_FAVORS:
             raise ValueError(f"invalid favor {favor!r}: expected one of {sorted(_cabi.MGM2_FAVORS)}")
-        inputs, state, scalars = mgm2_plan(L, precision, mode, threshold, favor, stop_cycle, seed, var_rank)
+        inputs, state, scalars = mgm2_plan(L, precision, mode, threshold, favor, stop_cycle, seed, var_rank,
+                                           var_global_id)
         self.nbr_ptr_host, self.nbr_idx_host = inputs["nbr_ptr"], inputs["nbr_idx"]
         self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
         self.offer_bytes = state["offer"][0] * np.dtype(self.np_dtype).itemsize
@@ -801,6 +807,55 @@ class Mgm2Engine(_LocalSearchEngine):
                    potential_value=np.where(conn, host(self.potential_value), -1).astype(np.int32),
                    go=host(self.go))
         return {k: L.vars_to_canonical(v) for k, v in out.items()}
+
+    # -- one rank of a sharded problem (pydcop_b200/multigpu_mgm2.py; fg_mgm2_shard_*) --
+
+    def shard_attach(self, arrays):
+        """Upload a shard plan (multigpu_mgm2.Mgm2Shard.plan_arrays: host arrays, internal order) and allocate the
+        exchange buffers send_buf[x] / recv_buf[x] in the run's precision."""
+        tdt = PRECISIONS[self.precision][1]
+        with torch.cuda.device(self.device):
+            dev = {k: self._dev(a, _TORCH_DTYPES[np.asarray(a).dtype]) for k, a in arrays.items()
+                   if not isinstance(a, list)}
+            lists = [{k: self._dev(a, _TORCH_DTYPES[np.asarray(a).dtype]) for k, a in x.items()}
+                     for x in arrays["x"]]
+            self.send_buf = [torch.zeros(max(int(x["send_off"][-1]), 1), dtype=tdt, device=self.device)
+                             for x in arrays["x"]]
+            self.recv_buf = [torch.zeros(max(int(x["recv_off"][-1]), 1), dtype=tdt, device=self.device)
+                             for x in arrays["x"]]
+        plan = _cabi.FgMgm2ShardPlan()
+        for i, x in enumerate(lists):
+            p = plan.x[i]
+            p.n_send, p.n_recv = len(arrays["x"][i]["send_var"]), len(arrays["x"][i]["recv_var"])
+            p.dev_send_var, p.dev_recv_var = _ptr(x["send_var"]), _ptr(x["recv_var"])
+            p.dev_send_off, p.dev_recv_off = _ptr(x["send_off"]), _ptr(x["recv_off"])
+            p.dev_send_buf, p.dev_recv_buf = _ptr(self.send_buf[i]), _ptr(self.recv_buf[i])
+        for k in ("ghost", "send_peer", "owner_rank", "owner_local"):
+            setattr(plan, "dev_" + k, _ptr(dev[k]))
+        self._shard_keep, self._shard_plan = (dev, lists), plan
+        self._shard_call("attach", C.byref(plan), None)
+
+    def shard_attach_peer(self, peer):
+        """Add the NVLink transport (a filled _cabi.FgMgm2PeerPlan) to the attached shard plan."""
+        self._shard_peer = peer
+        self._shard_call("attach", C.byref(self._shard_plan), C.byref(peer))
+
+    def _shard_call(self, name, *args, stream=False):
+        with torch.cuda.device(self.device):
+            a = list(args) + ([self._stream()] if stream else [])
+            self._check(getattr(self.lib, f"fg_mgm2_shard_{name}")(self._h, *a), f"fg_mgm2_shard_{name}")
+
+    def shard_init(self):
+        self._shard_call("init", stream=True)
+
+    def shard_phase(self, x):
+        self._shard_call("phase", int(x), stream=True)
+
+    def shard_unpack(self, x):
+        self._shard_call("unpack", int(x), stream=True)
+
+    def shard_step(self, n_cycles):
+        self._shard_call("step", int(n_cycles), stream=True)
 
 
 def gdba_host_arrays(layout: FactorGraphLayout, nbr_ptr, increase_mode="E", violation="NZ"):

@@ -275,7 +275,54 @@ class ValuePeerPush:
             raise RuntimeError(f"fg_dsa_shard_step failed rc={rc}: {e._last_error()}")
 
 
-class ShardedDsa:
+class ShardResults:
+    """The whole problem's results from one rank of a sharded local search (ShardedDsa, ShardedMgm2): subclasses
+    provide shard, engine, torch, device, global_n_vars, global_dom_size, group, local_values() and _value_tensor()
+    (the current values, internal order, on the engine's device)."""
+
+    def solution_cost(self, infinity=float("inf"), unary=None):
+        """(cost, violations) of the whole problem's current assignment.  A DSA shard keeps ALL constraints of
+        its variables, so a cut constraint lives on several ranks: a rank counts a constraint only if it
+        owns the constraint's FIRST scope variable (the MaxSum ownership rule) and a variable cost only for
+        the variables it owns; it reduces on its device and the ranks all-reduce the two sums
+        (pydcop/dcop/dcop.py:319-367)."""
+        import torch.distributed as dist
+        sh, e, torch = self.shard, self.engine, self.torch
+        L = sh.layout
+        if not hasattr(self, "_cost_masks"):
+            ghost_internal = np.zeros(L.n_vars, dtype=np.uint8)
+            ghost_internal[L.var_perm[np.nonzero(sh.frozen)[0]]] = 1
+            first_e = (np.concatenate([c.first_edge + np.arange(c.n_factors, dtype=np.int64) * c.arity
+                                       for c in L.classes]) if L.n_factors else np.zeros(0, np.int64))
+            fskip = ghost_internal[L.edge_var[first_e]] if L.n_factors else np.zeros(1, np.uint8)
+            self._cost_masks = (torch.from_numpy(np.ascontiguousarray(fskip, dtype=np.uint8)).to(e.device),
+                                torch.from_numpy(ghost_internal).to(e.device))
+        local_unary = None
+        if unary is not None:
+            dom = np.asarray(self.global_dom_size, dtype=np.int64)
+            uoff = np.concatenate([[0], np.cumsum(dom)])
+            gid = sh.local_global_id
+            local_unary = np.asarray(unary, dtype=np.float64)[_ranges(uoff[gid], dom[gid])]
+        out = e._solution_cost(self._value_tensor(), infinity, local_unary, factor_skip=self._cost_masks[0],
+                               var_skip=self._cost_masks[1])
+        dist.all_reduce(out, op=dist.ReduceOp.SUM, group=self.group)
+        o = out.cpu().numpy()
+        return float(o[0]), int(round(o[1]))
+
+    def values(self):
+        """All-gathered assignment in global variable order (every rank gets the full vector)."""
+        import torch.distributed as dist
+        torch = self.torch
+        ids, val = self.local_values()
+        out = torch.zeros(self.global_n_vars, dtype=torch.int32, device=self.device)
+        if len(ids):
+            out[torch.from_numpy(np.asarray(ids)).to(self.device)] = \
+                torch.from_numpy(val.astype(np.int32)).to(self.device)
+        dist.all_reduce(out, op=dist.ReduceOp.SUM, group=self.group)
+        return out.cpu().numpy()
+
+
+class ShardedDsa(ShardResults):
     """One rank of the partitioned DSA: same driving API as DsaEngine (init / step / values).
 
     `engine_factory(layout, inst=local arrays, **kwargs)` and `pack` / `unpack` exist so the partition and exchange
@@ -368,48 +415,15 @@ class ShardedDsa:
         if self.peer is not None:
             self.peer.sync.check()
 
-    def solution_cost(self, infinity=float("inf"), unary=None):
-        """(cost, violations) of the whole problem's current assignment.  A DSA shard keeps ALL constraints of
-        its variables, so a cut constraint lives on several ranks: a rank counts a constraint only if it
-        owns the constraint's FIRST scope variable (the MaxSum ownership rule) and a variable cost only for
-        the variables it owns; it reduces on its device and the ranks all-reduce the two sums
-        (pydcop/dcop/dcop.py:319-367)."""
-        import torch.distributed as dist
-        sh, e, torch = self.shard, self.engine, self.torch
-        L = sh.layout
-        if not hasattr(self, "_cost_masks"):
-            ghost_internal = np.zeros(L.n_vars, dtype=np.uint8)
-            ghost_internal[L.var_perm[np.nonzero(sh.frozen)[0]]] = 1
-            first_e = (np.concatenate([c.first_edge + np.arange(c.n_factors, dtype=np.int64) * c.arity
-                                       for c in L.classes]) if L.n_factors else np.zeros(0, np.int64))
-            fskip = ghost_internal[L.edge_var[first_e]] if L.n_factors else np.zeros(1, np.uint8)
-            self._cost_masks = (torch.from_numpy(np.ascontiguousarray(fskip, dtype=np.uint8)).to(e.device),
-                                torch.from_numpy(ghost_internal).to(e.device))
-        local_unary = None
-        if unary is not None:
-            dom = np.asarray(self.global_dom_size, dtype=np.int64)
-            uoff = np.concatenate([[0], np.cumsum(dom)])
-            gid = sh.local_global_id
-            local_unary = np.asarray(unary, dtype=np.float64)[_ranges(uoff[gid], dom[gid])]
-        out = e._solution_cost(e.value[e.cur], infinity, local_unary, factor_skip=self._cost_masks[0],
-                               var_skip=self._cost_masks[1])
-        dist.all_reduce(out, op=dist.ReduceOp.SUM, group=self.halo.group)
-        o = out.cpu().numpy()
-        return float(o[0]), int(round(o[1]))
-
     def local_values(self):
         """(global variable ids, value indices) of the variables this rank owns."""
         val = self.engine.values()
         return self.shard.own_vars, np.asarray(val)[:self.shard.n_own_vars]
 
-    def values(self):
-        """All-gathered assignment in global variable order (every rank gets the full vector)."""
-        import torch.distributed as dist
-        torch = self.torch
-        ids, val = self.local_values()
-        out = torch.zeros(self.global_n_vars, dtype=torch.int32, device=self.device)
-        if len(ids):
-            out[torch.from_numpy(np.asarray(ids)).to(self.device)] = \
-                torch.from_numpy(val.astype(np.int32)).to(self.device)
-        dist.all_reduce(out, op=dist.ReduceOp.SUM, group=self.halo.group)
-        return out.cpu().numpy()
+    def _value_tensor(self):
+        e = self.engine
+        return e.value[e.cur]
+
+    @property
+    def group(self):
+        return self.halo.group

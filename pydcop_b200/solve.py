@@ -180,12 +180,13 @@ def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
 def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, partition, halo, sharded_kwargs):
     """One rank's engine of a multi-process run (torch.distributed is initialised): the variables
     are split over the ranks (rank 0 computes the partition and broadcasts it), boundary rows /
-    values are exchanged every cycle (pydcop_b200.multigpu, multigpu_dsa)."""
+    values are exchanged every cycle (pydcop_b200.multigpu, multigpu_dsa, multigpu_mgm2)."""
     import torch
     import torch.distributed as dist
     from .multigpu import ShardedMaxSum, broadcast_owner
     from .multigpu_dsa import ShardedDsa
-    if kind in ("mgm", "mgm2", "gdba", "dpop", "dba", "syncbb", "mixeddsa"):
+    from .multigpu_mgm2 import ShardedMgm2
+    if kind in ("mgm", "gdba", "dpop", "dba", "syncbb", "mixeddsa"):
         raise ValueError(f"{kind} is not sharded: run it on one GPU")
     rank, world = dist.get_rank(), dist.get_world_size()
     kw = dict(sharded_kwargs or {})
@@ -201,6 +202,10 @@ def _sharded_engine(kind, inst, dcop, params, mode, precision, device, seed, par
                             damping=params["damping"], damping_nodes=params["damping_nodes"],
                             stability=params["stability"], start_messages=params["start_messages"],
                             **dict({"record_sent": False} if "engine_factory" not in kw else {}, **kw))
+    elif kind == "mgm2":
+        eng = ShardedMgm2(inst, rank, world, dev, precision=precision, halo=halo, partition=owner, mode=mode,
+                          threshold=params["threshold"], favor=params["favor"], stop_cycle=params["stop_cycle"],
+                          seed=seed or 0, var_rank=name_rank(dcop), **kw)
     else:
         eng = ShardedDsa(inst, rank, world, dev, precision=precision, halo=halo, partition=owner, mode=mode,
                          probability=params["probability"], p_mode=params.get("p_mode", "fixed"),
