@@ -889,6 +889,20 @@ int fg_solution_cost(int32_t precision, int32_t n_classes, const fg_class_t *cla
                      const int64_t *dev_unary_off, int32_t n_vars, const uint8_t *dev_factor_skip,
                      const uint8_t *dev_var_skip, double infinity, double *dev_out, void *stream);
 
+/* Solution cost per problem of a batch (pydcop_b200.solve.solve_batch: several problems packed into one layout as a
+ * disjoint union): fg_solution_cost's sums, split by dev_factor_seg[internal factor] and dev_var_seg[internal
+ * variable], the problem each belongs to, in 0..n_seg-1 (an id outside that range is not counted).  dev_out[2 * s] =
+ * cost, dev_out[2 * s + 1] = violations of problem s, n_seg pairs of doubles.  Any segment order is correct; each warp
+ * adds one atomic pair per run of consecutive factors (variables) of the same problem.  Both segment arrays are
+ * required, on the current device. */
+int fg_solution_cost_segmented(int32_t precision, int32_t n_classes, const fg_class_t *classes,
+                               const void *dev_tables, const int32_t *dev_edge_var,
+                               const int32_t *dev_value, const void *dev_unary,
+                               const int64_t *dev_unary_off, int32_t n_vars, const uint8_t *dev_factor_skip,
+                               const uint8_t *dev_var_skip, const int32_t *dev_factor_seg,
+                               const int32_t *dev_var_seg, int32_t n_seg, double infinity, double *dev_out,
+                               void *stream);
+
 /* Row permutation on the device (engine creation): dev_dst[i * row_elems + k] = dev_src[dev_rows[i] * row_elems + k]
  * for i < n_rows, k < row_elems, elements of the given precision.  MaxSumEngine packs a one-class layout's tables with it
  * when the factor order permutes them (layout.FactorGraphLayout.table_rows): the caller's array is uploaded as it is and

@@ -322,6 +322,8 @@ SYMBOLS = {
     "fg_mixeddsa_launch_count": (C.c_int64, [P]),
     "fg_solution_cost": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
                                    C.c_int32, P, P, C.c_double, P, P]),
+    "fg_solution_cost_segmented": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
+                                             C.c_int32, P, P, P, P, C.c_int32, C.c_double, P, P]),
     "fg_gather_rows": (C.c_int, [C.c_int32, P, P, P, C.c_int64, C.c_int64, P]),
 }
 

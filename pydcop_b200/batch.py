@@ -1,0 +1,127 @@
+"""Many problems in one engine run (solve.solve_batch): the disjoint union of their front-door arrays.
+
+Every kernel computes a variable or a factor from its own neighbourhood, in `node.constraints` order, so packing
+several problems into one layout changes nothing any problem computes, as long as every per-variable input a kernel
+reads is the problem's own: the Philox counter (`var_global_id`: the variable's index in its own problem, the
+mechanism the sharded engines use the other way round, DESIGN.md §6), the name rank (only ever compared between
+neighbours) and the start value of a variable without neighbours.  The union's canonical variable order is the
+concatenation of the problems', so problem k's values are one slice of the result.
+"""
+from dataclasses import dataclass
+from typing import Dict, List, Optional
+
+import numpy as np
+
+from . import ingest
+from .layout import FactorGraphLayout, build_layout
+
+INDEX_LIMIT = 2 ** 31 - 1      # variables, factors and edges of one engine are int32 indices
+MAX_BATCH_VARS = 1 << 20       # default bound on the variables of one engine: C4's size
+
+
+def _front_door_consistent(a: Dict[str, np.ndarray]) -> bool:
+    """The array sizes and ranges a union could hide: with them right, every other check build_layout makes on the
+    union is local to one problem's factors or variables."""
+    V, E = len(a["dom_size"]), len(a["edge_var"])
+    fp, to, vp = a["factor_ptr"], a["table_off"], a["var_ptr"]
+    ev = np.asarray(a["edge_var"])
+    return (len(fp) >= 1 and fp[0] == 0 and fp[-1] == E and len(to) == len(fp) and to[0] == 0
+            and to[-1] == len(a["tables"]) and len(vp) == V + 1 and vp[0] == 0 and vp[-1] == E
+            and len(a["var_edge"]) == E and len(a["unary"]) == int(np.sum(a["dom_size"], dtype=np.int64))
+            and len(a["init_value"]) == V and (not E or (ev.min() >= 0 and ev.max() < V)))
+
+
+def check_problem(index: int, dcop: ingest.DcopArrays):
+    """Raise what solve() raises on problem `index`'s arrays, with its index, if a union could hide it."""
+    if not _front_door_consistent(dcop.arrays):
+        layout_of(index, dcop.arrays)
+        raise ValueError(f"problem {index}: inconsistent front-door arrays")
+
+
+def layout_of(index: int, inst) -> FactorGraphLayout:
+    try:
+        return build_layout(**inst)
+    except ValueError as e:
+        raise ValueError(f"problem {index}: {e}") from e
+
+
+def groups(dcops: List[ingest.DcopArrays], max_vars: int = MAX_BATCH_VARS) -> List[List[int]]:
+    """Problem indices per engine: one objective per group (mode_max is one scalar per engine), min before max in
+    order of first appearance, input order inside; a group is cut before it would exceed `max_vars` variables or an
+    int32 index range (a problem larger than that runs alone)."""
+    out = []
+    for mode in dict.fromkeys(d.objective for d in dcops):
+        cur, size = [], np.zeros(3, dtype=np.int64)
+        for i, d in enumerate(dcops):
+            if d.objective != mode:
+                continue
+            a = d.arrays
+            s = np.array([d.n_vars, len(a["factor_ptr"]) - 1, len(a["edge_var"])], dtype=np.int64)
+            t = size + s
+            if cur and (t[0] > max_vars or (t > INDEX_LIMIT).any()):
+                out.append(cur)
+                cur, t = [], s
+            cur.append(i)
+            size = t
+        out.append(cur)
+    return out
+
+
+@dataclass
+class Union:
+    """The front-door arrays of problems `members` as one problem, and the per-problem inputs the engines take."""
+    members: List[int]
+    inst: Dict[str, np.ndarray]          # front-door arrays (MaxSum: unary with each problem's noise)
+    unary: np.ndarray                    # the variables' own costs, without noise: what the solution cost adds
+    var_start: np.ndarray                # [n + 1] first variable of every problem, then the total
+    var_global_id: np.ndarray            # each variable's index in its own problem
+    var_rank: Optional[np.ndarray]       # each variable's name rank in its own problem
+    isolated_value: Optional[np.ndarray]  # start value of the variables without neighbours, per problem
+    seg_factor: np.ndarray               # problem (0..n-1) of every canonical factor
+    seg_var: np.ndarray                  # problem of every canonical variable
+
+
+def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs, noise: float = 0.0,
+                seed: Optional[int] = None) -> Union:
+    """Concatenate the problems `members` of `dcops`: variable, edge and table indices are offset by the problems
+    before.  var_inputs(dcop) -> (var_rank or None, isolated_value or None), each problem's own; `noise`: MaxSum's, drawn
+    per problem with `seed` exactly as solve() draws it."""
+    parts = [dcops[i].arrays for i in members]
+    n_var = np.array([len(a["dom_size"]) for a in parts], dtype=np.int64)
+    n_fac = np.array([len(a["factor_ptr"]) - 1 for a in parts], dtype=np.int64)
+    n_edge = np.array([len(a["edge_var"]) for a in parts], dtype=np.int64)
+    n_tab = np.array([len(a["tables"]) for a in parts], dtype=np.int64)
+    v0, e0, t0 = (np.concatenate([[0], np.cumsum(x)]) for x in (n_var, n_edge, n_tab))
+
+    def ptr(key, off):
+        return np.concatenate([np.asarray(a[key][:-1], dtype=np.int64) + o for a, o in zip(parts, off[:-1])]
+                              + [[off[-1]]]).astype(np.int64)
+
+    cat = lambda key, dt=None: np.concatenate([np.asarray(a[key], dtype=dt) for a in parts])  # noqa: E731
+    unary = cat("unary", np.float64)
+    inst = dict(dom_size=cat("dom_size", np.int32), factor_ptr=ptr("factor_ptr", e0),
+                edge_var=np.concatenate([np.asarray(a["edge_var"], dtype=np.int64) + o
+                                         for a, o in zip(parts, v0[:-1])]).astype(np.int32),
+                table_off=ptr("table_off", t0), tables=np.concatenate([np.asarray(a["tables"]) for a in parts]),
+                unary=(np.concatenate([ingest.add_noise(a["unary"], noise, seed) for a in parts]) if noise else unary),
+                var_ptr=ptr("var_ptr", e0).astype(np.int32),
+                var_edge=np.concatenate([np.asarray(a["var_edge"], dtype=np.int64) + o
+                                         for a, o in zip(parts, e0[:-1])]).astype(np.int32),
+                init_value=cat("init_value", np.int32))
+    ranks, isos = zip(*(var_inputs(dcops[i]) for i in members))
+    seg = np.arange(len(members), dtype=np.int32)
+    return Union(members=list(members), inst=inst, unary=unary, var_start=v0,
+                 var_global_id=np.concatenate([np.arange(n, dtype=np.int32) for n in n_var]),
+                 var_rank=None if ranks[0] is None else np.concatenate(ranks).astype(np.int32),
+                 isolated_value=None if isos[0] is None else np.concatenate(isos).astype(np.int32),
+                 seg_factor=np.repeat(seg, n_fac), seg_var=np.repeat(seg, n_var))
+
+
+def union_layout(u: Union, dcops: List[ingest.DcopArrays]) -> FactorGraphLayout:
+    """build_layout of the union; a problem it refuses is named by its index in the batch, with solve()'s message."""
+    try:
+        return build_layout(**u.inst)
+    except ValueError:
+        for i in u.members:
+            layout_of(i, dcops[i].arrays)
+        raise

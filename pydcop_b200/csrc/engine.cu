@@ -853,57 +853,116 @@ extern "C" int fg_dsa_shard_step(fg_dsa_t h, int32_t n_cycles, void *stream) {
 
 // ---------------------------------------------------------------------------------------------
 // solution cost (dcop.py:319-367): costs equal to `infinity` are COUNTED, the others summed —
-// constraints and variable costs alike
+// constraints and variable costs alike.  `seg` (optional) gives every factor / variable the problem it belongs to
+// (fg_solution_cost_segmented); NULL puts everything in segment 0.
 // ---------------------------------------------------------------------------------------------
+
+// Adds the warp's (cost, violation) pairs into out[2 * s], out[2 * s + 1].  Without segments: a butterfly and one
+// atomic pair per warp.  With segments: an inclusive scan inside each run of consecutive lanes with the same segment,
+// and one atomic pair per run from its last lane, so any order is correct and runs (the usual case: a problem's
+// factors and variables lie in runs of the internal order) cost one atomic pair per warp and run.  A lane with
+// s < 0 adds nothing.
+__device__ __forceinline__ void cost_warp_add(double cst, double viol, int s, bool segmented, double *__restrict__ out) {
+  const unsigned lane = threadIdx.x & 31;
+  if (!segmented) {
+    for (int o = 16; o; o >>= 1) { cst += __shfl_xor_sync(0xffffffffu, cst, o); viol += __shfl_xor_sync(0xffffffffu, viol, o); }
+    if (lane == 0) { if (cst != 0.0) atomicAdd(out, cst); if (viol != 0.0) atomicAdd(out + 1, viol); }
+    return;
+  }
+  const int prev = __shfl_up_sync(0xffffffffu, s, 1);
+  const unsigned heads = __ballot_sync(0xffffffffu, lane == 0 || prev != s);
+  const unsigned run_start = 31u - __clz(heads & (0xffffffffu >> (31u - lane)));   // highest head at or below lane
+  for (unsigned o = 1; o < 32; o <<= 1) {
+    const double c = __shfl_up_sync(0xffffffffu, cst, o), v = __shfl_up_sync(0xffffffffu, viol, o);
+    if (lane >= run_start + o) { cst += c; viol += v; }
+  }
+  const bool run_end = lane == 31 || ((heads >> (lane + 1)) & 1u);
+  if (run_end && s >= 0) {
+    if (cst != 0.0) atomicAdd(out + 2 * (int64_t)s, cst);
+    if (viol != 0.0) atomicAdd(out + 2 * (int64_t)s + 1, viol);
+  }
+}
+
 template <typename T>
 __global__ void k_cost_factors(const fg_class_t c, const T *__restrict__ tables, const int32_t *__restrict__ edge_var,
                                const int32_t *__restrict__ value, const uint8_t *__restrict__ skip, T infinity,
-                               double *__restrict__ out) {
+                               const int32_t *__restrict__ seg, int32_t n_seg, double *__restrict__ out) {
   int f = blockIdx.x * blockDim.x + threadIdx.x;
   double cst = 0.0, viol = 0.0;
-  if (f < c.n_factors && !(skip && skip[c.first_factor + f])) {
+  int s = -1;
+  if (f < c.n_factors) {
+    s = seg ? seg[c.first_factor + f] : 0;
+    if (s >= n_seg) s = -1;
+  }
+  if (s >= 0 && !(skip && skip[c.first_factor + f])) {
     int64_t idx = 0, stride = 1;
     const int e0 = c.first_edge + f * c.arity;
     for (int i = c.arity - 1; i >= 0; --i) { idx += (int64_t)value[edge_var[e0 + i]] * stride; stride *= c.dom[i]; }
     const T t = tables[c.table_base + (int64_t)f * c.table_size + idx];
     if (t != infinity) cst = (double)t; else viol = 1.0;   // `r_cost != infinity`, dcop.py:355
   }
-  for (int o = 16; o; o >>= 1) { cst += __shfl_xor_sync(0xffffffffu, cst, o); viol += __shfl_xor_sync(0xffffffffu, viol, o); }
-  if ((threadIdx.x & 31) == 0) { if (cst != 0.0) atomicAdd(out, cst); if (viol != 0.0) atomicAdd(out + 1, viol); }
+  cost_warp_add(cst, viol, s, seg != nullptr, out);
 }
 
 template <typename T>
 __global__ void k_cost_unary(const T *__restrict__ unary, const int64_t *__restrict__ unary_off,
                              const int32_t *__restrict__ value, int n_vars, const uint8_t *__restrict__ skip,
-                             T infinity, double *__restrict__ out) {
+                             T infinity, const int32_t *__restrict__ seg, int32_t n_seg, double *__restrict__ out) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   double cst = 0.0, viol = 0.0;
-  if (v < n_vars && !(skip && skip[v])) {
+  int s = -1;
+  if (v < n_vars) {
+    s = seg ? seg[v] : 0;
+    if (s >= n_seg) s = -1;
+  }
+  if (s >= 0 && !(skip && skip[v])) {
     const T t = unary[unary_off[v] + value[v]];
     if (t != infinity) cst = (double)t; else viol = 1.0;   // `cost_for_val != infinity`, dcop.py:363
   }
-  for (int o = 16; o; o >>= 1) { cst += __shfl_xor_sync(0xffffffffu, cst, o); viol += __shfl_xor_sync(0xffffffffu, viol, o); }
-  if ((threadIdx.x & 31) == 0) { if (cst != 0.0) atomicAdd(out, cst); if (viol != 0.0) atomicAdd(out + 1, viol); }
+  cost_warp_add(cst, viol, s, seg != nullptr, out);
+}
+
+static int solution_cost_launch(int32_t precision, int32_t n_classes, const fg_class_t *classes, const void *dev_tables,
+                                const int32_t *dev_edge_var, const int32_t *dev_value, const void *dev_unary,
+                                const int64_t *dev_unary_off, int32_t n_vars, const uint8_t *dev_factor_skip,
+                                const uint8_t *dev_var_skip, const int32_t *dev_factor_seg, const int32_t *dev_var_seg,
+                                int32_t n_seg, double infinity, double *dev_out, void *stream) {
+  if (!fg_on_current_device(dev_out) || (dev_value && !fg_on_current_device(dev_value))) return FG_ERR_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (cudaMemsetAsync(dev_out, 0, 2 * sizeof(double) * (size_t)n_seg, st) != cudaSuccess) return FG_ERR_CUDA;
+  for (int i = 0; i < n_classes; ++i) {
+    const fg_class_t &c = classes[i];
+    if (!c.n_factors || (c.flags & FG_CLASS_GHOST)) continue;   // halo stubs stand for another rank's factors
+    if (precision == FG_F64) k_cost_factors<double><<<blocks_for(c.n_factors, 128), 128, 0, st>>>(c, (const double *)dev_tables, dev_edge_var, dev_value, dev_factor_skip, infinity, dev_factor_seg, n_seg, dev_out);
+    else k_cost_factors<float><<<blocks_for(c.n_factors, 128), 128, 0, st>>>(c, (const float *)dev_tables, dev_edge_var, dev_value, dev_factor_skip, (float)infinity, dev_factor_seg, n_seg, dev_out);
+  }
+  if (dev_unary && n_vars) {
+    if (precision == FG_F64) k_cost_unary<double><<<blocks_for(n_vars, 128), 128, 0, st>>>((const double *)dev_unary, dev_unary_off, dev_value, n_vars, dev_var_skip, infinity, dev_var_seg, n_seg, dev_out);
+    else k_cost_unary<float><<<blocks_for(n_vars, 128), 128, 0, st>>>((const float *)dev_unary, dev_unary_off, dev_value, n_vars, dev_var_skip, (float)infinity, dev_var_seg, n_seg, dev_out);
+  }
+  return cudaGetLastError() == cudaSuccess ? FG_OK : FG_ERR_CUDA;
 }
 
 extern "C" int fg_solution_cost(int32_t precision, int32_t n_classes, const fg_class_t *classes, const void *dev_tables,
                                 const int32_t *dev_edge_var, const int32_t *dev_value, const void *dev_unary,
                                 const int64_t *dev_unary_off, int32_t n_vars, const uint8_t *dev_factor_skip,
                                 const uint8_t *dev_var_skip, double infinity, double *dev_out, void *stream) {
-  if (!fg_on_current_device(dev_out) || (dev_value && !fg_on_current_device(dev_value))) return FG_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (cudaMemsetAsync(dev_out, 0, 2 * sizeof(double), st) != cudaSuccess) return FG_ERR_CUDA;
-  for (int i = 0; i < n_classes; ++i) {
-    const fg_class_t &c = classes[i];
-    if (!c.n_factors || (c.flags & FG_CLASS_GHOST)) continue;   // halo stubs stand for another rank's factors
-    if (precision == FG_F64) k_cost_factors<double><<<blocks_for(c.n_factors, 128), 128, 0, st>>>(c, (const double *)dev_tables, dev_edge_var, dev_value, dev_factor_skip, infinity, dev_out);
-    else k_cost_factors<float><<<blocks_for(c.n_factors, 128), 128, 0, st>>>(c, (const float *)dev_tables, dev_edge_var, dev_value, dev_factor_skip, (float)infinity, dev_out);
-  }
-  if (dev_unary && n_vars) {
-    if (precision == FG_F64) k_cost_unary<double><<<blocks_for(n_vars, 128), 128, 0, st>>>((const double *)dev_unary, dev_unary_off, dev_value, n_vars, dev_var_skip, infinity, dev_out);
-    else k_cost_unary<float><<<blocks_for(n_vars, 128), 128, 0, st>>>((const float *)dev_unary, dev_unary_off, dev_value, n_vars, dev_var_skip, (float)infinity, dev_out);
-  }
-  return cudaGetLastError() == cudaSuccess ? FG_OK : FG_ERR_CUDA;
+  return solution_cost_launch(precision, n_classes, classes, dev_tables, dev_edge_var, dev_value, dev_unary,
+                              dev_unary_off, n_vars, dev_factor_skip, dev_var_skip, nullptr, nullptr, 1, infinity,
+                              dev_out, stream);
+}
+
+extern "C" int fg_solution_cost_segmented(int32_t precision, int32_t n_classes, const fg_class_t *classes,
+                                          const void *dev_tables, const int32_t *dev_edge_var, const int32_t *dev_value,
+                                          const void *dev_unary, const int64_t *dev_unary_off, int32_t n_vars,
+                                          const uint8_t *dev_factor_skip, const uint8_t *dev_var_skip,
+                                          const int32_t *dev_factor_seg, const int32_t *dev_var_seg, int32_t n_seg,
+                                          double infinity, double *dev_out, void *stream) {
+  if (n_seg < 1 || !dev_factor_seg || !dev_var_seg) return FG_ERR_ARG;
+  if (!fg_on_current_device(dev_factor_seg) || !fg_on_current_device(dev_var_seg)) return FG_ERR_ARG;
+  return solution_cost_launch(precision, n_classes, classes, dev_tables, dev_edge_var, dev_value, dev_unary,
+                              dev_unary_off, n_vars, dev_factor_skip, dev_var_skip, dev_factor_seg, dev_var_seg, n_seg,
+                              infinity, dev_out, stream);
 }
 
 // one 16-, 8- or 4-byte word per thread and step: rows of C2's f32 tables (400 bytes) move as 25 16-byte words

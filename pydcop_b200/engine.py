@@ -181,6 +181,19 @@ class _EngineBase:
             out = self._solution_cost(self._assignment(), infinity, unary).cpu().numpy()
         return float(out[0]), int(out[1])
 
+    def solution_costs_segmented(self, seg_factor, seg_var, n_seg, infinity=float("inf"), unary=None):
+        """(cost float64[n_seg], violations int64[n_seg]) of the current assignment per segment, reduced on the device
+        (fg_solution_cost_segmented): what solution_cost computes over the factors and variables of each segment.
+        seg_factor / seg_var: the segment (problem of a batch) of every factor and variable, canonical order."""
+        L = self.layout
+        f_int = np.zeros(max(L.n_factors, 1), dtype=np.int32)
+        f_int[L.factor_perm] = np.asarray(seg_factor, dtype=np.int32)
+        v_int = _per_var(L, np.asarray(seg_var, dtype=np.int32)[L.var_order], np.int32)
+        with torch.cuda.device(self.device):
+            seg = (self._dev(f_int, torch.int32), self._dev(v_int, torch.int32), int(n_seg))
+            out = self._solution_cost(self._assignment(), infinity, unary, seg=seg).cpu().numpy().reshape(-1, 2)
+        return out[:, 0].copy(), out[:, 1].astype(np.int64)
+
     def _dev(self, a, dtype):
         a = np.ascontiguousarray(a)
         if not a.flags.writeable:      # e.g. a read-only memory map of the binary container
@@ -212,12 +225,14 @@ class _EngineBase:
             raise EngineError(f"{what} failed (rc={rc}): {self._last_error()}")
 
     def _solution_cost(self, value_tensor, infinity=float("inf"), unary=None, n_vars=None, factor_skip=None,
-                       var_skip=None):
+                       var_skip=None, seg=None):
         """(cost, violations) of `value_tensor` (internal variable order) as LOCAL sums, on the device:
         pydcop/dcop/dcop.py:319-367 — an entry equal to `infinity` is a violation, the others are
         summed, constraints and variable costs alike.  `unary`: the variables' own costs in CANONICAL
         order (default: none are added); n_vars: leading variables that count (a shard's own ones);
-        factor_skip / var_skip: uint8 device tensors in internal order, non-zero = owned by another rank."""
+        factor_skip / var_skip: uint8 device tensors in internal order, non-zero = owned by another rank;
+        seg: (factor segment, variable segment, n_seg), int32 device tensors in internal order, for n_seg
+        (cost, violations) pairs (fg_solution_cost_segmented)."""
         L = self.layout
         prec = PRECISIONS[self.precision][0]
         tdt = PRECISIONS[self.precision][1]
@@ -226,6 +241,7 @@ class _EngineBase:
                 self._edge_var_dev = self._dev(L.edge_var, torch.int32)
                 self._cost_out = torch.zeros(2, dtype=torch.float64, device=self.device)
                 self._cost_unary_off = self._dev(L.unary_off, torch.int64)
+            out = self._cost_out if seg is None else torch.zeros(2 * seg[2], dtype=torch.float64, device=self.device)
             un = None
             if unary is not None:   # canonical (variable-major) -> internal (class-major, padded bases)
                 un_host = np.zeros(max(int(L.unary_off[-1]), 1))
@@ -237,13 +253,16 @@ class _EngineBase:
                     dst = np.repeat(L.unary_off[:-1], dom) + (np.arange(int(dom.sum())) - np.repeat(np.cumsum(dom) - dom, dom))
                     un_host[dst] = cu[src]
                 un = self._dev(un_host, tdt)
-            rc = self.lib.fg_solution_cost(
-                prec, len(L.classes), C.cast(self._classes, C.POINTER(FgClass)), _ptr(self.tables),
-                _ptr(self._edge_var_dev), _ptr(value_tensor), _ptr(un), _ptr(self._cost_unary_off),
-                int(L.n_vars if n_vars is None else n_vars), _ptr(factor_skip), _ptr(var_skip), float(infinity),
-                _ptr(self._cost_out), self._stream())
-            self._check(rc, "fg_solution_cost")
-            return self._cost_out
+            args = (prec, len(L.classes), C.cast(self._classes, C.POINTER(FgClass)), _ptr(self.tables),
+                    _ptr(self._edge_var_dev), _ptr(value_tensor), _ptr(un), _ptr(self._cost_unary_off),
+                    int(L.n_vars if n_vars is None else n_vars), _ptr(factor_skip), _ptr(var_skip))
+            if seg is None:
+                rc = self.lib.fg_solution_cost(*args, float(infinity), _ptr(out), self._stream())
+            else:
+                rc = self.lib.fg_solution_cost_segmented(*args, _ptr(seg[0]), _ptr(seg[1]), seg[2], float(infinity),
+                                                         _ptr(out), self._stream())
+            self._check(rc, "fg_solution_cost" if seg is None else "fg_solution_cost_segmented")
+            return out
 
 
 class _CycleEngine(_EngineBase):
@@ -612,10 +631,19 @@ def _seed(seed):
     return int(seed) & (2 ** 64 - 1)
 
 
+def _set_global_ids(inputs, layout, var_global_id):
+    """Replace the uploaded var_id (the canonical index) by var_global_id (canonical order), the Philox counter of
+    every variable when the layout is part of a larger problem (a shard) or one problem of a union (a batch)."""
+    if var_global_id is not None:
+        inputs["var_id"] = _per_var(layout, np.asarray(var_global_id, dtype=np.int32)[layout.var_order], np.int32)
+    return inputs
+
+
 def mgm_plan(layout: FactorGraphLayout, precision="f32", mode="min", stop_cycle=0, seed=0, var_rank=None,
-             isolated_value=None):
+             isolated_value=None, var_global_id=None):
     """MgmEngine's host-array plan: (inputs: name -> array in its final dtype, in upload order; state: name ->
-    (length, dtype, fill); the descriptor's scalar fields).  Every name is a dev_<name> field of fg_mgm_desc_t."""
+    (length, dtype, fill); the descriptor's scalar fields).  Every name is a dev_<name> field of fg_mgm_desc_t.
+    var_global_id (canonical order): the Philox counter of every variable (default: the canonical index)."""
     L = layout
     dt = PRECISIONS[precision][2]
     h = mgm_host_arrays(L, mode, var_rank, isolated_value)
@@ -624,6 +652,7 @@ def mgm_plan(layout: FactorGraphLayout, precision="f32", mode="min", stop_cycle=
                   unary_off=np.ascontiguousarray(L.unary_off, np.int64), **nb,
                   value=_per_var(L, h["value0"], np.int32), cost=_per_var(L, h["cost0"], dt),
                   has_cost=_per_var(L, ~h["has_nbr"], np.uint8))
+    _set_global_ids(inputs, L, var_global_id)
     state = dict(gain=(L.n_vars, dt, 0), new_value=(L.n_vars, np.int32, 0))
     return inputs, state, dict(mode_max=int(mode == "max"), stop_cycle=int(stop_cycle), seed=_seed(seed))
 
@@ -664,20 +693,23 @@ class MgmEngine(_LocalSearchEngine):
     isolated_value canonical order: value index of the variables without neighbours
                    (optimal_cost_value over the real domain values, relations.py:1641-1669);
                    default: argopt of the own cost with ties broken on the value index
+    var_global_id  canonical order: the Philox counter of each variable when the layout holds several problems
+                   (pydcop_b200.batch; default: the canonical index)
     `break_mode` is accepted for the reference's signature; its 'random' branch is dead code in
     the reference (mgm.py:541 compares with the `random` module) and both settings act as 'lexic'.
     """
     FAMILY = "mgm"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
-                 stop_cycle=0, seed=0, break_mode="lexic", var_rank=None, isolated_value=None):
+                 stop_cycle=0, seed=0, break_mode="lexic", var_rank=None, isolated_value=None, var_global_id=None):
         L = layout
         tdt = self._open(layout, device, precision)
         if break_mode not in ("lexic", "random"):
             raise ValueError(f"invalid break_mode {break_mode!r}")
         if mode not in ("min", "max"):
             raise ValueError(f"invalid mode {mode!r}")
-        inputs, state, scalars = mgm_plan(L, precision, mode, stop_cycle, seed, var_rank, isolated_value)
+        inputs, state, scalars = mgm_plan(L, precision, mode, stop_cycle, seed, var_rank, isolated_value,
+                                          var_global_id)
         self.has_nbr_host = np.diff(inputs["nbr_ptr"]) > 0
         t = self._upload(inputs, state)
         self.__dict__.update(t)
@@ -739,9 +771,8 @@ def mgm2_plan(layout: FactorGraphLayout, precision="f32", mode="min", threshold=
     dt = PRECISIONS[precision][2]
     h = mgm_host_arrays(L, mode, var_rank)
     offer_off, offer_size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
-    inputs = dict(**_neighbourhood_inputs(L, dt, h), offer_off=_per_var(L, offer_off, np.int64))
-    if var_global_id is not None:
-        inputs["var_id"] = _per_var(L, np.asarray(var_global_id, dtype=np.int32)[L.var_order], np.int32)
+    inputs = _set_global_ids(dict(**_neighbourhood_inputs(L, dt, h), offer_off=_per_var(L, offer_off, np.int64)),
+                             L, var_global_id)
     n = L.n_vars
     state = dict(value=(n, np.int32, 0), potential_value=(n, np.int32, 0), answer_value=(n, np.int32, 0),
                  partner=(n, np.int32, -1), cost=(n, dt, 0), gain=(n, dt, 0), local_cost=(n, dt, 0),
@@ -914,7 +945,7 @@ def gdba_modifiers_view(h, mods, base_mod, increase_mode):
 
 
 def gdba_plan(layout: FactorGraphLayout, precision="f32", mode="min", modifier="A", violation="NZ", increase_mode="E",
-              stop_cycle=0, seed=0, var_rank=None, isolated_value=None):
+              stop_cycle=0, seed=0, var_rank=None, isolated_value=None, var_global_id=None):
     """GdbaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
     buffer, and viol_ref / mod_off are None where the modes do not read them."""
     L = layout
@@ -928,6 +959,7 @@ def gdba_plan(layout: FactorGraphLayout, precision="f32", mode="min", modifier="
                   viol_ref=None if g["viol_ref"] is None else np.ascontiguousarray(g["viol_ref"], dt), **nb,
                   value=[value0, value0.copy()], cost=_per_var(L, h["cost0"], dt), has_cost=_per_var(L, ~h["has_nbr"], np.uint8),
                   mod_off=None if g["mod_off"] is None else np.ascontiguousarray(g["mod_off"], np.int64))
+    _set_global_ids(inputs, L, var_global_id)
     n = L.n_vars
     state = dict(improve=(n, dt, 0), new_value=(n, np.int32, 0), breakout=(n, np.uint8, 0),
                  violated=(L.n_edges, np.uint8, 0), mod=(g["mod_size"], np.int32, 0))
@@ -950,11 +982,13 @@ class GdbaEngine(_LocalSearchEngine):
                    gdba.py:657-658 (default: the canonical index)
     isolated_value canonical order: value index of the variables without neighbours (optimal_cost_value);
                    default: argopt of the own cost with ties broken on the value index
+    var_global_id  canonical order: the Philox counter of each variable (default: the canonical index), as MgmEngine
     """
     FAMILY = "gdba"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", modifier="A",
-                 violation="NZ", increase_mode="E", stop_cycle=0, seed=0, var_rank=None, isolated_value=None):
+                 violation="NZ", increase_mode="E", stop_cycle=0, seed=0, var_rank=None, isolated_value=None,
+                 var_global_id=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -966,7 +1000,7 @@ class GdbaEngine(_LocalSearchEngine):
                 raise ValueError(f"invalid {name} {v!r}: expected one of {sorted(ok)}")
         self.modifier, self.violation, self.increase_mode = modifier, violation, increase_mode
         inputs, state, scalars = gdba_plan(L, precision, mode, modifier, violation, increase_mode, stop_cycle, seed,
-                                           var_rank, isolated_value)
+                                           var_rank, isolated_value, var_global_id)
         self.nbr_ptr_host = inputs["nbr_ptr"]
         self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
         self.modifier_bytes = scalars["mod_size"] * 4
@@ -1152,7 +1186,7 @@ def mixeddsa_slots(layout: FactorGraphLayout, hard):
 
 
 def mixeddsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", proba_hard=0.7, proba_soft=0.5, variant="B",
-                  stop_cycle=0, seed=0):
+                  stop_cycle=0, seed=0, var_global_id=None):
     """MixedDsaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
     buffer, `slot_edge` the soft-then-hard slot order of mixeddsa_slots, `con_opt` written by fg_mixeddsa_init."""
     L = layout
@@ -1169,6 +1203,7 @@ def mixeddsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", proba_
                   var_ptr=i32(L.var_ptr), slot_edge=slot_edge, soft_end=_per_var(L, soft_end, np.int32),
                   nbr_ptr=i32(nbr_ptr), nbr_idx=i32(nbr_idx), init_value=i32(L.init_value),
                   value=[value0, value0.copy()])
+    _set_global_ids(inputs, L, var_global_id)
     n = L.n_vars
     state = dict(con_opt=(L.n_factors, dt, 0), cost=(n, dt, 0), has_cost=(n, np.uint8, 0),
                  h_best=(n, np.int32, -1), branch=(n, np.uint8, 0))
@@ -1186,13 +1221,14 @@ class MixedDsaEngine(_LocalSearchEngine):
                 soft constraint (variants B and C)
     variant     A | B | C; C behaves as B (its own branch in the reference is unreachable)
     stop_cycle  0 = run forever; else the run ends after stop_cycle rounds (dsa_gpu's convention, dsa.py:352)
+    var_global_id  canonical order: the Philox counter of each variable (default: the canonical index), as MgmEngine
     `values()` reports the cost of the last move (inf while a hard constraint stays violated), NaN before the first
     one; `record()` the best H and the branch of the last round.
     """
     FAMILY = "mixeddsa"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", proba_hard=0.7,
-                 proba_soft=0.5, variant="B", stop_cycle=0, seed=0):
+                 proba_soft=0.5, variant="B", stop_cycle=0, seed=0, var_global_id=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -1201,7 +1237,8 @@ class MixedDsaEngine(_LocalSearchEngine):
             raise ValueError(f"invalid variant {variant!r}: expected one of {sorted(_cabi.MIXEDDSA_VARIANTS)}")
         if int(stop_cycle or 0) < 0:
             raise ValueError(f"invalid stop_cycle {stop_cycle!r}: must be >= 0")
-        inputs, state, scalars = mixeddsa_plan(L, precision, mode, proba_hard, proba_soft, variant, stop_cycle, seed)
+        inputs, state, scalars = mixeddsa_plan(L, precision, mode, proba_hard, proba_soft, variant, stop_cycle, seed,
+                                               var_global_id)
         t = self._upload(inputs, state)
         self.__dict__.update(t)
         self._classes = _class_array(L)
@@ -1490,10 +1527,12 @@ class SyncbbEngine(_EngineBase):
 
 
 def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precision="f32", device=None, seed=0,
-                var_rank=None, isolated_value=None, tree=None):
+                var_rank=None, isolated_value=None, tree=None, var_global_id=None):
     """The single-GPU engine of algorithm `kind` (a value of solve.ALGOS) over `layout`.  `params`: its algorithm
-    parameters, the missing ones taking solve.DEFAULTS; var_rank / isolated_value in canonical order as the engines
-    take them (var_rank None: the canonical index); tree: DPOP's pseudo-tree.  MaxSum records no sent flags."""
+    parameters, the missing ones taking solve.DEFAULTS; var_rank / isolated_value / var_global_id in canonical order
+    as the engines take them (var_rank None: the canonical index; var_global_id None: the canonical index as every
+    Philox counter, ignored by the families without draws: MaxSum, DPOP, SyncBB); tree: DPOP's pseudo-tree.  MaxSum
+    records no sent flags."""
     from .solve import DEFAULTS
     p = dict(DEFAULTS[kind], **params)
     if kind == "syncbb":
@@ -1505,21 +1544,25 @@ def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precisio
         return DpopEngine(layout, tree=tree, device=device, precision=precision, mode=mode)
     if kind == "mixeddsa":
         return MixedDsaEngine(layout, device=device, precision=precision, mode=mode, proba_hard=p["proba_hard"],
-                              proba_soft=p["proba_soft"], variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed)
+                              proba_soft=p["proba_soft"], variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed,
+                              var_global_id=var_global_id)
     if kind == "gdba":
         return GdbaEngine(layout, device=device, precision=precision, mode=mode, modifier=p["modifier"],
                           violation=p["violation"], increase_mode=p["increase_mode"], stop_cycle=p["stop_cycle"],
-                          seed=seed, var_rank=var_rank, isolated_value=isolated_value)
+                          seed=seed, var_rank=var_rank, isolated_value=isolated_value, var_global_id=var_global_id)
     if kind == "mgm2":
         return Mgm2Engine(layout, device=device, precision=precision, mode=mode, threshold=p["threshold"],
-                          favor=p["favor"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank)
+                          favor=p["favor"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank,
+                          var_global_id=var_global_id)
     if kind == "mgm":
         return MgmEngine(layout, device=device, precision=precision, mode=mode, stop_cycle=p["stop_cycle"], seed=seed,
-                         break_mode=p["break_mode"], var_rank=var_rank, isolated_value=isolated_value)
+                         break_mode=p["break_mode"], var_rank=var_rank, isolated_value=isolated_value,
+                         var_global_id=var_global_id)
     if kind == "maxsum":
         return MaxSumEngine(layout, device=device, precision=precision, mode=mode, damping=p["damping"],
                             damping_nodes=p["damping_nodes"], stability=p["stability"],
                             start_messages=p["start_messages"], record_sent=False)
     return DsaEngine(layout, device=device, precision=precision, mode=mode, probability=p["probability"],
                      p_mode=p.get("p_mode", "fixed"), variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed,
-                     isolated_value=isolated_value, var_costs=(kind == "adsa"))   # A-DSA: candidates carry own costs
+                     isolated_value=isolated_value, var_global_id=var_global_id,
+                     var_costs=(kind == "adsa"))   # A-DSA: candidates carry own costs

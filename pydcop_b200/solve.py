@@ -38,11 +38,11 @@ the host logic can be tested without one.
 import json
 import os
 import time
-from typing import Any, Callable, Dict, Optional
+from typing import Any, Callable, Dict, List, Optional
 
 import numpy as np
 
-from . import ingest
+from . import batch, ingest
 from .layout import build_layout
 
 MAXSUM_DEFAULTS = {"damping": 0.5, "damping_nodes": "both", "stability": 0.1, "noise": 0.01,
@@ -161,18 +161,23 @@ def name_rank(dcop: ingest.DcopArrays) -> np.ndarray:
     return rank
 
 
+def _var_inputs(kind, dcop, mode):
+    """(var_rank, isolated_value) of `dcop` as the engine of `kind` takes them, canonical order; None where it takes
+    none."""
+    if kind == "dpop":
+        return None, None
+    return (name_rank(dcop) if kind in ("mgm", "mgm2", "gdba", "dba", "syncbb") else None,
+            isolated_values(dcop, mode) if kind not in ("mgm2", "dba", "mixeddsa") else None)
+
+
 def _default_engine(kind, layout, dcop, params, mode, precision, device, seed):
     from .engine import make_engine
-    tree = var_rank = isolated_value = None
+    tree = None
     if kind == "dpop":
         from .pseudotree import build_tree
         a = dcop.arrays
         tree = build_tree(a["dom_size"], a["factor_ptr"], a["edge_var"])
-    else:
-        if kind not in ("mgm2", "dba", "mixeddsa"):
-            isolated_value = isolated_values(dcop, mode)
-        if kind in ("mgm", "mgm2", "gdba", "dba", "syncbb"):
-            var_rank = name_rank(dcop)
+    var_rank, isolated_value = _var_inputs(kind, dcop, mode)
     return make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=seed or 0,
                        var_rank=var_rank, isolated_value=isolated_value, tree=tree)
 
@@ -242,19 +247,9 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     SyncBB has no cycles to chunk: it ignores `chunk` and never calls `on_cycle` (a variable may have no value
     until the search ends).
     """
-    if algo not in ALGOS:
-        raise ValueError(f"unknown algorithm {algo!r}: expected one of {sorted(ALGOS)}")
-    kind = ALGOS[algo]
-    params = check_params(kind, algo_params)
-    stop_cycle = 1 if kind == "dpop" else 0 if kind == "syncbb" else int(params["stop_cycle"])   # DPOP: both phases in one step
-    if not stop_cycle and timeout is None and kind != "syncbb":
-        raise ValueError(f"{kind} does not stop by itself: give algo_params['stop_cycle'] or a timeout")
+    kind, params, stop_cycle = _algorithm(algo, algo_params, timeout)
     if distributed is None:
-        try:
-            import torch.distributed as dist
-            distributed = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
-        except ImportError:
-            distributed = False
+        distributed = _under_torchrun()
     if distributed and seed is None:
         seed = 0
     t0 = time.perf_counter()
@@ -287,29 +282,10 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
             engine = _default_engine(kind, layout, dcop, params, mode, precision, device, seed)
     t_packed = time.perf_counter()
     engine.init()
-    cycle, status = 0, "FINISHED"
     deadline = None if timeout is None else t0 + float(timeout)
     if kind == "syncbb":
         return _finish_syncbb(engine, dcop, deadline, infinity, precision, t0, t_packed)
-    while True:
-        n = chunk if not stop_cycle else min(chunk, stop_cycle - cycle)
-        if n <= 0:
-            break
-        expired = deadline is not None and time.perf_counter() >= deadline
-        if distributed and deadline is not None:   # every rank must leave the loop in the same round
-            import torch
-            flag = torch.tensor([int(expired)], dtype=torch.int32, device=engine.device)
-            dist.all_reduce(flag, op=dist.ReduceOp.MAX)
-            expired = bool(flag.item())
-        if expired:
-            status = "TIMEOUT"
-            break
-        engine.step(n)
-        cycle += n
-        if on_cycle is not None:
-            on_cycle(cycle, _indices(engine))
-        if kind == "dba" and engine.finished:   # every variable with neighbours finished, or stop_cycle
-            break
+    cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline, distributed, on_cycle, kind == "dba")
     if kind == "dba":                      # the rounds that changed the state
         cycle = engine.cycle
     idx = _indices(engine)
@@ -325,6 +301,142 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
             # bytes this process moved host -> device (problem arrays) and device -> host (assignment, costs)
             "h2d_bytes": int(getattr(getattr(engine, "engine", engine), "h2d_bytes", 0)),
             "d2h_bytes": int(len(idx) * 12 + 16)}
+
+
+def _algorithm(algo, algo_params, timeout):
+    """(kind, checked parameters, stop_cycle) of `algo`, or ValueError."""
+    if algo not in ALGOS:
+        raise ValueError(f"unknown algorithm {algo!r}: expected one of {sorted(ALGOS)}")
+    kind = ALGOS[algo]
+    params = check_params(kind, algo_params)
+    stop_cycle = 1 if kind == "dpop" else 0 if kind == "syncbb" else int(params["stop_cycle"])   # DPOP: both phases in one step
+    if not stop_cycle and timeout is None and kind != "syncbb":
+        raise ValueError(f"{kind} does not stop by itself: give algo_params['stop_cycle'] or a timeout")
+    return kind, params, stop_cycle
+
+
+def _under_torchrun():
+    try:
+        import torch.distributed as dist
+        return dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
+    except ImportError:
+        return False
+
+
+def _run_cycles(engine, stop_cycle, chunk, deadline, distributed=False, on_cycle=None, stops_itself=False):
+    """Step an initialised engine `chunk` cycles at a time until stop_cycle (0: none) or the deadline (checked before
+    every chunk; under torchrun every rank leaves in the same round), or, with `stops_itself`, until engine.finished.
+    Returns (cycles run, FINISHED | TIMEOUT)."""
+    cycle, status = 0, "FINISHED"
+    while True:
+        n = chunk if not stop_cycle else min(chunk, stop_cycle - cycle)
+        if n <= 0:
+            break
+        expired = deadline is not None and time.perf_counter() >= deadline
+        if distributed and deadline is not None:   # every rank must leave the loop in the same round
+            import torch
+            import torch.distributed as dist
+            flag = torch.tensor([int(expired)], dtype=torch.int32, device=engine.device)
+            dist.all_reduce(flag, op=dist.ReduceOp.MAX)
+            expired = bool(flag.item())
+        if expired:
+            status = "TIMEOUT"
+            break
+        engine.step(n)
+        cycle += n
+        if on_cycle is not None:
+            on_cycle(cycle, _indices(engine))
+        if stops_itself and engine.finished:   # DBA: every variable with neighbours finished, or stop_cycle
+            break
+    return cycle, status
+
+
+BATCHED = ("maxsum", "dsa", "adsa", "mgm", "mgm2", "gdba", "mixeddsa")
+NOT_BATCHED = {"dba": "it stops per problem by itself, so each problem would need its own finish cycle",
+               "dpop": "it computes over a pseudo-tree of the whole problem",
+               "syncbb": "it searches over an order of the whole problem"}
+
+
+def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = None, timeout: Optional[float] = None,
+                precision: str = "f32", device=None, seed: Optional[int] = None, infinity: float = float("inf"),
+                chunk: int = 50, max_vars: int = batch.MAX_BATCH_VARS,
+                engine_factory: Optional[Callable] = None) -> List[Dict[str, Any]]:
+    """Run `algo` on every problem of `problems` and return one result dict per problem, in input order, with
+    solve()'s keys.
+
+    problems  a list of anything `load` accepts, ONE problem per entry (a list of paths inside it is one DCOP split
+              over files, as in solve())
+    The problems run as disjoint unions, one engine per group: problems of one objective (min or max), cut in input
+    order so that no engine exceeds `max_vars` variables or an int32 index range; the groups run one after the other.
+    Every problem keeps its own Philox counters, name ranks and start values, so `assignment`, `status` and `cycle`
+    equal those of solve(problem, algo, algo_params, precision=precision, seed=seed) and `cost` / `violation` equal
+    them up to the order of the device reduction (per problem, fg_solution_cost_segmented).  One `seed` serves every
+    problem (solve()'s default draws with 0).
+    `timeout` bounds the whole batch: a problem whose group has not reached stop_cycle when it expires reports
+    TIMEOUT at the cycle its group reached (0 for groups that had not started).
+    `time` and `ingest_time` are the whole batch's (loading, unions, layouts and engines for ingest_time);
+    `h2d_bytes` is the problem's engine's.  `n_gpus` is 1: a batch runs on one device, never under torchrun.
+    algo: maxsum | dsa | adsa | mgm | mgm2 | gdba | mixeddsa (the fixed-length families; dba, dpop and syncbb are
+    refused).  engine_factory(kind, layout, inst, params): as in solve(), `inst` with var_rank and var_global_id.
+    """
+    kind = ALGOS.get(algo)
+    if kind in NOT_BATCHED:
+        raise ValueError(f"{kind} is not batched: {NOT_BATCHED[kind]}")
+    kind, params, stop_cycle = _algorithm(algo, algo_params, timeout)
+    problems = list(problems)
+    if not problems:
+        raise ValueError("solve_batch needs at least one problem")
+    if _under_torchrun():
+        raise ValueError("solve_batch runs on one GPU: start it without torchrun")
+    t0 = time.perf_counter()
+    deadline = None if timeout is None else t0 + float(timeout)
+    dcops = []
+    for i, p in enumerate(problems):
+        try:
+            dcops.append(load(p, seed))
+        except (ValueError, TypeError) as e:
+            raise ValueError(f"problem {i}: {e}") from e
+        batch.check_problem(i, dcops[-1])
+    results: List[Optional[Dict[str, Any]]] = [None] * len(dcops)
+    ingest_time = time.perf_counter() - t0
+    noise = params["noise"] if kind == "maxsum" else 0.0
+    for members in batch.groups(dcops, max_vars):
+        t_group = time.perf_counter()
+        mode = dcops[members[0]].objective
+        if engine_factory is not None:
+            var_inputs = lambda d: (name_rank(d), None)  # noqa: E731
+        else:
+            var_inputs = lambda d: _var_inputs(kind, d, mode)  # noqa: E731
+        u = batch.build_union(dcops, members, var_inputs, noise, seed)
+        layout = batch.union_layout(u, dcops)
+        if engine_factory is not None:
+            engine = engine_factory(kind, layout, dict(u.inst, var_rank=u.var_rank, var_global_id=u.var_global_id),
+                                    dict(params, mode=mode, seed=seed or 0))
+        else:
+            from .engine import make_engine
+            engine = make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=seed or 0,
+                                 var_rank=u.var_rank, isolated_value=u.isolated_value, var_global_id=u.var_global_id)
+        ingest_time += time.perf_counter() - t_group
+        engine.init()
+        cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline)
+        idx = _indices(engine)
+        if hasattr(engine, "solution_costs_segmented"):   # reduced per problem on the device
+            costs, violations = engine.solution_costs_segmented(u.seg_factor, u.seg_var, len(members), infinity,
+                                                                u.unary)
+        else:                                  # engine seam of the CPU tests
+            violations, costs = zip(*(solution_cost(dcops[i], idx[u.var_start[k]:u.var_start[k + 1]], infinity)
+                                      for k, i in enumerate(members)))
+        h2d = int(getattr(engine, "h2d_bytes", 0))
+        for k, i in enumerate(members):
+            v = idx[u.var_start[k]:u.var_start[k + 1]]
+            results[i] = {"status": status, "assignment": dcops[i].assignment(v), "cost": float(costs[k]),
+                          "violation": int(violations[k]), "cycle": cycle, "msg_count": 0, "msg_size": 0,
+                          "algo": kind, "precision": precision, "n_gpus": 1, "h2d_bytes": h2d,
+                          "d2h_bytes": int(len(v) * 12 + 16)}
+    total = time.perf_counter() - t0
+    for r in results:
+        r.update(time=total, ingest_time=ingest_time)
+    return results
 
 
 def _finish_syncbb(engine, dcop, deadline, infinity, precision, t0, t_packed):
@@ -360,7 +472,8 @@ def _indices(engine) -> np.ndarray:
 def main(argv=None):
     """`python -m pydcop_b200.solve --algo maxsum -p stop_cycle:100 problem.yaml` — argument names
     follow `pydcop solve` (commands/solve.py:380-470): -a/--algo, -p/--algo_params name:value,
-    -t/--timeout; prints the result as JSON."""
+    -t/--timeout; prints the result as JSON.  With --batch every file is one problem (solve_batch) and the output
+    is a JSON list in file order, each entry with "problem": its path."""
     import argparse
     ap = argparse.ArgumentParser(prog="pydcop_b200.solve")
     ap.add_argument("dcop_files", nargs="+")
@@ -381,20 +494,22 @@ def main(argv=None):
     ap.add_argument("--metrics_every", type=int, default=10, metavar="CYCLES")
     ap.add_argument("--partition", default="auto", choices=["auto", "blocks", "multilevel"],
                     help="under torchrun: how the variables are split over the GPUs")
+    ap.add_argument("--batch", action="store_true",
+                    help="every file is one problem, all solved in one engine run per objective (solve_batch); "
+                         "prints a JSON list in file order")
     args = ap.parse_args(argv)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
+    if args.batch:
+        if args.run_metrics or args.save or world > 1:
+            ap.error("--batch runs on one GPU and takes neither --run_metrics, --save nor torchrun")
+        return _main_batch(args, _algo_params(ap, args))
     if world > 1:   # launched by torchrun: one process per GPU over NCCL
         import torch
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
         dist.init_process_group("nccl", device_id=torch.device("cuda", torch.cuda.current_device()))
-    params = {}
-    for p in args.algo_params:
-        if ":" not in p:
-            ap.error(f"algo_params must be name:value, got {p!r}")
-        k, v = p.split(":", 1)
-        params[k] = v
+    params = _algo_params(ap, args)
     files = args.dcop_files if len(args.dcop_files) > 1 else args.dcop_files[0]
     dcop = load(files, args.seed)
     if args.save and rank == 0:
@@ -422,6 +537,27 @@ def main(argv=None):
         print(json.dumps(res, indent=2, sort_keys=True, default=str))
     if world > 1:
         dist.destroy_process_group()
+    return 0
+
+
+def _algo_params(ap, args):
+    params = {}
+    for p in args.algo_params:
+        if ":" not in p:
+            ap.error(f"algo_params must be name:value, got {p!r}")
+        k, v = p.split(":", 1)
+        params[k] = v
+    return params
+
+
+def _main_batch(args, params):
+    res = solve_batch(args.dcop_files, args.algo, params, args.timeout, args.precision, seed=args.seed,
+                      infinity=args.infinity)
+    for path, r in zip(args.dcop_files, res):
+        r["problem"] = path
+        if args.no_assignment:
+            r.pop("assignment")
+    print(json.dumps(res, indent=2, sort_keys=True, default=str))
     return 0
 
 
