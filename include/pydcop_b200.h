@@ -54,7 +54,7 @@
 extern "C" {
 #endif
 
-#define FG_ABI_VERSION 1
+#define FG_ABI_VERSION 2
 #define FG_MAX_ARITY 8
 #define FG_MAX_DOM 256
 
@@ -266,6 +266,8 @@ typedef struct {
    * goes to the oriented tables only for the slots whose neighbour changed; results are identical. */
   void *dev_row_cache;
   uint8_t *dev_slot_last;        /* [n_edges] */
+  const uint64_t *dev_var_seed;  /* [n_vars] optional: the Philox key of internal variable v, in place of `seed`
+                                   (a batch of problems, each run with its own seed); NULL = `seed` for all */
 } fg_dsa_desc_t;
 
 typedef struct fg_dsa *fg_dsa_t;
@@ -406,6 +408,7 @@ typedef struct {
    * phase streams these rows and reads the oriented tables only where a neighbour moved; results are identical. */
   void *dev_row_cache;
   uint8_t *dev_slot_last;         /* [n_edges] */
+  const uint64_t *dev_var_seed;   /* [n_vars] optional: Philox key of internal variable v; NULL = `seed` */
 } fg_mgm_desc_t;
 
 typedef struct fg_mgm *fg_mgm_t;
@@ -475,6 +478,7 @@ typedef struct {
   int32_t stop_cycle;             /* 0 = never; a run ends when round + 1 >= stop_cycle (mgm2.py:613) */
   int32_t reserved0;
   uint64_t seed;
+  const uint64_t *dev_var_seed;   /* [n_vars] optional: Philox key of internal variable v; NULL = `seed` */
 } fg_mgm2_desc_t;
 
 typedef struct fg_mgm2 *fg_mgm2_t;
@@ -601,6 +605,7 @@ typedef struct {
   int32_t reserved0;
   int64_t mod_size;               /* elements of dev_mod */
   uint64_t seed;
+  const uint64_t *dev_var_seed;   /* [n_vars] optional: Philox key of internal variable v; NULL = `seed` */
 } fg_gdba_desc_t;
 
 typedef struct fg_gdba *fg_gdba_t;
@@ -858,6 +863,7 @@ typedef struct {
   int32_t stop_cycle;             /* 0 = never; a run ends after stop_cycle rounds (as fg_dsa_desc_t) */
   int32_t reserved0;
   uint64_t seed;
+  const uint64_t *dev_var_seed;   /* [n_vars] optional: Philox key of internal variable v; NULL = `seed` */
 } fg_mixeddsa_desc_t;
 
 typedef struct fg_mixeddsa *fg_mixeddsa_t;

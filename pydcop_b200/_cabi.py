@@ -5,7 +5,7 @@ Fails loudly when the library is missing: there is no Python/CPU fallback for th
 import ctypes as C
 import os
 
-FG_ABI_VERSION = 1
+FG_ABI_VERSION = 2
 FG_MAX_ARITY = 8
 FG_MAX_DOM = 256
 FG_OK, FG_ERR_ARG, FG_ERR_CUDA, FG_ERR_UNSUPPORTED = 0, 1, 2, 3
@@ -66,7 +66,8 @@ class FgDsaDesc(C.Structure):
                 ("dev_value", P * 2), ("dev_value_cost", P),
                 ("mode_max", C.c_int32), ("variant", C.c_int32), ("stop_cycle", C.c_int32),
                 ("seed", C.c_uint64), ("dev_var_cost", P), ("dev_unary_off", P),
-                ("dev_row_cache", P), ("dev_slot_last", P)]
+                ("dev_row_cache", P), ("dev_slot_last", P),
+                ("dev_var_seed", P)]
 
 
 class FgMgmDesc(C.Structure):
@@ -81,7 +82,8 @@ class FgMgmDesc(C.Structure):
                 ("mode_max", C.c_int32), ("stop_cycle", C.c_int32), ("seed", C.c_uint64),
                 ("dev_tables_or", P), ("dev_slot_nbr", P), ("dev_slot_tab", P),
                 ("fast_dom", C.c_int32), ("fast_chunk", C.c_int32),
-                ("dev_row_cache", P), ("dev_slot_last", P)]
+                ("dev_row_cache", P), ("dev_slot_last", P),
+                ("dev_var_seed", P)]
 
 
 class FgMgm2Desc(C.Structure):
@@ -96,7 +98,8 @@ class FgMgm2Desc(C.Structure):
                 ("dev_committed", P), ("dev_go", P), ("dev_answer", P), ("dev_answer_value", P),
                 ("dev_answer_gain", P), ("dev_offer_off", P), ("dev_offer", P),
                 ("mode_max", C.c_int32), ("favor", C.c_int32), ("threshold", C.c_double),
-                ("stop_cycle", C.c_int32), ("reserved0", C.c_int32), ("seed", C.c_uint64)]
+                ("stop_cycle", C.c_int32), ("reserved0", C.c_int32), ("seed", C.c_uint64),
+                ("dev_var_seed", P)]
 
 
 MGM2_FAVORS = {"unilateral": 0, "no": 1, "coordinated": 2}
@@ -114,7 +117,8 @@ class FgGdbaDesc(C.Structure):
                 ("dev_new_value", P), ("dev_violated", P), ("dev_breakout", P), ("dev_mod", P), ("dev_mod_off", P),
                 ("mode_max", C.c_int32), ("modifier", C.c_int32), ("violation", C.c_int32),
                 ("increase_mode", C.c_int32), ("stop_cycle", C.c_int32), ("reserved0", C.c_int32),
-                ("mod_size", C.c_int64), ("seed", C.c_uint64)]
+                ("mod_size", C.c_int64), ("seed", C.c_uint64),
+                ("dev_var_seed", P)]
 
 
 class FgDpopLaunch(C.Structure):
@@ -173,7 +177,7 @@ class FgMixedDsaDesc(C.Structure):
                 ("dev_h_best", P), ("dev_branch", P),
                 ("proba_hard", C.c_double), ("proba_soft", C.c_double),
                 ("mode_max", C.c_int32), ("variant", C.c_int32), ("stop_cycle", C.c_int32),
-                ("reserved0", C.c_int32), ("seed", C.c_uint64)]
+                ("reserved0", C.c_int32), ("seed", C.c_uint64), ("dev_var_seed", P)]
 
 
 MIXEDDSA_VARIANTS = {"A": 0, "B": 1, "C": 2}

@@ -5,10 +5,12 @@ several problems into one layout changes nothing any problem computes, as long a
 reads is the problem's own: the Philox counter (`var_global_id`: the variable's index in its own problem, the
 mechanism the sharded engines use the other way round, DESIGN.md §6), the name rank (only ever compared between
 neighbours) and the start value of a variable without neighbours.  The union's canonical variable order is the
-concatenation of the problems', so problem k's values are one slice of the result.
+concatenation of the problems', so problem k's values are one slice of the result.  Problems with seeds of their own
+also carry their own Philox key (`var_seed`: the problem's seed on each of its variables), so one problem can run many
+times in one union, once per seed.
 """
 from dataclasses import dataclass
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence, Union as AnyOf
 
 import numpy as np
 
@@ -75,6 +77,7 @@ class Union:
     unary: np.ndarray                    # the variables' own costs, without noise: what the solution cost adds
     var_start: np.ndarray                # [n + 1] first variable of every problem, then the total
     var_global_id: np.ndarray            # each variable's index in its own problem
+    var_seed: Optional[np.ndarray]       # each variable's problem's seed (uint64), None when all problems share one
     var_rank: Optional[np.ndarray]       # each variable's name rank in its own problem
     isolated_value: Optional[np.ndarray]  # start value of the variables without neighbours, per problem
     seg_factor: np.ndarray               # problem (0..n-1) of every canonical factor
@@ -82,11 +85,15 @@ class Union:
 
 
 def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs, noise: float = 0.0,
-                seed: Optional[int] = None) -> Union:
+                seed: AnyOf[None, int, Sequence[int]] = None) -> Union:
     """Concatenate the problems `members` of `dcops`: variable, edge and table indices are offset by the problems
-    before.  var_inputs(dcop) -> (var_rank or None, isolated_value or None), each problem's own; `noise`: MaxSum's, drawn
-    per problem with `seed` exactly as solve() draws it."""
+    before.  var_inputs(dcop) -> (var_rank or None, isolated_value or None), each problem's own; `seed`: one for every
+    member, or a sequence with one per member; `noise`: MaxSum's, drawn per problem with its seed exactly as solve()
+    draws it."""
     parts = [dcops[i].arrays for i in members]
+    seeds = [seed] * len(members) if seed is None or isinstance(seed, (int, np.integer)) else list(seed)
+    if len(seeds) != len(members):
+        raise ValueError(f"{len(seeds)} seeds for {len(members)} problems")
     n_var = np.array([len(a["dom_size"]) for a in parts], dtype=np.int64)
     n_fac = np.array([len(a["factor_ptr"]) - 1 for a in parts], dtype=np.int64)
     n_edge = np.array([len(a["edge_var"]) for a in parts], dtype=np.int64)
@@ -103,7 +110,8 @@ def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs, 
                 edge_var=np.concatenate([np.asarray(a["edge_var"], dtype=np.int64) + o
                                          for a, o in zip(parts, v0[:-1])]).astype(np.int32),
                 table_off=ptr("table_off", t0), tables=np.concatenate([np.asarray(a["tables"]) for a in parts]),
-                unary=(np.concatenate([ingest.add_noise(a["unary"], noise, seed) for a in parts]) if noise else unary),
+                unary=(np.concatenate([ingest.add_noise(a["unary"], noise, s) for a, s in zip(parts, seeds)])
+                       if noise else unary),
                 var_ptr=ptr("var_ptr", e0).astype(np.int32),
                 var_edge=np.concatenate([np.asarray(a["var_edge"], dtype=np.int64) + o
                                          for a, o in zip(parts, e0[:-1])]).astype(np.int32),
@@ -112,6 +120,8 @@ def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs, 
     seg = np.arange(len(members), dtype=np.int32)
     return Union(members=list(members), inst=inst, unary=unary, var_start=v0,
                  var_global_id=np.concatenate([np.arange(n, dtype=np.int32) for n in n_var]),
+                 var_seed=(None if len(set(seeds)) == 1 else
+                           np.repeat(np.array([int(s) & (2 ** 64 - 1) for s in seeds], dtype=np.uint64), n_var)),
                  var_rank=None if ranks[0] is None else np.concatenate(ranks).astype(np.int32),
                  isolated_value=None if isos[0] is None else np.concatenate(isos).astype(np.int32),
                  seg_factor=np.repeat(seg, n_fac), seg_var=np.repeat(seg, n_var))

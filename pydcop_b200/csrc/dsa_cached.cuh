@@ -34,6 +34,7 @@ __global__ void __launch_bounds__(DsaCachedCfg<T, D>::THREADS)
 k_dsa_step_cached(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *__restrict__ slot_nbr,
                   const int64_t *__restrict__ slot_tab, const T *__restrict__ slot_opt, const T *__restrict__ tables_or,
                   const uint8_t *__restrict__ has_nbr, const double *__restrict__ prob, const int32_t *__restrict__ var_id,
+                  const uint64_t *__restrict__ var_seed,
                   const int32_t *__restrict__ val, int32_t *__restrict__ val_next, T *__restrict__ val_cost, int mode_max,
                   int variant, uint64_t seed, uint32_t cycle, const T *__restrict__ var_cost,
                   const int64_t *__restrict__ unary_off, T *row_cache, uint8_t *slot_last) {
@@ -167,7 +168,7 @@ k_dsa_step_cached(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t
   int nvv = cur;
   if (attempt) {  // probabilistic_change, dsa.py:407-417
     uint32_t b[4];
-    philox4x32_10((uint32_t)var_id[v], cycle, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), b);
+    philox_draw((uint32_t)var_id[v], cycle, 0u, fg_var_seed(var_seed, v, seed), b);
     if (prob[v] > philox_u53(b)) {
       int pick = philox_choice(b, drop_cur ? nbest - 1 : nbest);
       bool done = false;
@@ -199,8 +200,8 @@ inline bool dsa_cached_step(const fg_dsa_desc_t &d, const int32_t *val, int32_t 
     const unsigned blocks = (unsigned)((d.n_vars + Cfg::NV - 1) / Cfg::NV);                                           \
     k_dsa_step_cached<T, n><<<blocks, Cfg::THREADS, 0, st>>>(                                                         \
         d.n_vars, d.dev_var_ptr, d.dev_slot_nbr, d.dev_slot_tab, (const T *)d.dev_slot_opt, (const T *)d.dev_tables_or, \
-        d.dev_has_nbr, d.dev_prob, d.dev_var_id, val, val_next, (T *)d.dev_value_cost, d.mode_max, d.variant, d.seed,   \
-        cycle, (const T *)d.dev_var_cost, d.dev_unary_off, (T *)d.dev_row_cache, d.dev_slot_last);                     \
+        d.dev_has_nbr, d.dev_prob, d.dev_var_id, d.dev_var_seed, val, val_next, (T *)d.dev_value_cost, d.mode_max,       \
+        d.variant, d.seed, cycle, (const T *)d.dev_var_cost, d.dev_unary_off, (T *)d.dev_row_cache, d.dev_slot_last);                     \
     ++launches;                                                                                                       \
     return true;                                                                                                      \
   }

@@ -17,6 +17,7 @@ k_dsa_step_bin(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *_
                const int64_t *__restrict__ slot_tab, const T *__restrict__ slot_opt,
                const T *__restrict__ tables_or, const uint8_t *__restrict__ has_nbr,
                const double *__restrict__ prob, const int32_t *__restrict__ var_id,
+               const uint64_t *__restrict__ var_seed,
                const int32_t *__restrict__ val, int32_t *__restrict__ val_next, T *__restrict__ val_cost,
                int mode_max, int variant, uint64_t seed, uint32_t cycle, const T *__restrict__ var_cost,
                const int64_t *__restrict__ unary_off) {
@@ -76,7 +77,7 @@ k_dsa_step_bin(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *_
   int nv = cur;
   if (attempt) {  // probabilistic_change, dsa.py:407-417
     uint32_t b[4];
-    philox4x32_10((uint32_t)var_id[v], cycle, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), b);
+    philox_draw((uint32_t)var_id[v], cycle, 0u, fg_var_seed(var_seed, v, seed), b);
     if (prob[v] > philox_u53(b)) {
       int pick = philox_choice(b, drop_cur ? nbest - 1 : nbest);
       bool done = false;
@@ -104,8 +105,9 @@ inline bool dsa_fast_step(const fg_dsa_desc_t &d, const std::vector<fg_class_t> 
   case n:                                                                                                  \
     k_dsa_step_bin<T, n><<<blocks, 128, 0, st>>>(d.n_vars, d.dev_var_ptr, d.dev_slot_nbr, d.dev_slot_tab,   \
                                                  (const T *)d.dev_slot_opt, (const T *)d.dev_tables_or,     \
-                                                 d.dev_has_nbr, d.dev_prob, d.dev_var_id, val, val_next,    \
-                                                 (T *)d.dev_value_cost, d.mode_max, d.variant, d.seed, cycle, \
+                                                 d.dev_has_nbr, d.dev_prob, d.dev_var_id, d.dev_var_seed,   \
+                                                 val, val_next, (T *)d.dev_value_cost, d.mode_max, d.variant,   \
+                                                 d.seed, cycle,                                                 \
                                                  (const T *)d.dev_var_cost, d.dev_unary_off);               \
     ++launches;                                                                                            \
     return true;

@@ -8,6 +8,7 @@ struct DsaSide {
   const int32_t *dom_size, *var_id, *edge_var, *edge_class, *var_ptr, *slot_edge;
   const uint8_t *has_nbr;
   const double *prob;
+  const uint64_t *var_seed;  // [n_vars] Philox key of each variable, NULL: the run's seed
 };
 
 // find_optimum (relations.py:1367-1400): optimum of the whole table of each constraint
@@ -30,7 +31,7 @@ __global__ void k_dsa_init(DsaSide g, int n_vars, uint64_t seed, int32_t *__rest
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= n_vars || g.has_nbr[v] != 1) return;
   uint32_t b[4];
-  philox4x32_10((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), b);
+  philox_draw((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, 0u, fg_var_seed(g.var_seed, v, seed), b);
   value[v] = philox_choice(b, g.dom_size[v]);
 }
 
@@ -100,7 +101,7 @@ k_dsa_step_generic(DsaSide g, int n_vars, const T *__restrict__ tables,
   int nv = cur;
   if (attempt) {  // probabilistic_change, dsa.py:407-417
     uint32_t b[4];
-    philox4x32_10((uint32_t)g.var_id[v], cycle, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), b);
+    philox_draw((uint32_t)g.var_id[v], cycle, 0u, fg_var_seed(g.var_seed, v, seed), b);
     if (g.prob[v] > philox_u53(b)) {
       int n = drop_cur ? nbest - 1 : nbest;
       int pick = philox_choice(b, n);

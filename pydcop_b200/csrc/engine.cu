@@ -713,7 +713,8 @@ extern "C" int fg_dsa_create(const fg_dsa_desc_t *desc, fg_dsa_t *out) {
                              FG_FIELD(d, dev_con_opt), FG_FIELD(d, dev_tables_or), FG_FIELD(d, dev_slot_nbr),
                              FG_FIELD(d, dev_slot_tab), FG_FIELD(d, dev_slot_opt), FG_FIELD(d, dev_value[0]),
                              FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_value_cost), FG_FIELD(d, dev_var_cost),
-                             FG_FIELD(d, dev_unary_off), FG_FIELD(d, dev_row_cache), FG_FIELD(d, dev_slot_last)});
+                             FG_FIELD(d, dev_unary_off), FG_FIELD(d, dev_row_cache), FG_FIELD(d, dev_slot_last),
+                             FG_FIELD(d, dev_var_seed)});
   if (rc != FG_OK) return rc;
   {  // experiment knob: L2 -> DRAM fetch granularity hint (32 | 64 | 128 bytes) for the sparse row reads
     const int g = fg_env_int("PYDCOP_B200_L2_FETCH", 0);
@@ -729,7 +730,7 @@ extern "C" const char *fg_dsa_last_error(fg_dsa_t h) { return fg_last_error(h); 
 static DsaSide dsa_side(const fg_dsa *h) {
   const fg_dsa_desc_t &d = h->d;
   return DsaSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_edge_var, d.dev_edge_class, d.dev_var_ptr,
-                 d.dev_slot_edge, d.dev_has_nbr, d.dev_prob};
+                 d.dev_slot_edge, d.dev_has_nbr, d.dev_prob, d.dev_var_seed};
 }
 
 template <typename T>

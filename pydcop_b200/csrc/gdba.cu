@@ -13,7 +13,8 @@ static inline unsigned gdba_blocks(int64_t n, int t) { return (unsigned)((n + t 
 static MgmSide gdba_side(const fg_gdba *h) {
   const fg_gdba_desc_t &d = h->d;
   return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr};
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr,
+                 d.dev_var_seed};
 }
 
 extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
@@ -65,7 +66,8 @@ extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
                              FG_FIELD(d, dev_nbr_idx), FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_value[0]),
                              FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_cost), FG_FIELD(d, dev_has_cost),
                              FG_FIELD(d, dev_improve), FG_FIELD(d, dev_new_value), FG_FIELD(d, dev_violated),
-                             FG_FIELD(d, dev_breakout), FG_FIELD(d, dev_mod), FG_FIELD(d, dev_mod_off)});
+                             FG_FIELD(d, dev_breakout), FG_FIELD(d, dev_mod), FG_FIELD(d, dev_mod_off),
+                             FG_FIELD(d, dev_var_seed)});
   if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }

@@ -114,7 +114,7 @@ k_gdba_eval(MgmSide g, int n_vars, const T *__restrict__ tables, const T *__rest
   int nv = cur;
   if (mode_max ? (gn < (T)0) : (gn > (T)0)) {
     uint32_t b[4];
-    philox_draw((uint32_t)g.var_id[v], cycle, 0u, seed, b);
+    philox_draw((uint32_t)g.var_id[v], cycle, 0u, fg_var_seed(g.var_seed, v, seed), b);
     int pick = philox_choice(b, nbest);
     for (int x = 0; x < d; ++x) {
       if (rel[x] == best) {

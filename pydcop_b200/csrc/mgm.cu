@@ -21,7 +21,8 @@ static inline unsigned mgm_blocks(int64_t n, int t) { return (unsigned)((n + t -
 static MgmSide mgm_side(const fg_mgm *h) {
   const fg_mgm_desc_t &d = h->d;
   return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off};
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off,
+                 d.dev_var_seed};
 }
 
 extern "C" int fg_mgm_create(const fg_mgm_desc_t *desc, fg_mgm_t *out) {
@@ -42,7 +43,7 @@ extern "C" int fg_mgm_create(const fg_mgm_desc_t *desc, fg_mgm_t *out) {
                              FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_value), FG_FIELD(d, dev_cost),
                              FG_FIELD(d, dev_has_cost), FG_FIELD(d, dev_gain), FG_FIELD(d, dev_new_value),
                              FG_FIELD(d, dev_tables_or), FG_FIELD(d, dev_slot_nbr), FG_FIELD(d, dev_slot_tab),
-                             FG_FIELD(d, dev_row_cache), FG_FIELD(d, dev_slot_last)});
+                             FG_FIELD(d, dev_row_cache), FG_FIELD(d, dev_slot_last), FG_FIELD(d, dev_var_seed)});
   if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }

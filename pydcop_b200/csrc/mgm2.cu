@@ -32,7 +32,8 @@ static inline unsigned mgm2_blocks(int64_t n, int t) { return (unsigned)((n + t 
 static MgmSide mgm2_side(const fg_mgm2 *h) {
   const fg_mgm2_desc_t &d = h->d;
   return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr};
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr,
+                 d.dev_var_seed};
 }
 
 extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
@@ -74,7 +75,7 @@ extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
                              FG_FIELD(d, dev_potential_value), FG_FIELD(d, dev_local_cost), FG_FIELD(d, dev_offerer),
                              FG_FIELD(d, dev_partner), FG_FIELD(d, dev_committed), FG_FIELD(d, dev_go),
                              FG_FIELD(d, dev_answer), FG_FIELD(d, dev_answer_value), FG_FIELD(d, dev_answer_gain),
-                             FG_FIELD(d, dev_offer_off), FG_FIELD(d, dev_offer)});
+                             FG_FIELD(d, dev_offer_off), FG_FIELD(d, dev_offer), FG_FIELD(d, dev_var_seed)});
   if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }

@@ -104,7 +104,7 @@ __device__ __forceinline__ void mgm2_init_at(int v, const MgmSide &g, const T *_
                                              uint8_t *__restrict__ has_cost) {
   const int d = g.dom_size[v];
   uint32_t b[4];
-  philox_draw((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, MGM2_PURPOSE_INIT, seed, b);
+  philox_draw((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, MGM2_PURPOSE_INIT, fg_var_seed(g.var_seed, v, seed), b);
   if (g.nbr_ptr[v + 1] != g.nbr_ptr[v]) {
     has_cost[v] = 0;
     value[v] = (init_value && init_value[v] >= 0) ? init_value[v] : philox_choice(b, d);
@@ -145,6 +145,7 @@ __device__ __forceinline__ void mgm2_value_at(int v, const MgmSide &g, const T *
   const int cur = val[v];
   const int d = g.dom_size[v];
   const uint32_t vid = (uint32_t)g.var_id[v];
+  const uint64_t key = fg_var_seed(g.var_seed, v, seed);   // every connected variable draws its offer coin
   T rel[FG_MAX_DOM];
   mgm2_local_costs(g, tables, val, v, d, rel);
   const T cst = rel[cur];  // _current_local_cost
@@ -158,7 +159,7 @@ __device__ __forceinline__ void mgm2_value_at(int v, const MgmSide &g, const T *
   int pv = cur;
   if (mode_max ? (pg < (T)0) : (pg > (T)0)) {
     uint32_t b[4];
-    philox_draw(vid, cycle, MGM2_PURPOSE_VALUE, seed, b);
+    philox_draw(vid, cycle, MGM2_PURPOSE_VALUE, key, b);
     pv = mgm2_nth_best(rel, d, best, philox_choice(b, nbest));
   }
   gain[v] = pg;
@@ -167,7 +168,7 @@ __device__ __forceinline__ void mgm2_value_at(int v, const MgmSide &g, const T *
   answer[v] = 0;
   // offerer coin and partner pick (one Philox block)
   uint32_t b[4];
-  philox_draw(vid, cycle, MGM2_PURPOSE_OFFER, seed, b);
+  philox_draw(vid, cycle, MGM2_PURPOSE_OFFER, key, b);
   if (!(philox_u53(b) < threshold)) {
     offerer[v] = 0;
     partner[v] = -1;
@@ -272,13 +273,13 @@ __device__ __forceinline__ void mgm2_answer_at(int v, const MgmSide &g, const T 
         commit = true;
       } else if (favor == FG_MGM2_FAVOR_NO) {
         uint32_t b[4];
-        philox_draw((uint32_t)g.var_id[v], cycle, MGM2_PURPOSE_FAVOR, seed, b);
+        philox_draw((uint32_t)g.var_id[v], cycle, MGM2_PURPOSE_FAVOR, fg_var_seed(g.var_seed, v, seed), b);
         commit = philox_u53(b) > 0.5;
       }
     }
     if (!commit) return;
     uint32_t b[4];
-    philox_draw((uint32_t)g.var_id[v], cycle, MGM2_PURPOSE_PICK, seed, b);
+    philox_draw((uint32_t)g.var_id[v], cycle, MGM2_PURPOSE_PICK, fg_var_seed(g.var_seed, v, seed), b);
     pick = philox_choice(b, nb);
   }
   committed[v] = 1;

@@ -87,7 +87,7 @@ k_mgm_gain_bin(MgmSide g, int n_vars, const int32_t *__restrict__ slot_nbr, cons
   int nv = cur;
   if (mode_max ? (gn < (T)0) : (gn > (T)0)) {  // mgm.py:382-385
     uint32_t b[4];
-    philox4x32_10((uint32_t)g.var_id[v], cycle, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), b);
+    philox_draw((uint32_t)g.var_id[v], cycle, 0u, fg_var_seed(g.var_seed, v, seed), b);
     int pick = philox_choice(b, nbest);
     bool done = false;
 #pragma unroll

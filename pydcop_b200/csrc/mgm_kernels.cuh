@@ -14,6 +14,7 @@ struct MgmSide {
   const int32_t *dom_size, *var_id, *var_rank, *edge_var, *edge_class, *var_ptr, *slot_edge;
   const int32_t *nbr_ptr, *nbr_idx;
   const int64_t *unary_off;
+  const uint64_t *var_seed;  // [n_vars] Philox key of each variable, NULL: the run's seed
 };
 
 // on_start (mgm.py:296-310): connected variables take initial_value or random.choice(domain)
@@ -24,7 +25,7 @@ __global__ void k_mgm_init(MgmSide g, int n_vars, const int32_t *__restrict__ in
   has_cost[v] = 0;
   if (init_value && init_value[v] >= 0) { value[v] = init_value[v]; return; }
   uint32_t b[4];
-  philox4x32_10((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), b);
+  philox_draw((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, 0u, fg_var_seed(g.var_seed, v, seed), b);
   value[v] = philox_choice(b, g.dom_size[v]);
 }
 
@@ -94,7 +95,7 @@ k_mgm_gain(MgmSide g, int n_vars, const T *__restrict__ tables, const T *__restr
   int nv = cur;
   if (mode_max ? (gn < (T)0) : (gn > (T)0)) {  // mgm.py:382-385
     uint32_t b[4];
-    philox4x32_10((uint32_t)g.var_id[v], cycle, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), b);
+    philox_draw((uint32_t)g.var_id[v], cycle, 0u, fg_var_seed(g.var_seed, v, seed), b);
     int pick = philox_choice(b, nbest);
     for (int x = 0; x < d; ++x) {
       if (rel[x] == best) {

@@ -23,7 +23,8 @@ static inline unsigned mixeddsa_blocks(int64_t n, int t) { return (unsigned)((n 
 static MgmSide mixeddsa_side(const fg_mixeddsa *h) {
   const fg_mixeddsa_desc_t &d = h->d;
   return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, nullptr, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off};
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off,
+                 d.dev_var_seed};
 }
 
 // stop_cycle as fg_dsa_*: a run ends after stop_cycle rounds (dsa.py:352)
@@ -70,7 +71,7 @@ extern "C" int fg_mixeddsa_create(const fg_mixeddsa_desc_t *desc, fg_mixeddsa_t 
                              FG_FIELD(d, dev_soft_end), FG_FIELD(d, dev_nbr_ptr), FG_FIELD(d, dev_nbr_idx),
                              FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_con_opt), FG_FIELD(d, dev_value[0]),
                              FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_cost), FG_FIELD(d, dev_has_cost),
-                             FG_FIELD(d, dev_h_best), FG_FIELD(d, dev_branch)});
+                             FG_FIELD(d, dev_h_best), FG_FIELD(d, dev_branch), FG_FIELD(d, dev_var_seed)});
   if (rc != FG_OK) return rc;
   return fg_upload_classes(h);
 }

@@ -46,7 +46,7 @@ __global__ void k_mixeddsa_init(MgmSide g, int n_vars, const int32_t *__restrict
     return;
   }
   uint32_t b[4];
-  philox_draw((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, 0u, seed, b);
+  philox_draw((uint32_t)g.var_id[v], FG_PHILOX_INIT_CYCLE, 0u, fg_var_seed(g.var_seed, v, seed), b);
   value[v] = philox_choice(b, g.dom_size[v]);
 }
 
@@ -168,7 +168,7 @@ k_mixeddsa_step(MgmSide g, int n_vars, const T *__restrict__ tables, const T *__
   int moved = 0;
   if (p > 0.0) {
     uint32_t b[4];
-    philox_draw((uint32_t)g.var_id[v], cycle, 0u, seed, b);
+    philox_draw((uint32_t)g.var_id[v], cycle, 0u, fg_var_seed(g.var_seed, v, seed), b);
     if (p > philox_u53(b)) {
       // bests: `first` (the value that set the best last) and every later value with the same (H, C)
       int pick = philox_choice(b, drop_cur ? nbest - 1 : nbest);

@@ -32,3 +32,9 @@ __host__ __device__ __forceinline__ void philox_draw(uint32_t var, uint32_t cycl
                                                      uint32_t out[4]) {
   philox4x32_10(var, cycle, purpose, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), out);
 }
+
+// Philox key of internal variable v: its own entry of var_seed (a batch of problems, each with its own seed), or the
+// run's one seed when var_seed is NULL.  Read at the draw only, so the paths that draw nothing load nothing.
+__host__ __device__ __forceinline__ uint64_t fg_var_seed(const uint64_t *var_seed, int v, uint64_t seed) {
+  return var_seed ? var_seed[v] : seed;
+}

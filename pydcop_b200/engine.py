@@ -103,7 +103,8 @@ def host_state(state):
 
 
 _TORCH_DTYPES = {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64,
-                 np.dtype(np.int32): torch.int32, np.dtype(np.int64): torch.int64, np.dtype(np.uint8): torch.uint8}
+                 np.dtype(np.int32): torch.int32, np.dtype(np.int64): torch.int64, np.dtype(np.uint8): torch.uint8,
+                 np.dtype(np.uint64): torch.uint64}
 
 
 class _EngineBase:
@@ -463,12 +464,14 @@ class DsaEngine(_CycleEngine):
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
                  probability=0.7, p_mode="fixed", variant="B", stop_cycle=0, seed=0,
-                 isolated_value=None, var_global_id=None, frozen=None, var_costs=False):
+                 isolated_value=None, var_global_id=None, frozen=None, var_costs=False, var_seed=None):
         """var_costs: A-DSA's decision (pydcop/algorithms/adsa.py:344-377: every candidate value carries the
         variable's own cost, the current cost does not); False: DSA.
         var_global_id / frozen (canonical order) serve the multi-GPU partition
         (pydcop_b200/multigpu_dsa.py): the Philox counter of each variable when the layout is a
-        shard of a larger problem, and the ghost variables whose value is only copied through."""
+        shard of a larger problem, and the ghost variables whose value is only copied through.
+        var_seed (canonical order): the Philox key of each variable when the layout holds several problems with
+        seeds of their own (pydcop_b200.batch); default: `seed` for every variable."""
         L = layout
         tdt = self._open(layout, device, precision)
         if variant not in _cabi.DSA_VARIANTS:
@@ -518,6 +521,7 @@ class DsaEngine(_CycleEngine):
             self.value_cost = z(L.n_vars, tdt)
             self.var_cost = self._dev(L.unary, tdt) if var_costs else None
             self.unary_off = self._dev(L.unary_off, torch.int64) if var_costs else None
+            self.var_seed = None if var_seed is None else self._dev(_var_seeds(L, var_seed), torch.uint64)
         # fast path: every constraint binary over ONE domain size -> oriented tables, one contiguous
         # row per incidence (transposed copy for scope position 0)
         self.tables_or = self.slot_nbr = self.slot_tab = self.slot_opt = None
@@ -535,7 +539,7 @@ class DsaEngine(_CycleEngine):
         fill_desc(d, {k: getattr(self, k) for k in (
             "tables", "dom_size", "var_id", "edge_var", "edge_class", "var_ptr", "slot_edge", "has_nbr", "prob",
             "con_opt", "value", "value_cost", "tables_or", "slot_nbr", "slot_tab", "slot_opt", "var_cost", "unary_off",
-            "row_cache", "slot_last")})
+            "row_cache", "slot_last", "var_seed")})
         d.fast_dom = fast_dom
         d.mode_max, d.variant = int(mode == "max"), _cabi.DSA_VARIANTS[variant]
         d.stop_cycle, d.seed = int(stop_cycle), int(seed) & (2 ** 64 - 1)
@@ -631,19 +635,30 @@ def _seed(seed):
     return int(seed) & (2 ** 64 - 1)
 
 
-def _set_global_ids(inputs, layout, var_global_id):
+def _var_seeds(layout, var_seed):
+    """var_seed (canonical order, any ints) as uint64 in internal order, each masked as _seed masks the scalar seed."""
+    keys = (np.asarray(var_seed, dtype=object) & (2 ** 64 - 1)).astype(np.uint64)
+    return _per_var(layout, keys[layout.var_order], np.uint64)
+
+
+def _set_global_ids(inputs, layout, var_global_id, var_seed=None):
     """Replace the uploaded var_id (the canonical index) by var_global_id (canonical order), the Philox counter of
-    every variable when the layout is part of a larger problem (a shard) or one problem of a union (a batch)."""
+    every variable when the layout is part of a larger problem (a shard) or one problem of a union (a batch).  Add
+    var_seed (canonical order), the Philox key of every variable when the problems of a union have seeds of their
+    own; without it the descriptor's dev_var_seed stays NULL and every draw is keyed by the scalar seed."""
     if var_global_id is not None:
         inputs["var_id"] = _per_var(layout, np.asarray(var_global_id, dtype=np.int32)[layout.var_order], np.int32)
+    if var_seed is not None:
+        inputs["var_seed"] = _var_seeds(layout, var_seed)
     return inputs
 
 
 def mgm_plan(layout: FactorGraphLayout, precision="f32", mode="min", stop_cycle=0, seed=0, var_rank=None,
-             isolated_value=None, var_global_id=None):
+             isolated_value=None, var_global_id=None, var_seed=None):
     """MgmEngine's host-array plan: (inputs: name -> array in its final dtype, in upload order; state: name ->
     (length, dtype, fill); the descriptor's scalar fields).  Every name is a dev_<name> field of fg_mgm_desc_t.
-    var_global_id (canonical order): the Philox counter of every variable (default: the canonical index)."""
+    var_global_id (canonical order): the Philox counter of every variable (default: the canonical index); var_seed
+    (canonical order): the Philox key of every variable (default: `seed` for all)."""
     L = layout
     dt = PRECISIONS[precision][2]
     h = mgm_host_arrays(L, mode, var_rank, isolated_value)
@@ -652,7 +667,7 @@ def mgm_plan(layout: FactorGraphLayout, precision="f32", mode="min", stop_cycle=
                   unary_off=np.ascontiguousarray(L.unary_off, np.int64), **nb,
                   value=_per_var(L, h["value0"], np.int32), cost=_per_var(L, h["cost0"], dt),
                   has_cost=_per_var(L, ~h["has_nbr"], np.uint8))
-    _set_global_ids(inputs, L, var_global_id)
+    _set_global_ids(inputs, L, var_global_id, var_seed)
     state = dict(gain=(L.n_vars, dt, 0), new_value=(L.n_vars, np.int32, 0))
     return inputs, state, dict(mode_max=int(mode == "max"), stop_cycle=int(stop_cycle), seed=_seed(seed))
 
@@ -695,13 +710,16 @@ class MgmEngine(_LocalSearchEngine):
                    default: argopt of the own cost with ties broken on the value index
     var_global_id  canonical order: the Philox counter of each variable when the layout holds several problems
                    (pydcop_b200.batch; default: the canonical index)
+    var_seed       canonical order: the Philox key of each variable when those problems have seeds of their own
+                   (default: `seed` for every variable)
     `break_mode` is accepted for the reference's signature; its 'random' branch is dead code in
     the reference (mgm.py:541 compares with the `random` module) and both settings act as 'lexic'.
     """
     FAMILY = "mgm"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
-                 stop_cycle=0, seed=0, break_mode="lexic", var_rank=None, isolated_value=None, var_global_id=None):
+                 stop_cycle=0, seed=0, break_mode="lexic", var_rank=None, isolated_value=None, var_global_id=None,
+                 var_seed=None):
         L = layout
         tdt = self._open(layout, device, precision)
         if break_mode not in ("lexic", "random"):
@@ -709,7 +727,7 @@ class MgmEngine(_LocalSearchEngine):
         if mode not in ("min", "max"):
             raise ValueError(f"invalid mode {mode!r}")
         inputs, state, scalars = mgm_plan(L, precision, mode, stop_cycle, seed, var_rank, isolated_value,
-                                          var_global_id)
+                                          var_global_id, var_seed)
         self.has_nbr_host = np.diff(inputs["nbr_ptr"]) > 0
         t = self._upload(inputs, state)
         self.__dict__.update(t)
@@ -764,15 +782,16 @@ def mgm2_offer_offsets(layout: FactorGraphLayout, nbr_ptr, nbr_idx):
 
 
 def mgm2_plan(layout: FactorGraphLayout, precision="f32", mode="min", threshold=0.5, favor="unilateral",
-              stop_cycle=0, seed=0, var_rank=None, var_global_id=None):
+              stop_cycle=0, seed=0, var_rank=None, var_global_id=None, var_seed=None):
     """Mgm2Engine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan.  var_global_id (canonical
-    order): the Philox counter of every variable when the layout is a shard of a larger problem."""
+    order): the Philox counter of every variable when the layout is a shard of a larger problem; var_seed as
+    mgm_plan."""
     L = layout
     dt = PRECISIONS[precision][2]
     h = mgm_host_arrays(L, mode, var_rank)
     offer_off, offer_size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
     inputs = _set_global_ids(dict(**_neighbourhood_inputs(L, dt, h), offer_off=_per_var(L, offer_off, np.int64)),
-                             L, var_global_id)
+                             L, var_global_id, var_seed)
     n = L.n_vars
     state = dict(value=(n, np.int32, 0), potential_value=(n, np.int32, 0), answer_value=(n, np.int32, 0),
                  partner=(n, np.int32, -1), cost=(n, dt, 0), gain=(n, dt, 0), local_cost=(n, dt, 0),
@@ -793,13 +812,15 @@ class Mgm2Engine(_LocalSearchEngine):
                tie break of mgm2.py:944-949 (default: the canonical index)
     var_global_id  canonical order: the Philox counter of each variable when the layout is one rank's shard
                of a larger problem (pydcop_b200/multigpu_mgm2.py; default: the canonical index)
+    var_seed   canonical order: the Philox key of each variable, as MgmEngine (default: `seed` for every variable)
     Variable costs are not part of MGM-2's costs (assignment_cost without them); a variable without
     neighbours takes a drawn value among its best over its unary constraints on the device.
     """
     FAMILY = "mgm2"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
-                 threshold=0.5, favor="unilateral", stop_cycle=0, seed=0, var_rank=None, var_global_id=None):
+                 threshold=0.5, favor="unilateral", stop_cycle=0, seed=0, var_rank=None, var_global_id=None,
+                 var_seed=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -807,7 +828,7 @@ class Mgm2Engine(_LocalSearchEngine):
         if favor not in _cabi.MGM2_FAVORS:
             raise ValueError(f"invalid favor {favor!r}: expected one of {sorted(_cabi.MGM2_FAVORS)}")
         inputs, state, scalars = mgm2_plan(L, precision, mode, threshold, favor, stop_cycle, seed, var_rank,
-                                           var_global_id)
+                                           var_global_id, var_seed)
         self.nbr_ptr_host, self.nbr_idx_host = inputs["nbr_ptr"], inputs["nbr_idx"]
         self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
         self.offer_bytes = state["offer"][0] * np.dtype(self.np_dtype).itemsize
@@ -945,7 +966,7 @@ def gdba_modifiers_view(h, mods, base_mod, increase_mode):
 
 
 def gdba_plan(layout: FactorGraphLayout, precision="f32", mode="min", modifier="A", violation="NZ", increase_mode="E",
-              stop_cycle=0, seed=0, var_rank=None, isolated_value=None, var_global_id=None):
+              stop_cycle=0, seed=0, var_rank=None, isolated_value=None, var_global_id=None, var_seed=None):
     """GdbaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
     buffer, and viol_ref / mod_off are None where the modes do not read them."""
     L = layout
@@ -959,7 +980,7 @@ def gdba_plan(layout: FactorGraphLayout, precision="f32", mode="min", modifier="
                   viol_ref=None if g["viol_ref"] is None else np.ascontiguousarray(g["viol_ref"], dt), **nb,
                   value=[value0, value0.copy()], cost=_per_var(L, h["cost0"], dt), has_cost=_per_var(L, ~h["has_nbr"], np.uint8),
                   mod_off=None if g["mod_off"] is None else np.ascontiguousarray(g["mod_off"], np.int64))
-    _set_global_ids(inputs, L, var_global_id)
+    _set_global_ids(inputs, L, var_global_id, var_seed)
     n = L.n_vars
     state = dict(improve=(n, dt, 0), new_value=(n, np.int32, 0), breakout=(n, np.uint8, 0),
                  violated=(L.n_edges, np.uint8, 0), mod=(g["mod_size"], np.int32, 0))
@@ -983,12 +1004,13 @@ class GdbaEngine(_LocalSearchEngine):
     isolated_value canonical order: value index of the variables without neighbours (optimal_cost_value);
                    default: argopt of the own cost with ties broken on the value index
     var_global_id  canonical order: the Philox counter of each variable (default: the canonical index), as MgmEngine
+    var_seed       canonical order: the Philox key of each variable (default: `seed` for every variable), as MgmEngine
     """
     FAMILY = "gdba"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", modifier="A",
                  violation="NZ", increase_mode="E", stop_cycle=0, seed=0, var_rank=None, isolated_value=None,
-                 var_global_id=None):
+                 var_global_id=None, var_seed=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -1000,7 +1022,7 @@ class GdbaEngine(_LocalSearchEngine):
                 raise ValueError(f"invalid {name} {v!r}: expected one of {sorted(ok)}")
         self.modifier, self.violation, self.increase_mode = modifier, violation, increase_mode
         inputs, state, scalars = gdba_plan(L, precision, mode, modifier, violation, increase_mode, stop_cycle, seed,
-                                           var_rank, isolated_value, var_global_id)
+                                           var_rank, isolated_value, var_global_id, var_seed)
         self.nbr_ptr_host = inputs["nbr_ptr"]
         self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
         self.modifier_bytes = scalars["mod_size"] * 4
@@ -1186,7 +1208,7 @@ def mixeddsa_slots(layout: FactorGraphLayout, hard):
 
 
 def mixeddsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", proba_hard=0.7, proba_soft=0.5, variant="B",
-                  stop_cycle=0, seed=0, var_global_id=None):
+                  stop_cycle=0, seed=0, var_global_id=None, var_seed=None):
     """MixedDsaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
     buffer, `slot_edge` the soft-then-hard slot order of mixeddsa_slots, `con_opt` written by fg_mixeddsa_init."""
     L = layout
@@ -1203,7 +1225,7 @@ def mixeddsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", proba_
                   var_ptr=i32(L.var_ptr), slot_edge=slot_edge, soft_end=_per_var(L, soft_end, np.int32),
                   nbr_ptr=i32(nbr_ptr), nbr_idx=i32(nbr_idx), init_value=i32(L.init_value),
                   value=[value0, value0.copy()])
-    _set_global_ids(inputs, L, var_global_id)
+    _set_global_ids(inputs, L, var_global_id, var_seed)
     n = L.n_vars
     state = dict(con_opt=(L.n_factors, dt, 0), cost=(n, dt, 0), has_cost=(n, np.uint8, 0),
                  h_best=(n, np.int32, -1), branch=(n, np.uint8, 0))
@@ -1222,13 +1244,14 @@ class MixedDsaEngine(_LocalSearchEngine):
     variant     A | B | C; C behaves as B (its own branch in the reference is unreachable)
     stop_cycle  0 = run forever; else the run ends after stop_cycle rounds (dsa_gpu's convention, dsa.py:352)
     var_global_id  canonical order: the Philox counter of each variable (default: the canonical index), as MgmEngine
+    var_seed    canonical order: the Philox key of each variable (default: `seed` for every variable), as MgmEngine
     `values()` reports the cost of the last move (inf while a hard constraint stays violated), NaN before the first
     one; `record()` the best H and the branch of the last round.
     """
     FAMILY = "mixeddsa"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", proba_hard=0.7,
-                 proba_soft=0.5, variant="B", stop_cycle=0, seed=0, var_global_id=None):
+                 proba_soft=0.5, variant="B", stop_cycle=0, seed=0, var_global_id=None, var_seed=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -1238,7 +1261,7 @@ class MixedDsaEngine(_LocalSearchEngine):
         if int(stop_cycle or 0) < 0:
             raise ValueError(f"invalid stop_cycle {stop_cycle!r}: must be >= 0")
         inputs, state, scalars = mixeddsa_plan(L, precision, mode, proba_hard, proba_soft, variant, stop_cycle, seed,
-                                               var_global_id)
+                                               var_global_id, var_seed)
         t = self._upload(inputs, state)
         self.__dict__.update(t)
         self._classes = _class_array(L)
@@ -1527,14 +1550,17 @@ class SyncbbEngine(_EngineBase):
 
 
 def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precision="f32", device=None, seed=0,
-                var_rank=None, isolated_value=None, tree=None, var_global_id=None):
+                var_rank=None, isolated_value=None, tree=None, var_global_id=None, var_seed=None):
     """The single-GPU engine of algorithm `kind` (a value of solve.ALGOS) over `layout`.  `params`: its algorithm
     parameters, the missing ones taking solve.DEFAULTS; var_rank / isolated_value / var_global_id in canonical order
     as the engines take them (var_rank None: the canonical index; var_global_id None: the canonical index as every
-    Philox counter, ignored by the families without draws: MaxSum, DPOP, SyncBB); tree: DPOP's pseudo-tree.  MaxSum
-    records no sent flags."""
+    Philox counter, ignored by the families without draws: MaxSum, DPOP, SyncBB); var_seed in canonical order: the
+    Philox key of every variable (None: `seed` for all; DBA, MaxSum, DPOP and SyncBB take none and refuse one);
+    tree: DPOP's pseudo-tree.  MaxSum records no sent flags."""
     from .solve import DEFAULTS
     p = dict(DEFAULTS[kind], **params)
+    if var_seed is not None and kind in ("syncbb", "dba", "dpop", "maxsum"):
+        raise ValueError(f"{kind} takes no per-variable seeds")
     if kind == "syncbb":
         return SyncbbEngine(layout, device=device, precision=precision, mode=mode, var_rank=var_rank)
     if kind == "dba":
@@ -1545,24 +1571,25 @@ def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precisio
     if kind == "mixeddsa":
         return MixedDsaEngine(layout, device=device, precision=precision, mode=mode, proba_hard=p["proba_hard"],
                               proba_soft=p["proba_soft"], variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed,
-                              var_global_id=var_global_id)
+                              var_global_id=var_global_id, var_seed=var_seed)
     if kind == "gdba":
         return GdbaEngine(layout, device=device, precision=precision, mode=mode, modifier=p["modifier"],
                           violation=p["violation"], increase_mode=p["increase_mode"], stop_cycle=p["stop_cycle"],
-                          seed=seed, var_rank=var_rank, isolated_value=isolated_value, var_global_id=var_global_id)
+                          seed=seed, var_rank=var_rank, isolated_value=isolated_value, var_global_id=var_global_id,
+                          var_seed=var_seed)
     if kind == "mgm2":
         return Mgm2Engine(layout, device=device, precision=precision, mode=mode, threshold=p["threshold"],
                           favor=p["favor"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank,
-                          var_global_id=var_global_id)
+                          var_global_id=var_global_id, var_seed=var_seed)
     if kind == "mgm":
         return MgmEngine(layout, device=device, precision=precision, mode=mode, stop_cycle=p["stop_cycle"], seed=seed,
                          break_mode=p["break_mode"], var_rank=var_rank, isolated_value=isolated_value,
-                         var_global_id=var_global_id)
+                         var_global_id=var_global_id, var_seed=var_seed)
     if kind == "maxsum":
         return MaxSumEngine(layout, device=device, precision=precision, mode=mode, damping=p["damping"],
                             damping_nodes=p["damping_nodes"], stability=p["stability"],
                             start_messages=p["start_messages"], record_sent=False)
     return DsaEngine(layout, device=device, precision=precision, mode=mode, probability=p["probability"],
                      p_mode=p.get("p_mode", "fixed"), variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed,
-                     isolated_value=isolated_value, var_global_id=var_global_id,
+                     isolated_value=isolated_value, var_global_id=var_global_id, var_seed=var_seed,
                      var_costs=(kind == "adsa"))   # A-DSA: candidates carry own costs

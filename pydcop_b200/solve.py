@@ -38,7 +38,7 @@ the host logic can be tested without one.
 import json
 import os
 import time
-from typing import Any, Callable, Dict, List, Optional
+from typing import Any, Callable, Dict, List, Optional, Sequence, Union
 
 import numpy as np
 
@@ -358,7 +358,8 @@ NOT_BATCHED = {"dba": "it stops per problem by itself, so each problem would nee
 
 
 def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = None, timeout: Optional[float] = None,
-                precision: str = "f32", device=None, seed: Optional[int] = None, infinity: float = float("inf"),
+                precision: str = "f32", device=None, seed: Union[None, int, Sequence[int]] = None,
+                infinity: float = float("inf"),
                 chunk: int = 50, max_vars: int = batch.MAX_BATCH_VARS,
                 engine_factory: Optional[Callable] = None) -> List[Dict[str, Any]]:
     """Run `algo` on every problem of `problems` and return one result dict per problem, in input order, with
@@ -370,14 +371,18 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
     order so that no engine exceeds `max_vars` variables or an int32 index range; the groups run one after the other.
     Every problem keeps its own Philox counters, name ranks and start values, so `assignment`, `status` and `cycle`
     equal those of solve(problem, algo, algo_params, precision=precision, seed=seed) and `cost` / `violation` equal
-    them up to the order of the device reduction (per problem, fg_solution_cost_segmented).  One `seed` serves every
-    problem (solve()'s default draws with 0).
+    them up to the order of the device reduction (per problem, fg_solution_cost_segmented).
+    seed      None or an int: one seed for every problem (solve()'s default draws with 0); or a sequence of ints, one
+              per problem: problem i's result is then solve(problems[i], ..., seed=seed[i])'s.  With it the same
+              problem can appear many times, once per seed, to compare runs of a stochastic algorithm (pydcop
+              batch's iterations); a DcopArrays entry is not re-parsed.
     `timeout` bounds the whole batch: a problem whose group has not reached stop_cycle when it expires reports
     TIMEOUT at the cycle its group reached (0 for groups that had not started).
     `time` and `ingest_time` are the whole batch's (loading, unions, layouts and engines for ingest_time);
     `h2d_bytes` is the problem's engine's.  `n_gpus` is 1: a batch runs on one device, never under torchrun.
     algo: maxsum | dsa | adsa | mgm | mgm2 | gdba | mixeddsa (the fixed-length families; dba, dpop and syncbb are
-    refused).  engine_factory(kind, layout, inst, params): as in solve(), `inst` with var_rank and var_global_id.
+    refused).  engine_factory(kind, layout, inst, params): as in solve(), `inst` with var_rank, var_global_id and
+    var_seed (None when the group's problems share one seed, params["seed"]).
     """
     kind = ALGOS.get(algo)
     if kind in NOT_BATCHED:
@@ -386,6 +391,7 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
     problems = list(problems)
     if not problems:
         raise ValueError("solve_batch needs at least one problem")
+    seeds = _batch_seeds(seed, len(problems))
     if _under_torchrun():
         raise ValueError("solve_batch runs on one GPU: start it without torchrun")
     t0 = time.perf_counter()
@@ -393,7 +399,7 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
     dcops = []
     for i, p in enumerate(problems):
         try:
-            dcops.append(load(p, seed))
+            dcops.append(load(p, seeds[i]))
         except (ValueError, TypeError) as e:
             raise ValueError(f"problem {i}: {e}") from e
         batch.check_problem(i, dcops[-1])
@@ -407,15 +413,20 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
             var_inputs = lambda d: (name_rank(d), None)  # noqa: E731
         else:
             var_inputs = lambda d: _var_inputs(kind, d, mode)  # noqa: E731
-        u = batch.build_union(dcops, members, var_inputs, noise, seed)
+        u = batch.build_union(dcops, members, var_inputs, noise, [seeds[i] for i in members])
         layout = batch.union_layout(u, dcops)
+        # one seed for the whole group: the scalar key, as solve() runs; else each variable's own (u.var_seed)
+        group_seed = seeds[members[0]] or 0
+        var_seed = None if kind == "maxsum" else u.var_seed   # MaxSum draws nothing on the device: its noise is in u
         if engine_factory is not None:
-            engine = engine_factory(kind, layout, dict(u.inst, var_rank=u.var_rank, var_global_id=u.var_global_id),
-                                    dict(params, mode=mode, seed=seed or 0))
+            engine = engine_factory(kind, layout, dict(u.inst, var_rank=u.var_rank, var_global_id=u.var_global_id,
+                                                       var_seed=var_seed),
+                                    dict(params, mode=mode, seed=group_seed))
         else:
             from .engine import make_engine
-            engine = make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=seed or 0,
-                                 var_rank=u.var_rank, isolated_value=u.isolated_value, var_global_id=u.var_global_id)
+            engine = make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=group_seed,
+                                 var_rank=u.var_rank, isolated_value=u.isolated_value, var_global_id=u.var_global_id,
+                                 var_seed=var_seed)
         ingest_time += time.perf_counter() - t_group
         engine.init()
         cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline)
@@ -437,6 +448,22 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
     for r in results:
         r.update(time=total, ingest_time=ingest_time)
     return results
+
+
+def _batch_seeds(seed, n: int) -> list:
+    """solve_batch's `seed` as one seed per problem: None or an int serves all `n`, a sequence must hold n ints."""
+    if seed is None or isinstance(seed, (int, np.integer)):
+        return [seed] * n
+    try:
+        seeds = list(seed)
+    except TypeError:
+        raise ValueError(f"seed must be an int or a sequence of ints, got {type(seed).__name__}") from None
+    if len(seeds) != n:
+        raise ValueError(f"seed: {len(seeds)} seeds for {n} problems")
+    for i, s in enumerate(seeds):
+        if isinstance(s, bool) or not isinstance(s, (int, np.integer)):
+            raise ValueError(f"seed {i}: expected an int, got {s!r}")
+    return [int(s) for s in seeds]
 
 
 def _finish_syncbb(engine, dcop, deadline, infinity, precision, t0, t_packed):
@@ -497,7 +524,15 @@ def main(argv=None):
     ap.add_argument("--batch", action="store_true",
                     help="every file is one problem, all solved in one engine run per objective (solve_batch); "
                          "prints a JSON list in file order")
+    ap.add_argument("--iterations", type=int, default=None, metavar="N",
+                    help="with --batch: solve every file N times, with seeds --seed + r for r = 0..N-1 (--seed "
+                         "defaults to 0 here), as `pydcop batch` iterations; the list is file-major and every entry "
+                         "carries \"iteration\" and \"seed\"")
     args = ap.parse_args(argv)
+    if args.iterations is not None and not args.batch:
+        ap.error("--iterations needs --batch")
+    if args.iterations is not None and args.iterations < 1:
+        ap.error("--iterations must be >= 1")
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     if args.batch:
@@ -551,10 +586,20 @@ def _algo_params(ap, args):
 
 
 def _main_batch(args, params):
-    res = solve_batch(args.dcop_files, args.algo, params, args.timeout, args.precision, seed=args.seed,
-                      infinity=args.infinity)
-    for path, r in zip(args.dcop_files, res):
-        r["problem"] = path
+    if args.iterations is None:
+        res = solve_batch(args.dcop_files, args.algo, params, args.timeout, args.precision, seed=args.seed,
+                          infinity=args.infinity)
+        for path, r in zip(args.dcop_files, res):
+            r["problem"] = path
+    else:
+        # every file is read once; a YAML file's own noise_level draws are made then, with the first seed
+        base, n = args.seed or 0, args.iterations
+        dcops = [load(path, base) for path in args.dcop_files]
+        res = solve_batch([d for d in dcops for _ in range(n)], args.algo, params, args.timeout, args.precision,
+                          seed=[base + r for _ in dcops for r in range(n)], infinity=args.infinity)
+        for k, r in enumerate(res):
+            r.update(problem=args.dcop_files[k // n], iteration=k % n, seed=base + k % n)
+    for r in res:
         if args.no_assignment:
             r.pop("assignment")
     print(json.dumps(res, indent=2, sort_keys=True, default=str))
