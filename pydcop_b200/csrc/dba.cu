@@ -12,14 +12,6 @@ struct fg_dba : fg_handle_base {
   int eval_dmax = FG_MAX_DOM;          // dba_eval_dmax of the class table: which k_dba_ok instance runs
 };
 
-static inline unsigned dba_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
-static MgmSide dba_side(const fg_dba *h) {
-  const fg_dba_desc_t &d = h->d;
-  return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr};
-}
-
 // stop_cycle as fg_gdba_*: rounds stop once cycle + 1 >= stop_cycle
 static bool dba_finished(const fg_dba *h) {
   return h->ended || (h->d.stop_cycle && h->cycle + 1 >= h->d.stop_cycle);
@@ -83,27 +75,13 @@ extern "C" int fg_dba_destroy(fg_dba_t h) { return fg_close(h); }
 
 extern "C" const char *fg_dba_last_error(fg_dba_t h) { return fg_last_error(h); }
 
-template <typename T>
-static void dba_bits_t(fg_dba *h, cudaStream_t st) {
-  const fg_dba_desc_t &d = h->d;
-  k_dba_bits<T><<<dba_blocks(d.n_words, 256), 256, 0, st>>>(dba_side(h), d.n_edges, (const T *)d.dev_tables,
-                                                            d.dev_bit_off, d.n_words, (T)d.infinity, d.dev_bits);
-}
-
 extern "C" int fg_dba_init(fg_dba_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
   FG_ON_DEVICE(h);
-  const fg_dba_desc_t &d = h->d;
   cudaStream_t st = (cudaStream_t)stream;
-  if (d.n_edges) {
-    if (d.precision == FG_F64) dba_bits_t<double>(h, st);
-    else dba_bits_t<float>(h, st);
-    ++h->launches;
-  }
-  k_dba_init<<<dba_blocks(d.n_vars > 0 ? d.n_vars : 1, 128), 128, 0, st>>>(
-      dba_side(h), d.n_vars, d.seed, d.n_live, d.dev_value[0], d.dev_has_cost, d.dev_counter_own, d.dev_finish_phase,
-      d.dev_weight, d.dev_status, d.dev_unresolved);
-  ++h->launches;
+  fg_launcher launch(h, st);
+  if (h->d.precision == FG_F64) dba_init<double>(h->d, h->dev_classes, launch);
+  else dba_init<float>(h->d, h->dev_classes, launch);
   CUDA_TRY(h, cudaGetLastError());
   h->cycle = 0;
   h->started = true;
@@ -114,25 +92,8 @@ extern "C" int fg_dba_init(fg_dba_t h, void *stream) {
 }
 
 static int dba_round(fg_dba *h, cudaStream_t st) {
-  const fg_dba_desc_t &d = h->d;
-  if (d.n_vars) {
-    const MgmSide g = dba_side(h);
-    const int32_t k = (int32_t)(h->cycle + 1);
-    const int n = d.n_vars;
-    int32_t *vin = d.dev_value[h->cycle & 1], *vout = d.dev_value[(h->cycle + 1) & 1];
-    auto ok = h->eval_dmax <= 32 ? k_dba_ok<32> : k_dba_ok<FG_MAX_DOM>;
-    ok<<<dba_blocks(n, 128), 128, 0, st>>>(g, n, d.dev_bits, d.dev_bit_off, d.dev_weight, vin, d.infinity, d.seed, k,
-                                           d.dev_finish_phase, d.dev_status, d.dev_counter_own, d.dev_eval,
-                                           d.dev_improve, d.dev_counter, d.dev_new_value, d.dev_can_move, d.dev_qlm,
-                                           d.dev_consistent, d.dev_violated, d.dev_cost, d.dev_has_cost,
-                                           d.dev_unresolved);
-    k_dba_improve<<<dba_blocks(n, 256), 256, 0, st>>>(g, n, d.dev_eval, d.dev_improve, d.dev_counter,
-                                                      d.dev_new_value, d.max_distance, k, d.dev_finish_phase,
-                                                      d.dev_status, d.dev_violated, vin, vout, d.dev_counter_own,
-                                                      d.dev_can_move, d.dev_qlm, d.dev_consistent, d.dev_weight,
-                                                      d.dev_cost);
-    h->launches += 2;
-  }
+  fg_launcher launch(h, st);
+  if (h->d.n_vars) dba_cycle(h->d, h->dev_classes, h->eval_dmax, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
   return FG_OK;

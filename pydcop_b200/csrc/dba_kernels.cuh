@@ -274,3 +274,39 @@ k_dba_improve(MgmSide g, int n_vars, const int64_t *__restrict__ eval, const int
     cost[v] = eval[v] - mine;
   }
 }
+
+// ---- launch sequences of fg_dba_init / fg_dba_step, shared with tests/hostshim/dba_host.cpp -----------------------
+// L is a launcher (fg_launcher in handle.cuh, fg_host_launcher on the CPU); `classes` is the class table the kernels
+// read; `eval_dmax` is dba_eval_dmax of the class table.
+
+static inline MgmSide dba_side(const fg_dba_desc_t &d, const fg_class_t *classes) {
+  return MgmSide{classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr};
+}
+
+// the violation bit rows, then the start values and the round state
+template <typename T, class L>
+static void dba_init(const fg_dba_desc_t &d, const fg_class_t *classes, L &launch) {
+  const MgmSide g = dba_side(d, classes);
+  if (d.n_edges)
+    launch(d.n_words, 256, k_dba_bits<T>, g, d.n_edges, (const T *)d.dev_tables, d.dev_bit_off, d.n_words,
+           (T)d.infinity, d.dev_bits);
+  launch(d.n_vars > 0 ? d.n_vars : 1, 128, k_dba_init, g, d.n_vars, d.seed, d.n_live, d.dev_value[0], d.dev_has_cost,
+         d.dev_counter_own, d.dev_finish_phase, d.dev_weight, d.dev_status, d.dev_unresolved);
+}
+
+// round done + 1
+template <class L>
+static void dba_cycle(const fg_dba_desc_t &d, const fg_class_t *classes, int eval_dmax, int64_t done, L &launch) {
+  const MgmSide g = dba_side(d, classes);
+  const int32_t k = (int32_t)(done + 1);
+  const int n = d.n_vars;
+  int32_t *vin = d.dev_value[done & 1], *vout = d.dev_value[(done + 1) & 1];
+  launch(n, 128, eval_dmax <= 32 ? k_dba_ok<32> : k_dba_ok<FG_MAX_DOM>, g, n, d.dev_bits, d.dev_bit_off,
+         d.dev_weight, vin, d.infinity, d.seed, k, d.dev_finish_phase, d.dev_status, d.dev_counter_own, d.dev_eval,
+         d.dev_improve, d.dev_counter, d.dev_new_value, d.dev_can_move, d.dev_qlm, d.dev_consistent, d.dev_violated,
+         d.dev_cost, d.dev_has_cost, d.dev_unresolved);
+  launch(n, 256, k_dba_improve, g, n, d.dev_eval, d.dev_improve, d.dev_counter, d.dev_new_value, d.max_distance, k,
+         d.dev_finish_phase, d.dev_status, d.dev_violated, vin, vout, d.dev_counter_own, d.dev_can_move, d.dev_qlm,
+         d.dev_consistent, d.dev_weight, d.dev_cost);
+}

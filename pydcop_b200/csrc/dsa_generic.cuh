@@ -116,3 +116,35 @@ k_dsa_step_generic(DsaSide g, int n_vars, const T *__restrict__ tables,
   }
   val_next[v] = nv;
 }
+
+// ---- launch sequences of fg_dsa_init / fg_dsa_cycle_compute, shared with tests/hostshim/dsa_generic_host.cpp -------
+// L is a launcher (fg_launcher in handle.cuh, fg_host_launcher on the CPU); `classes` is the class table the kernels
+// read.  engine.cu tries the active-row and oriented-table steps (dsa_cached.cuh, dsa_fast.cuh) before dsa_step.
+
+static inline DsaSide dsa_side(const fg_dsa_desc_t &d, const fg_class_t *classes) {
+  return DsaSide{classes, d.dev_dom_size, d.dev_var_id, d.dev_edge_var, d.dev_edge_class, d.dev_var_ptr,
+                 d.dev_slot_edge, d.dev_has_nbr, d.dev_prob, d.dev_var_seed};
+}
+
+// constraint optima, start values into both buffers, and the active-row array's "no row read yet"
+template <typename T, class L>
+static void dsa_init(const fg_dsa_desc_t &d, const fg_class_t *classes, L &launch) {
+  for (int ci = 0; ci < d.n_classes; ++ci) {
+    const fg_class_t &c = d.classes[ci];
+    if (c.n_factors)
+      launch(c.n_factors, 128, k_dsa_con_opt<T>, c, (const T *)d.dev_tables, (T *)d.dev_con_opt, d.mode_max);
+  }
+  if (d.n_vars) {
+    launch(d.n_vars, 128, k_dsa_init, dsa_side(d, classes), d.n_vars, d.seed, d.dev_value[0]);
+    launch.copy(d.dev_value[1], d.dev_value[0], sizeof(int32_t) * (size_t)d.n_vars);
+  }
+  if (d.dev_slot_last && d.n_edges) launch.fill(d.dev_slot_last, 0xFF, (size_t)d.n_edges);
+}
+
+// evaluate_cycle of round `cycle` from buffer cur into buffer cur ^ 1, on the generic kernel
+template <typename T, class L>
+static void dsa_step(const fg_dsa_desc_t &d, const fg_class_t *classes, int cur, uint32_t cycle, L &launch) {
+  launch(d.n_vars, 128, k_dsa_step_generic<T>, dsa_side(d, classes), d.n_vars, (const T *)d.dev_tables,
+         (const T *)d.dev_con_opt, d.dev_value[cur], d.dev_value[cur ^ 1], (T *)d.dev_value_cost, d.mode_max,
+         d.variant, d.seed, cycle, (const T *)d.dev_var_cost, d.dev_unary_off);
+}

@@ -727,38 +727,17 @@ extern "C" int fg_dsa_destroy(fg_dsa_t h) { return fg_close(h); }
 
 extern "C" const char *fg_dsa_last_error(fg_dsa_t h) { return fg_last_error(h); }
 
-static DsaSide dsa_side(const fg_dsa *h) {
-  const fg_dsa_desc_t &d = h->d;
-  return DsaSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_edge_var, d.dev_edge_class, d.dev_var_ptr,
-                 d.dev_slot_edge, d.dev_has_nbr, d.dev_prob, d.dev_var_seed};
-}
-
-template <typename T>
-static int dsa_init_t(fg_dsa *h, cudaStream_t st) {
-  const fg_dsa_desc_t &d = h->d;
-  for (const fg_class_t &c : h->classes) {
-    if (!c.n_factors) continue;
-    k_dsa_con_opt<T><<<blocks_for(c.n_factors, 128), 128, 0, st>>>(c, (const T *)d.dev_tables, (T *)d.dev_con_opt, d.mode_max);
-    ++h->launches;
-  }
-  if (d.n_vars) {
-    k_dsa_init<<<blocks_for(d.n_vars, 128), 128, 0, st>>>(dsa_side(h), d.n_vars, d.seed, d.dev_value[0]);
-    ++h->launches;
-    CUDA_TRY(h, cudaMemcpyAsync(d.dev_value[1], d.dev_value[0], sizeof(int32_t) * (size_t)d.n_vars, cudaMemcpyDeviceToDevice, st));
-  }
-  if (d.dev_slot_last && d.n_edges)   // active-row array (dsa_cached.cuh): no row has been read yet
-    CUDA_TRY(h, cudaMemsetAsync(d.dev_slot_last, 0xFF, (size_t)d.n_edges, st));
+extern "C" int fg_dsa_init(fg_dsa_t h, void *stream) {
+  if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
+  fg_launcher launch(h, (cudaStream_t)stream);
+  if (h->d.precision == FG_F64) dsa_init<double>(h->d, h->dev_classes, launch);
+  else dsa_init<float>(h->d, h->dev_classes, launch);
+  if (int rc = launch.status()) return rc;
   CUDA_TRY(h, cudaGetLastError());
   h->cur = 0;
   h->cycle = 0;
   return FG_OK;
-}
-
-extern "C" int fg_dsa_init(fg_dsa_t h, void *stream) {
-  if (!h) return FG_ERR_ARG;
-  FG_ON_DEVICE(h);
-  cudaStream_t st = (cudaStream_t)stream;
-  return h->d.precision == FG_F64 ? dsa_init_t<double>(h, st) : dsa_init_t<float>(h, st);
 }
 
 template <typename T>
@@ -769,11 +748,8 @@ static int dsa_compute_t(fg_dsa *h, cudaStream_t st) {
   int32_t *val_next = d.dev_value[h->cur ^ 1];
   if (dsa_cached_step<T>(h->d, val, val_next, (uint32_t)h->cycle, st, h->launches)) {
   } else if (!dsa_fast_step<T>(h->d, h->classes, val, val_next, (uint32_t)h->cycle, st, h->launches)) {
-    k_dsa_step_generic<T><<<blocks_for(d.n_vars, 128), 128, 0, st>>>(
-        dsa_side(h), d.n_vars, (const T *)d.dev_tables, (const T *)d.dev_con_opt, val, val_next,
-        (T *)d.dev_value_cost, d.mode_max, d.variant, d.seed, (uint32_t)h->cycle, (const T *)d.dev_var_cost,
-        d.dev_unary_off);
-    ++h->launches;
+    fg_launcher launch(h, st);
+    dsa_step<T>(d, h->dev_classes, h->cur, (uint32_t)h->cycle, launch);
   }
   CUDA_TRY(h, cudaGetLastError());
   return FG_OK;

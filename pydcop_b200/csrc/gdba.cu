@@ -8,15 +8,6 @@ struct fg_gdba : fg_handle_base {
   fg_gdba_desc_t d;
 };
 
-static inline unsigned gdba_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
-static MgmSide gdba_side(const fg_gdba *h) {
-  const fg_gdba_desc_t &d = h->d;
-  return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr,
-                 d.dev_var_seed};
-}
-
 extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
   int rc = fg_open(desc, out);
   if (rc != FG_OK) return rc;
@@ -79,14 +70,9 @@ extern "C" const char *fg_gdba_last_error(fg_gdba_t h) { return fg_last_error(h)
 extern "C" int fg_gdba_init(fg_gdba_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
   FG_ON_DEVICE(h);
-  const fg_gdba_desc_t &d = h->d;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (d.mod_size > 0) CUDA_TRY(h, cudaMemsetAsync(d.dev_mod, 0, sizeof(int32_t) * (size_t)d.mod_size, st));
-  if (d.n_vars) {
-    k_mgm_init<<<gdba_blocks(d.n_vars, 128), 128, 0, st>>>(gdba_side(h), d.n_vars, d.dev_init_value, d.seed,
-                                                          d.dev_value[0], d.dev_has_cost);
-    ++h->launches;
-  }
+  fg_launcher launch(h, (cudaStream_t)stream);
+  gdba_init(h->d, h->dev_classes, launch);
+  if (int rc = launch.status()) return rc;
   CUDA_TRY(h, cudaGetLastError());
   h->cycle = 0;
   return FG_OK;
@@ -94,23 +80,8 @@ extern "C" int fg_gdba_init(fg_gdba_t h, void *stream) {
 
 template <typename T>
 static int gdba_cycle_t(fg_gdba *h, cudaStream_t st) {
-  const fg_gdba_desc_t &d = h->d;
-  if (d.n_vars) {
-    const MgmSide g = gdba_side(h);
-    const uint32_t cyc = (uint32_t)(h->cycle + 1);
-    const int n = d.n_vars;
-    int32_t *vin = d.dev_value[h->cycle & 1], *vout = d.dev_value[(h->cycle + 1) & 1];
-    const int64_t *mod_off = d.increase_mode == FG_GDBA_INCREASE_T ? nullptr : d.dev_mod_off;
-    k_gdba_eval<T><<<gdba_blocks(n, 128), 128, 0, st>>>(
-        g, n, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_unary_off, (const T *)d.dev_viol_ref,
-        d.dev_mod, mod_off, d.modifier, d.violation, vin, (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_improve,
-        d.dev_new_value, d.dev_violated, d.mode_max, d.seed, cyc);
-    k_gdba_decide<T><<<gdba_blocks(n, 256), 256, 0, st>>>(g, n, (const T *)d.dev_improve, d.dev_new_value,
-                                                          d.dev_violated, d.dev_mod, mod_off, d.increase_mode,
-                                                          d.mode_max, vin, vout, (T *)d.dev_cost,
-                                                          d.dev_breakout);
-    h->launches += 2;
-  }
+  fg_launcher launch(h, st);
+  if (h->d.n_vars) gdba_cycle<T>(h->d, h->dev_classes, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
   return FG_OK;

@@ -192,3 +192,35 @@ k_gdba_decide(MgmSide g, int n_vars, const T *__restrict__ improve, const int32_
   breakout[v] = broke;
   val_out[v] = nv;
 }
+
+// ---- launch sequences of fg_gdba_init / fg_gdba_step, shared with tests/hostshim/gdba_host.cpp -------------------
+// L is a launcher (fg_launcher in handle.cuh, fg_host_launcher on the CPU); `classes` is the class table the kernels
+// read.  fg_gdba_step runs gdba_cycle only when there are variables.
+
+static inline MgmSide gdba_side(const fg_gdba_desc_t &d, const fg_class_t *classes) {
+  return MgmSide{classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr, d.dev_var_seed};
+}
+
+template <class L>
+static void gdba_init(const fg_gdba_desc_t &d, const fg_class_t *classes, L &launch) {
+  if (d.mod_size > 0) launch.fill(d.dev_mod, 0, sizeof(int32_t) * (size_t)d.mod_size);
+  if (d.n_vars)
+    launch(d.n_vars, 128, k_mgm_init, gdba_side(d, classes), d.n_vars, d.dev_init_value, d.seed, d.dev_value[0],
+           d.dev_has_cost);
+}
+
+// round done + 1
+template <typename T, class L>
+static void gdba_cycle(const fg_gdba_desc_t &d, const fg_class_t *classes, int64_t done, L &launch) {
+  const MgmSide g = gdba_side(d, classes);
+  const uint32_t cyc = (uint32_t)(done + 1);
+  const int n = d.n_vars;
+  int32_t *vin = d.dev_value[done & 1], *vout = d.dev_value[(done + 1) & 1];
+  const int64_t *mod_off = d.increase_mode == FG_GDBA_INCREASE_T ? nullptr : d.dev_mod_off;
+  launch(n, 128, k_gdba_eval<T>, g, n, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_unary_off,
+         (const T *)d.dev_viol_ref, d.dev_mod, mod_off, d.modifier, d.violation, vin, (T *)d.dev_cost, d.dev_has_cost,
+         (T *)d.dev_improve, d.dev_new_value, d.dev_violated, d.mode_max, d.seed, cyc);
+  launch(n, 256, k_gdba_decide<T>, g, n, (const T *)d.dev_improve, d.dev_new_value, d.dev_violated, d.dev_mod,
+         mod_off, d.increase_mode, d.mode_max, vin, vout, (T *)d.dev_cost, d.dev_breakout);
+}

@@ -1,6 +1,7 @@
 // Host-side scaffolding shared by the fg_<family>_* handles (engine.cu, mgm.cu, mgm2.cu, gdba.cu, dpop.cu): opening a
 // handle over a copy of its descriptor, the class-table checks and upload, the device a handle belongs to, closing,
-// and the step loop of the families that stop at cycle + 1 >= stop_cycle.  No device code.
+// the step loop of the families that stop at cycle + 1 >= stop_cycle, and the launcher the kernel headers' shared
+// launch sequences run on.  No device code.
 #pragma once
 
 #include <cstdio>
@@ -169,6 +170,37 @@ static inline int fg_close(H *h) {
   delete h;
   return FG_OK;
 }
+
+// The launcher the shared host sequences of the kernel headers run on (mgm_kernels.cuh & co.; tests/hostshim/
+// cuda_host.h is the other one, on the CPU): L(n, block, kernel, args...) launches ceil(n / block) blocks of `block`
+// threads on the stream and counts the launch; fill / copy are cudaMemsetAsync / cudaMemcpyAsync.  After the first
+// failed fill or copy every call does nothing, and status() reports it as CUDA_TRY would.
+struct fg_launcher {
+  fg_handle_base *h;
+  cudaStream_t st;
+  cudaError_t e = cudaSuccess;
+  const char *what = nullptr;
+
+  fg_launcher(fg_handle_base *h, cudaStream_t st) : h(h), st(st) {}
+  template <class... P, class... A>
+  void operator()(int64_t n, int block, void (*kernel)(P...), const A &...args) {
+    if (e != cudaSuccess) return;
+    kernel<<<(unsigned)((n + block - 1) / block), block, 0, st>>>(args...);
+    ++h->launches;
+  }
+  void fill(void *p, int byte, size_t bytes) {
+    if (e == cudaSuccess && (e = cudaMemsetAsync(p, byte, bytes, st)) != cudaSuccess) what = "cudaMemsetAsync";
+  }
+  void copy(void *dst, const void *src, size_t bytes) {
+    if (e == cudaSuccess && (e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+      what = "cudaMemcpyAsync";
+  }
+  int status() const {
+    if (e == cudaSuccess) return FG_OK;
+    snprintf(h->err, sizeof(h->err), "%s: %s", what, cudaGetErrorString(e));
+    return FG_ERR_CUDA;
+  }
+};
 
 static inline const char *fg_last_error(const fg_handle_base *h) { return h ? h->err : "invalid handle"; }
 

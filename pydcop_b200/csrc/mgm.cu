@@ -16,15 +16,6 @@ struct fg_mgm : fg_handle_base {
   fg_mgm_desc_t d;
 };
 
-static inline unsigned mgm_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
-static MgmSide mgm_side(const fg_mgm *h) {
-  const fg_mgm_desc_t &d = h->d;
-  return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off,
-                 d.dev_var_seed};
-}
-
 extern "C" int fg_mgm_create(const fg_mgm_desc_t *desc, fg_mgm_t *out) {
   int rc = fg_open(desc, out);
   if (rc != FG_OK) return rc;
@@ -57,11 +48,8 @@ extern "C" int fg_mgm_init(fg_mgm_t h, void *stream) {
   FG_ON_DEVICE(h);
   const fg_mgm_desc_t &d = h->d;
   cudaStream_t st = (cudaStream_t)stream;
-  if (d.n_vars) {
-    k_mgm_init<<<mgm_blocks(d.n_vars, 128), 128, 0, st>>>(mgm_side(h), d.n_vars, d.dev_init_value, d.seed, d.dev_value,
-                                                          d.dev_has_cost);
-    ++h->launches;
-  }
+  fg_launcher launch(h, st);
+  if (d.n_vars) mgm_init(d, h->dev_classes, launch);
   if (d.dev_slot_last && d.n_edges)   // active-row array: no row has been read yet
     CUDA_TRY(h, cudaMemsetAsync(d.dev_slot_last, 0xFF, (size_t)d.n_edges, st));
   CUDA_TRY(h, cudaGetLastError());
@@ -69,62 +57,39 @@ extern "C" int fg_mgm_init(fg_mgm_t h, void *stream) {
   return FG_OK;
 }
 
-template <typename T, int D, int U>
-static void mgm_gain_fast_launch(fg_mgm *h, cudaStream_t st) {
-  const fg_mgm_desc_t &d = h->d;
-  k_mgm_gain_bin<T, D, U><<<mgm_blocks(d.n_vars, 128), 128, 0, st>>>(
-      mgm_side(h), d.n_vars, d.dev_slot_nbr, d.dev_slot_tab, (const T *)d.dev_tables_or, (const T *)d.dev_unary,
-      d.dev_value, (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_gain, d.dev_new_value, d.mode_max, d.seed,
-      (uint32_t)(h->cycle + 1));
-}
-
 template <typename T, int D>
 static void mgm_gain_cached_launch(fg_mgm *h, cudaStream_t st) {
   const fg_mgm_desc_t &d = h->d;
   using Cfg = MgmCachedCfg<T, D>;
   static_assert(sizeof(T) * Cfg::CH * D + 2 * Cfg::CH + 4 * (Cfg::NV + 1) + 16 <= 48 * 1024, "static shared memory");
-  k_mgm_gain_cached<T, D><<<mgm_blocks(d.n_vars, Cfg::NV), Cfg::THREADS, 0, st>>>(
-      mgm_side(h), d.n_vars, d.dev_slot_nbr, d.dev_slot_tab, (const T *)d.dev_tables_or, (const T *)d.dev_unary, d.dev_value,
-      (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_gain, d.dev_new_value, d.mode_max, d.seed, (uint32_t)(h->cycle + 1),
-      (T *)d.dev_row_cache, d.dev_slot_last);
+  k_mgm_gain_cached<T, D><<<(unsigned)((d.n_vars + Cfg::NV - 1) / Cfg::NV), Cfg::THREADS, 0, st>>>(
+      mgm_side(d, h->dev_classes), d.n_vars, d.dev_slot_nbr, d.dev_slot_tab, (const T *)d.dev_tables_or,
+      (const T *)d.dev_unary, d.dev_value, (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_gain, d.dev_new_value,
+      d.mode_max, d.seed, (uint32_t)(h->cycle + 1), (T *)d.dev_row_cache, d.dev_slot_last);
+  ++h->launches;
 }
 
-// the fast value-phase kernel when the descriptor carries the oriented tables, else false; with the active-row array
-// (dev_row_cache) the streaming variant
+// the active-row value phase (a block per Cfg::NV variables, so not a launch of the shared sequence) when the
+// descriptor carries the active-row arrays over oriented tables, else false
 template <typename T>
-static bool mgm_gain_fast(fg_mgm *h, cudaStream_t st) {
+static bool mgm_gain_cached(fg_mgm *h, cudaStream_t st) {
   const fg_mgm_desc_t &d = h->d;
-  if (!d.dev_tables_or || !d.dev_slot_nbr || !d.dev_slot_tab || (d.fast_chunk != 2 && d.fast_chunk != 4)) return false;
-  if (d.dev_row_cache && d.dev_slot_last) {
-    switch (d.fast_dom) {
-#define FG_MGM_CC(n) case n: mgm_gain_cached_launch<T, n>(h, st); return true;
-      FG_MGM_CC(4) FG_MGM_CC(8) FG_MGM_CC(10) FG_MGM_CC(16) FG_MGM_CC(20)
-#undef FG_MGM_CC
-    }
-  }
-#define FG_MGM_CASE(n)                                                              \
-  case n:                                                                           \
-    if (d.fast_chunk == 2) mgm_gain_fast_launch<T, n, 2>(h, st);                    \
-    else mgm_gain_fast_launch<T, n, 4>(h, st);                                      \
-    return true;
+  if (!d.dev_row_cache || !d.dev_slot_last || !mgm_fast_shape(d)) return false;
   switch (d.fast_dom) {
-    FG_MGM_CASE(4) FG_MGM_CASE(8) FG_MGM_CASE(10) FG_MGM_CASE(16) FG_MGM_CASE(20)
+#define FG_MGM_CC(n) case n: mgm_gain_cached_launch<T, n>(h, st); return true;
+    FG_MGM_CC(4) FG_MGM_CC(8) FG_MGM_CC(10) FG_MGM_CC(16) FG_MGM_CC(20)
+#undef FG_MGM_CC
   }
-#undef FG_MGM_CASE
   return false;
 }
 
 template <typename T>
 static int mgm_cycle_t(fg_mgm *h, cudaStream_t st) {
   const fg_mgm_desc_t &d = h->d;
+  fg_launcher launch(h, st);
   if (d.n_vars) {
-    if (!mgm_gain_fast<T>(h, st))
-      k_mgm_gain<T><<<mgm_blocks(d.n_vars, 128), 128, 0, st>>>(
-          mgm_side(h), d.n_vars, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_value, (T *)d.dev_cost,
-          d.dev_has_cost, (T *)d.dev_gain, d.dev_new_value, d.mode_max, d.seed, (uint32_t)(h->cycle + 1));
-    k_mgm_decide<T><<<mgm_blocks(d.n_vars, 256), 256, 0, st>>>(mgm_side(h), d.n_vars, (const T *)d.dev_gain,
-                                                                d.dev_new_value, d.dev_value, (T *)d.dev_cost);
-    h->launches += 2;
+    if (!mgm_gain_cached<T>(h, st)) mgm_gain<T>(d, h->dev_classes, h->cycle, launch);
+    mgm_decide<T>(d, h->dev_classes, launch);
   }
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;

@@ -27,15 +27,6 @@ struct fg_mgm2 : fg_handle_base {
   ~fg_mgm2();
 };
 
-static inline unsigned mgm2_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
-static MgmSide mgm2_side(const fg_mgm2 *h) {
-  const fg_mgm2_desc_t &d = h->d;
-  return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr,
-                 d.dev_var_seed};
-}
-
 extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
   int rc = fg_open(desc, out);
   if (rc != FG_OK) return rc;
@@ -84,23 +75,13 @@ extern "C" int fg_mgm2_destroy(fg_mgm2_t h) { return fg_close(h); }
 
 extern "C" const char *fg_mgm2_last_error(fg_mgm2_t h) { return fg_last_error(h); }
 
-template <typename T>
-static void mgm2_init_t(fg_mgm2 *h, cudaStream_t st) {
-  const fg_mgm2_desc_t &d = h->d;
-  k_mgm2_init<T><<<mgm2_blocks(d.n_vars, 128), 128, 0, st>>>(mgm2_side(h), d.n_vars, (const T *)d.dev_tables,
-                                                             d.dev_init_value, d.mode_max, d.seed, d.dev_value,
-                                                             (T *)d.dev_cost, d.dev_has_cost);
-}
-
 extern "C" int fg_mgm2_init(fg_mgm2_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
   FG_ON_DEVICE(h);
-  const fg_mgm2_desc_t &d = h->d;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (d.n_vars) {
-    if (d.precision == FG_F64) mgm2_init_t<double>(h, st);
-    else mgm2_init_t<float>(h, st);
-    ++h->launches;
+  fg_launcher launch(h, (cudaStream_t)stream);
+  if (h->d.n_vars) {
+    if (h->d.precision == FG_F64) mgm2_init<double>(h->d, h->dev_classes, launch);
+    else mgm2_init<float>(h->d, h->dev_classes, launch);
   }
   CUDA_TRY(h, cudaGetLastError());
   h->cycle = 0;
@@ -109,29 +90,8 @@ extern "C" int fg_mgm2_init(fg_mgm2_t h, void *stream) {
 
 template <typename T>
 static int mgm2_cycle_t(fg_mgm2 *h, cudaStream_t st) {
-  const fg_mgm2_desc_t &d = h->d;
-  if (d.n_vars) {
-    const MgmSide g = mgm2_side(h);
-    const uint32_t cyc = (uint32_t)(h->cycle + 1);
-    const int n = d.n_vars;
-    T *cost = (T *)d.dev_cost, *local = (T *)d.dev_local_cost, *gain = (T *)d.dev_gain;
-    k_mgm2_value<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
-        g, n, (const T *)d.dev_tables, d.dev_value, cost, d.dev_has_cost, local, gain, d.dev_potential_value,
-        d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_offer_off, (T *)d.dev_offer, d.mode_max,
-        d.threshold, d.seed, cyc);
-    k_mgm2_answer<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
-        g, n, (const T *)d.dev_tables, d.dev_value, local, gain, d.dev_potential_value, d.dev_offerer, d.dev_partner,
-        d.dev_committed, d.dev_answer, d.dev_answer_value, (T *)d.dev_answer_gain, d.dev_offer_off,
-        (const T *)d.dev_offer, d.mode_max, d.favor, d.seed, cyc);
-    k_mgm2_commit<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, d.dev_offerer, d.dev_answer, d.dev_answer_value,
-                                                          (const T *)d.dev_answer_gain, gain, d.dev_potential_value,
-                                                          d.dev_committed);
-    k_mgm2_gain<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(g, n, gain, d.dev_potential_value, d.dev_committed,
-                                                        d.dev_partner, d.dev_go, d.dev_value, cost);
-    k_mgm2_go<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, d.dev_committed, d.dev_partner, d.dev_go, gain,
-                                                      d.dev_potential_value, d.dev_value, cost);
-    h->launches += 5;
-  }
+  fg_launcher launch(h, st);
+  if (h->d.n_vars) mgm2_cycle<T>(h->d, h->dev_classes, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
   return FG_OK;
@@ -158,77 +118,11 @@ struct fg_mgm2_shard {
 
 fg_mgm2::~fg_mgm2() { delete shard; }
 
-template <typename T>
-static Mgm2State<T> mgm2_state(const fg_mgm2 *h) {
-  const fg_mgm2_desc_t &d = h->d;
-  return Mgm2State<T>{d.dev_value, d.dev_offerer, d.dev_partner, d.dev_answer, d.dev_answer_value,
-                      (T *)d.dev_answer_gain, (T *)d.dev_gain, d.dev_go, d.dev_offer_off, (T *)d.dev_offer};
-}
-
-template <typename T>
-static Mgm2List<T> mgm2_list(const fg_mgm2_xfer_t &x, bool send) {
-  return send ? Mgm2List<T>{x.n_send, x.dev_send_var, x.dev_send_off, (T *)x.dev_send_buf}
-              : Mgm2List<T>{x.n_recv, x.dev_recv_var, x.dev_recv_off, (T *)x.dev_recv_buf};
-}
-
-template <typename T>
-static void mgm2_pack_t(fg_mgm2 *h, int x, cudaStream_t st) {
-  const fg_mgm2_shard_plan_t &p = h->shard->plan;
-  const Mgm2List<T> l = mgm2_list<T>(p.x[x], true);
-  if (!l.n) return;
-  k_mgm2x_pack<T><<<mgm2_blocks(l.n, 256), 256, 0, st>>>(x, l, mgm2_state<T>(h),
-                                                         Mgm2Xlat{p.dev_send_peer, p.dev_owner_rank, p.dev_owner_local});
-  ++h->launches;
-}
-
-template <typename T>
-static void mgm2_unpack_t(fg_mgm2 *h, int x, cudaStream_t st) {
-  const Mgm2List<T> l = mgm2_list<T>(h->shard->plan.x[x], false);
-  if (!l.n) return;
-  k_mgm2x_unpack<T><<<mgm2_blocks(l.n, 256), 256, 0, st>>>(x, l, mgm2_state<T>(h));
-  ++h->launches;
-}
-
 // the phase kernel that produces exchange x, on the owned variables, then the pack of x
 template <typename T>
 static int mgm2_phase_t(fg_mgm2 *h, int x, cudaStream_t st) {
-  const fg_mgm2_desc_t &d = h->d;
-  const uint8_t *gh = h->shard->plan.dev_ghost;
-  const int n = d.n_vars;
-  if (n) {
-    const MgmSide g = mgm2_side(h);
-    const uint32_t cyc = (uint32_t)(h->cycle + 1);
-    T *cost = (T *)d.dev_cost, *local = (T *)d.dev_local_cost, *gain = (T *)d.dev_gain;
-    switch (x) {
-      case MGM2X_OFFERS:
-        k_mgm2s_value<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
-            g, n, gh, (const T *)d.dev_tables, d.dev_value, cost, d.dev_has_cost, local, gain, d.dev_potential_value,
-            d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_offer_off, (T *)d.dev_offer, d.mode_max,
-            d.threshold, d.seed, cyc);
-        break;
-      case MGM2X_ANSWERS:
-        k_mgm2s_answer<T><<<mgm2_blocks(n, 128), 128, 0, st>>>(
-            g, n, gh, (const T *)d.dev_tables, d.dev_value, local, gain, d.dev_potential_value, d.dev_offerer,
-            d.dev_partner, d.dev_committed, d.dev_answer, d.dev_answer_value, (T *)d.dev_answer_gain, d.dev_offer_off,
-            (const T *)d.dev_offer, d.mode_max, d.favor, d.seed, cyc);
-        break;
-      case MGM2X_GAINS:
-        k_mgm2s_commit<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, gh, d.dev_offerer, d.dev_answer, d.dev_answer_value,
-                                                               (const T *)d.dev_answer_gain, gain,
-                                                               d.dev_potential_value, d.dev_committed);
-        break;
-      case MGM2X_GO:
-        k_mgm2s_gain<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(g, n, gh, gain, d.dev_potential_value, d.dev_committed,
-                                                             d.dev_partner, d.dev_go, d.dev_value, cost);
-        break;
-      default:
-        k_mgm2s_go<T><<<mgm2_blocks(n, 256), 256, 0, st>>>(n, gh, d.dev_committed, d.dev_partner, d.dev_go, gain,
-                                                           d.dev_potential_value, d.dev_value, cost);
-        break;
-    }
-    ++h->launches;
-  }
-  mgm2_pack_t<T>(h, x, st);
+  fg_launcher launch(h, st);
+  mgm2s_phase<T>(h->d, h->dev_classes, h->shard->plan, x, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   if (x == MGM2X_VALUES) ++h->cycle;
   return FG_OK;
@@ -295,7 +189,8 @@ static int mgm2_shard_cycle_t(fg_mgm2 *h, cudaStream_t st) {
       if (rc != FG_OK) { snprintf(h->err, sizeof(h->err), "peer push / wait launch failed"); return rc; }
       ++s->epoch;
     }
-    mgm2_unpack_t<T>(h, x, st);
+    fg_launcher launch(h, st);
+    mgm2x_unpack<T>(h->d, s->plan, x, launch);
   }
   CUDA_TRY(h, cudaGetLastError());
   return FG_OK;
@@ -374,14 +269,8 @@ extern "C" int fg_mgm2_shard_attach(fg_mgm2_t h, const fg_mgm2_shard_plan_t *pla
 
 template <typename T>
 static int mgm2_shard_init_t(fg_mgm2 *h, cudaStream_t st) {
-  const fg_mgm2_desc_t &d = h->d;
-  if (d.n_vars) {
-    k_mgm2s_init<T><<<mgm2_blocks(d.n_vars, 128), 128, 0, st>>>(mgm2_side(h), d.n_vars, h->shard->plan.dev_ghost,
-                                                                (const T *)d.dev_tables, d.dev_init_value, d.mode_max,
-                                                                d.seed, d.dev_value, (T *)d.dev_cost, d.dev_has_cost);
-    ++h->launches;
-  }
-  mgm2_pack_t<T>(h, MGM2X_VALUES, st);
+  fg_launcher launch(h, st);
+  mgm2s_init<T>(h->d, h->dev_classes, h->shard->plan, launch);
   CUDA_TRY(h, cudaGetLastError());
   h->cycle = 0;
   return FG_OK;
@@ -404,9 +293,9 @@ extern "C" int fg_mgm2_shard_phase(fg_mgm2_t h, int32_t x, void *stream) {
 extern "C" int fg_mgm2_shard_unpack(fg_mgm2_t h, int32_t x, void *stream) {
   if (!h || !h->shard || x < 0 || x >= MGM2X_N) return FG_ERR_ARG;
   FG_ON_DEVICE(h);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (h->d.precision == FG_F64) mgm2_unpack_t<double>(h, x, st);
-  else mgm2_unpack_t<float>(h, x, st);
+  fg_launcher launch(h, (cudaStream_t)stream);
+  if (h->d.precision == FG_F64) mgm2x_unpack<double>(h->d, h->shard->plan, x, launch);
+  else mgm2x_unpack<float>(h->d, h->shard->plan, x, launch);
   CUDA_TRY(h, cudaGetLastError());
   return FG_OK;
 }

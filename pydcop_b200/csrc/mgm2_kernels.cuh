@@ -405,3 +405,39 @@ k_mgm2_go(int n_vars, const uint8_t *__restrict__ committed, const int32_t *__re
   if (v >= n_vars) return;
   mgm2_go_at<T>(v, committed, partner, go, gain, pvalue, val, cost);
 }
+
+// ---- launch sequences of fg_mgm2_init / fg_mgm2_step, shared with tests/hostshim/mgm2_host.cpp -------------------
+// L is a launcher (fg_launcher in handle.cuh, fg_host_launcher on the CPU); `classes` is the class table the kernels
+// read.  The entry points run them only when there are variables.
+
+static inline MgmSide mgm2_side(const fg_mgm2_desc_t &d, const fg_class_t *classes) {
+  return MgmSide{classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, nullptr, d.dev_var_seed};
+}
+
+template <typename T, class L>
+static void mgm2_init(const fg_mgm2_desc_t &d, const fg_class_t *classes, L &launch) {
+  launch(d.n_vars, 128, k_mgm2_init<T>, mgm2_side(d, classes), d.n_vars, (const T *)d.dev_tables, d.dev_init_value,
+         d.mode_max, d.seed, d.dev_value, (T *)d.dev_cost, d.dev_has_cost);
+}
+
+// round done + 1: five kernels, each boundary a synchronisation point of the reference's message exchange
+template <typename T, class L>
+static void mgm2_cycle(const fg_mgm2_desc_t &d, const fg_class_t *classes, int64_t done, L &launch) {
+  const MgmSide g = mgm2_side(d, classes);
+  const uint32_t cyc = (uint32_t)(done + 1);
+  const int n = d.n_vars;
+  T *cost = (T *)d.dev_cost, *local = (T *)d.dev_local_cost, *gain = (T *)d.dev_gain;
+  launch(n, 128, k_mgm2_value<T>, g, n, (const T *)d.dev_tables, d.dev_value, cost, d.dev_has_cost, local, gain,
+         d.dev_potential_value, d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_offer_off,
+         (T *)d.dev_offer, d.mode_max, d.threshold, d.seed, cyc);
+  launch(n, 128, k_mgm2_answer<T>, g, n, (const T *)d.dev_tables, d.dev_value, local, gain, d.dev_potential_value,
+         d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_answer_value, (T *)d.dev_answer_gain,
+         d.dev_offer_off, (const T *)d.dev_offer, d.mode_max, d.favor, d.seed, cyc);
+  launch(n, 256, k_mgm2_commit<T>, n, d.dev_offerer, d.dev_answer, d.dev_answer_value, (const T *)d.dev_answer_gain,
+         gain, d.dev_potential_value, d.dev_committed);
+  launch(n, 256, k_mgm2_gain<T>, g, n, gain, d.dev_potential_value, d.dev_committed, d.dev_partner, d.dev_go,
+         d.dev_value, cost);
+  launch(n, 256, k_mgm2_go<T>, n, d.dev_committed, d.dev_partner, d.dev_go, gain, d.dev_potential_value, d.dev_value,
+         cost);
+}

@@ -218,3 +218,74 @@ k_mgm2s_go(int n_vars, const uint8_t *__restrict__ ghost, const uint8_t *__restr
   if (v >= n_vars || ghost[v]) return;
   mgm2_go_at<T>(v, committed, partner, go, gain, pvalue, val, cost);
 }
+
+// ---- launch sequences of fg_mgm2_shard_init / _phase / _unpack, shared with tests/hostshim/mgm2_shard_host.cpp ----
+// The NVLink push, the epochs and the cycle count stay in mgm2.cu.
+
+template <typename T>
+static Mgm2State<T> mgm2_state(const fg_mgm2_desc_t &d) {
+  return Mgm2State<T>{d.dev_value, d.dev_offerer, d.dev_partner, d.dev_answer, d.dev_answer_value,
+                      (T *)d.dev_answer_gain, (T *)d.dev_gain, d.dev_go, d.dev_offer_off, (T *)d.dev_offer};
+}
+
+template <typename T, class L>
+static void mgm2x_pack(const fg_mgm2_desc_t &d, const fg_mgm2_shard_plan_t &p, int x, L &launch) {
+  const fg_mgm2_xfer_t &q = p.x[x];
+  if (!q.n_send) return;
+  launch(q.n_send, 256, k_mgm2x_pack<T>, x, Mgm2List<T>{q.n_send, q.dev_send_var, q.dev_send_off, (T *)q.dev_send_buf},
+         mgm2_state<T>(d), Mgm2Xlat{p.dev_send_peer, p.dev_owner_rank, p.dev_owner_local});
+}
+
+template <typename T, class L>
+static void mgm2x_unpack(const fg_mgm2_desc_t &d, const fg_mgm2_shard_plan_t &p, int x, L &launch) {
+  const fg_mgm2_xfer_t &q = p.x[x];
+  if (!q.n_recv) return;
+  launch(q.n_recv, 256, k_mgm2x_unpack<T>, x, Mgm2List<T>{q.n_recv, q.dev_recv_var, q.dev_recv_off, (T *)q.dev_recv_buf},
+         mgm2_state<T>(d));
+}
+
+template <typename T, class L>
+static void mgm2s_init(const fg_mgm2_desc_t &d, const fg_class_t *classes, const fg_mgm2_shard_plan_t &p, L &launch) {
+  if (d.n_vars)
+    launch(d.n_vars, 128, k_mgm2s_init<T>, mgm2_side(d, classes), d.n_vars, p.dev_ghost, (const T *)d.dev_tables,
+           d.dev_init_value, d.mode_max, d.seed, d.dev_value, (T *)d.dev_cost, d.dev_has_cost);
+  mgm2x_pack<T>(d, p, MGM2X_VALUES, launch);
+}
+
+// the phase kernel of round done + 1 that produces exchange x, on the owned variables, then the pack of x
+template <typename T, class L>
+static void mgm2s_phase(const fg_mgm2_desc_t &d, const fg_class_t *classes, const fg_mgm2_shard_plan_t &p, int x,
+                        int64_t done, L &launch) {
+  const uint8_t *gh = p.dev_ghost;
+  const int n = d.n_vars;
+  if (n) {
+    const MgmSide g = mgm2_side(d, classes);
+    const uint32_t cyc = (uint32_t)(done + 1);
+    T *cost = (T *)d.dev_cost, *local = (T *)d.dev_local_cost, *gain = (T *)d.dev_gain;
+    switch (x) {
+      case MGM2X_OFFERS:
+        launch(n, 128, k_mgm2s_value<T>, g, n, gh, (const T *)d.dev_tables, d.dev_value, cost, d.dev_has_cost, local,
+               gain, d.dev_potential_value, d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer,
+               d.dev_offer_off, (T *)d.dev_offer, d.mode_max, d.threshold, d.seed, cyc);
+        break;
+      case MGM2X_ANSWERS:
+        launch(n, 128, k_mgm2s_answer<T>, g, n, gh, (const T *)d.dev_tables, d.dev_value, local, gain,
+               d.dev_potential_value, d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_answer_value,
+               (T *)d.dev_answer_gain, d.dev_offer_off, (const T *)d.dev_offer, d.mode_max, d.favor, d.seed, cyc);
+        break;
+      case MGM2X_GAINS:
+        launch(n, 256, k_mgm2s_commit<T>, n, gh, d.dev_offerer, d.dev_answer, d.dev_answer_value,
+               (const T *)d.dev_answer_gain, gain, d.dev_potential_value, d.dev_committed);
+        break;
+      case MGM2X_GO:
+        launch(n, 256, k_mgm2s_gain<T>, g, n, gh, gain, d.dev_potential_value, d.dev_committed, d.dev_partner,
+               d.dev_go, d.dev_value, cost);
+        break;
+      default:
+        launch(n, 256, k_mgm2s_go<T>, n, gh, d.dev_committed, d.dev_partner, d.dev_go, gain, d.dev_potential_value,
+               d.dev_value, cost);
+        break;
+    }
+  }
+  mgm2x_pack<T>(d, p, x, launch);
+}

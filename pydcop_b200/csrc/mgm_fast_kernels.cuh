@@ -100,3 +100,58 @@ k_mgm_gain_bin(MgmSide g, int n_vars, const int32_t *__restrict__ slot_nbr, cons
   }
   new_val[v] = nv;
 }
+
+// ---- launch sequences of fg_mgm_init / fg_mgm_step, shared with tests/hostshim/mgm_host.cpp ----------------------
+// Here rather than in mgm_kernels.cuh because the value phase picks between both headers' kernels.  L is a launcher
+// (fg_launcher in handle.cuh, fg_host_launcher on the CPU); `classes` is the class table the kernels read.  The entry
+// points run them only when there are variables.  mgm.cu tries the active-row value phase (mgm_cached_kernels.cuh)
+// before mgm_gain.
+
+static inline MgmSide mgm_side(const fg_mgm_desc_t &d, const fg_class_t *classes) {
+  return MgmSide{classes, d.dev_dom_size, d.dev_var_id, d.dev_var_rank, d.dev_edge_var, d.dev_edge_class,
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off, d.dev_var_seed};
+}
+
+// the descriptor carries the oriented tables in a shape k_mgm_gain_bin is compiled for
+static inline bool mgm_fast_shape(const fg_mgm_desc_t &d) {
+  if (!d.dev_tables_or || !d.dev_slot_nbr || !d.dev_slot_tab || (d.fast_chunk != 2 && d.fast_chunk != 4)) return false;
+  return d.fast_dom == 4 || d.fast_dom == 8 || d.fast_dom == 10 || d.fast_dom == 16 || d.fast_dom == 20;
+}
+
+template <class L>
+static void mgm_init(const fg_mgm_desc_t &d, const fg_class_t *classes, L &launch) {
+  launch(d.n_vars, 128, k_mgm_init, mgm_side(d, classes), d.n_vars, d.dev_init_value, d.seed, d.dev_value,
+         d.dev_has_cost);
+}
+
+template <typename T, int D, class L>
+static void mgm_gain_bin(const fg_mgm_desc_t &d, const MgmSide &g, uint32_t cyc, L &launch) {
+  launch(d.n_vars, 128, d.fast_chunk == 2 ? k_mgm_gain_bin<T, D, 2> : k_mgm_gain_bin<T, D, 4>, g, d.n_vars,
+         d.dev_slot_nbr, d.dev_slot_tab, (const T *)d.dev_tables_or, (const T *)d.dev_unary, d.dev_value,
+         (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_gain, d.dev_new_value, d.mode_max, d.seed, cyc);
+}
+
+// value phase of round done + 1: the oriented tables when mgm_fast_shape, else the generic kernel
+template <typename T, class L>
+static void mgm_gain(const fg_mgm_desc_t &d, const fg_class_t *classes, int64_t done, L &launch) {
+  const MgmSide g = mgm_side(d, classes);
+  const uint32_t cyc = (uint32_t)(done + 1);
+  if (mgm_fast_shape(d)) {
+    switch (d.fast_dom) {
+      case 4: mgm_gain_bin<T, 4>(d, g, cyc, launch); return;
+      case 8: mgm_gain_bin<T, 8>(d, g, cyc, launch); return;
+      case 10: mgm_gain_bin<T, 10>(d, g, cyc, launch); return;
+      case 16: mgm_gain_bin<T, 16>(d, g, cyc, launch); return;
+      default: mgm_gain_bin<T, 20>(d, g, cyc, launch); return;
+    }
+  }
+  launch(d.n_vars, 128, k_mgm_gain<T>, g, d.n_vars, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_value,
+         (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_gain, d.dev_new_value, d.mode_max, d.seed, cyc);
+}
+
+// gain phase
+template <typename T, class L>
+static void mgm_decide(const fg_mgm_desc_t &d, const fg_class_t *classes, L &launch) {
+  launch(d.n_vars, 256, k_mgm_decide<T>, mgm_side(d, classes), d.n_vars, (const T *)d.dev_gain, d.dev_new_value,
+         d.dev_value, (T *)d.dev_cost);
+}

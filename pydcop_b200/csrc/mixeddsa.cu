@@ -1,8 +1,6 @@
 // MixedDSA for all variables at once: C-ABI entry points fg_mixeddsa_* and their kernels (csrc/mixeddsa_kernels.cuh,
 // which states the floating-point operand order).  Its own translation unit, so the other families' code is compiled
 // exactly as before.
-#include <limits>
-
 #include "handle.cuh"
 #include "philox.cuh"
 
@@ -17,15 +15,6 @@ struct fg_mixeddsa : fg_handle_base {
   fg_mixeddsa_desc_t d;
   int dmax = FG_MAX_DOM;  // mixeddsa_dmax of the class table: which k_mixeddsa_step instance runs
 };
-
-static inline unsigned mixeddsa_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
-static MgmSide mixeddsa_side(const fg_mixeddsa *h) {
-  const fg_mixeddsa_desc_t &d = h->d;
-  return MgmSide{h->dev_classes, d.dev_dom_size, d.dev_var_id, nullptr, d.dev_edge_var, d.dev_edge_class,
-                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off,
-                 d.dev_var_seed};
-}
 
 // stop_cycle as fg_dsa_*: a run ends after stop_cycle rounds (dsa.py:352)
 static bool mixeddsa_finished(const fg_mixeddsa *h) { return h->d.stop_cycle && h->cycle >= h->d.stop_cycle; }
@@ -80,28 +69,12 @@ extern "C" int fg_mixeddsa_destroy(fg_mixeddsa_t h) { return fg_close(h); }
 
 extern "C" const char *fg_mixeddsa_last_error(fg_mixeddsa_t h) { return fg_last_error(h); }
 
-template <typename T>
-static void mixeddsa_con_opt_t(fg_mixeddsa *h, cudaStream_t st) {
-  for (const fg_class_t &c : h->classes) {
-    if (!c.n_factors) continue;
-    k_dsa_con_opt<T><<<mixeddsa_blocks(c.n_factors, 128), 128, 0, st>>>(c, (const T *)h->d.dev_tables,
-                                                                         (T *)h->d.dev_con_opt, h->d.mode_max);
-    ++h->launches;
-  }
-}
-
 extern "C" int fg_mixeddsa_init(fg_mixeddsa_t h, void *stream) {
   if (!h) return FG_ERR_ARG;
   FG_ON_DEVICE(h);
-  const fg_mixeddsa_desc_t &d = h->d;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (d.precision == FG_F64) mixeddsa_con_opt_t<double>(h, st);
-  else mixeddsa_con_opt_t<float>(h, st);
-  if (d.n_vars) {
-    k_mixeddsa_init<<<mixeddsa_blocks(d.n_vars, 128), 128, 0, st>>>(mixeddsa_side(h), d.n_vars, d.dev_init_value,
-                                                                    d.seed, d.dev_value[0], d.dev_has_cost);
-    ++h->launches;
-  }
+  fg_launcher launch(h, (cudaStream_t)stream);
+  if (h->d.precision == FG_F64) mixeddsa_init<double>(h->d, h->dev_classes, launch);
+  else mixeddsa_init<float>(h->d, h->dev_classes, launch);
   CUDA_TRY(h, cudaGetLastError());
   h->cycle = 0;
   return FG_OK;
@@ -109,17 +82,8 @@ extern "C" int fg_mixeddsa_init(fg_mixeddsa_t h, void *stream) {
 
 template <typename T>
 static int mixeddsa_round_t(fg_mixeddsa *h, cudaStream_t st) {
-  const fg_mixeddsa_desc_t &d = h->d;
-  if (d.n_vars) {
-    const int n = d.n_vars;
-    int32_t *vin = d.dev_value[h->cycle & 1], *vout = d.dev_value[(h->cycle + 1) & 1];
-    auto step = h->dmax <= 32 ? k_mixeddsa_step<T, 32> : k_mixeddsa_step<T, FG_MAX_DOM>;
-    step<<<mixeddsa_blocks(n, 128), 128, 0, st>>>(
-        mixeddsa_side(h), n, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_soft_end,
-        (const T *)d.dev_con_opt, vin, vout, (T *)d.dev_cost, d.dev_has_cost, d.dev_h_best, d.dev_branch, d.mode_max,
-        d.variant, d.proba_hard, d.proba_soft, std::numeric_limits<T>::infinity(), d.seed, (uint32_t)(h->cycle + 1));
-    ++h->launches;
-  }
+  fg_launcher launch(h, st);
+  if (h->d.n_vars) mixeddsa_cycle<T>(h->d, h->dev_classes, h->dmax, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
   return FG_OK;

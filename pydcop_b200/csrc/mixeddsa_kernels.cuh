@@ -15,6 +15,8 @@
 #pragma once
 #include <stdint.h>
 
+#include <limits>
+
 #include "../../include/pydcop_b200.h"
 #include "philox.cuh"
 
@@ -187,4 +189,36 @@ k_mixeddsa_step(MgmSide g, int n_vars, const T *__restrict__ tables, const T *__
   }
   h_best[v] = hb;
   branch[v] = (uint8_t)(br | moved);
+}
+
+// ---- launch sequences of fg_mixeddsa_init / fg_mixeddsa_step, shared with tests/hostshim/mixeddsa_host.cpp --------
+// L is a launcher (fg_launcher in handle.cuh, fg_host_launcher on the CPU); `classes` is the class table the kernels
+// read; `dmax` is mixeddsa_dmax of the class table.  k_dsa_con_opt comes from dsa_generic.cuh, which the includer
+// includes first.
+
+static inline MgmSide mixeddsa_side(const fg_mixeddsa_desc_t &d, const fg_class_t *classes) {
+  return MgmSide{classes, d.dev_dom_size, d.dev_var_id, nullptr, d.dev_edge_var, d.dev_edge_class,
+                 d.dev_var_ptr, d.dev_slot_edge, d.dev_nbr_ptr, d.dev_nbr_idx, d.dev_unary_off, d.dev_var_seed};
+}
+
+template <typename T, class L>
+static void mixeddsa_init(const fg_mixeddsa_desc_t &d, const fg_class_t *classes, L &launch) {
+  for (int ci = 0; ci < d.n_classes; ++ci) {
+    const fg_class_t &c = d.classes[ci];
+    if (c.n_factors)
+      launch(c.n_factors, 128, k_dsa_con_opt<T>, c, (const T *)d.dev_tables, (T *)d.dev_con_opt, d.mode_max);
+  }
+  if (d.n_vars)
+    launch(d.n_vars, 128, k_mixeddsa_init, mixeddsa_side(d, classes), d.n_vars, d.dev_init_value, d.seed,
+           d.dev_value[0], d.dev_has_cost);
+}
+
+// round done + 1
+template <typename T, class L>
+static void mixeddsa_cycle(const fg_mixeddsa_desc_t &d, const fg_class_t *classes, int dmax, int64_t done, L &launch) {
+  int32_t *vin = d.dev_value[done & 1], *vout = d.dev_value[(done + 1) & 1];
+  launch(d.n_vars, 128, dmax <= 32 ? k_mixeddsa_step<T, 32> : k_mixeddsa_step<T, FG_MAX_DOM>,
+         mixeddsa_side(d, classes), d.n_vars, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_soft_end,
+         (const T *)d.dev_con_opt, vin, vout, (T *)d.dev_cost, d.dev_has_cost, d.dev_h_best, d.dev_branch, d.mode_max,
+         d.variant, d.proba_hard, d.proba_soft, std::numeric_limits<T>::infinity(), d.seed, (uint32_t)(done + 1));
 }

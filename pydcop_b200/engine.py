@@ -458,6 +458,55 @@ def dsa_fast_arrays(layout: FactorGraphLayout, tables: torch.Tensor, mode="min")
             opt[torch.from_numpy(f).to(dev)].contiguous(), D)
 
 
+def dsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", probability=0.7, p_mode="fixed", variant="B",
+             stop_cycle=0, seed=0, isolated_value=None, var_global_id=None, frozen=None, var_costs=False,
+             var_seed=None):
+    """DsaEngine's host-array plan for the generic kernels (inputs, state, scalar descriptor fields), as mgm_plan;
+    `value` is the double buffer, its second half uploaded as zeros.  The oriented-table and active-row arrays are
+    DsaEngine's own.  frozen (canonical order): ghost variables of a shard, has_nbr = 2 (never written by the local
+    kernels); var_costs: A-DSA's var_cost / unary_off."""
+    L = layout
+    dt = PRECISIONS[precision][2]
+    if variant not in _cabi.DSA_VARIANTS:
+        raise ValueError(f"invalid variant {variant!r}")
+    if p_mode not in ("fixed", "arity"):
+        raise ValueError(f"invalid p_mode {p_mode!r}")
+    arity = np.array([c.arity for c in L.classes], dtype=np.int64)
+    n_count = np.zeros(L.n_vars, dtype=np.int64)
+    if L.n_edges:
+        np.add.at(n_count, L.slot_var, arity[L.edge_class[L.slot_edge]] - 1)
+    has_nbr = (n_count > 0).astype(np.uint8)
+    if frozen is not None:   # 2 = ghost of another rank's variable: never written by the local kernels
+        has_nbr[np.asarray(frozen, dtype=bool)[L.var_order]] = 2
+    if p_mode == "arity":  # dsa.py:257-260: 1 / n_count * 1.2
+        with np.errstate(divide="ignore"):
+            prob = np.where(n_count > 0, 1.0 / np.maximum(n_count, 1) * 1.2, 0.0)
+    else:
+        prob = np.full(L.n_vars, float(probability))
+    # isolated variables (dsa.py:278-289): argopt of (own cost, value), tuple order
+    if isolated_value is not None:   # given in canonical order
+        isolated_value = np.asarray(isolated_value, dtype=np.int32)[L.var_order]
+    else:
+        isolated_value = np.zeros(L.n_vars, dtype=np.int32)
+        for v in np.nonzero(n_count == 0)[0]:  # (frozen ghosts are filled by the exchange)
+            c = L.unary[L.unary_off[v]:L.unary_off[v] + L.dom_size[v]]
+            if mode == "min":
+                isolated_value[v] = int(np.argmin(c))
+            else:
+                isolated_value[v] = int(len(c) - 1 - np.argmax(c[::-1]))
+    i32 = lambda a: np.ascontiguousarray(a, np.int32)  # noqa: E731
+    inputs = dict(tables=np.ascontiguousarray(L.tables, dt), dom_size=i32(L.dom_size), var_id=i32(L.var_order),
+                  edge_var=i32(L.edge_var), edge_class=i32(L.edge_class), var_ptr=i32(L.var_ptr),
+                  slot_edge=i32(L.slot_edge), has_nbr=has_nbr, prob=np.ascontiguousarray(prob, np.float64),
+                  value=[_per_var(L, isolated_value, np.int32), np.zeros(max(L.n_vars, 1), np.int32)],
+                  var_cost=np.ascontiguousarray(L.unary, dt) if var_costs else None,
+                  unary_off=np.ascontiguousarray(L.unary_off, np.int64) if var_costs else None)
+    _set_global_ids(inputs, L, var_global_id, var_seed)
+    state = dict(con_opt=(L.n_factors, dt, 0), value_cost=(L.n_vars, dt, 0))
+    return inputs, state, dict(mode_max=int(mode == "max"), variant=_cabi.DSA_VARIANTS[variant],
+                               stop_cycle=int(stop_cycle), seed=_seed(seed))
+
+
 class DsaEngine(_CycleEngine):
     """All-variables-at-once DSA-A/B/C (pydcop/algorithms/dsa.py:130-135 parameters)."""
     FAMILY = "dsa"
@@ -474,54 +523,14 @@ class DsaEngine(_CycleEngine):
         seeds of their own (pydcop_b200.batch); default: `seed` for every variable."""
         L = layout
         tdt = self._open(layout, device, precision)
-        if variant not in _cabi.DSA_VARIANTS:
-            raise ValueError(f"invalid variant {variant!r}")
-        if p_mode not in ("fixed", "arity"):
-            raise ValueError(f"invalid p_mode {p_mode!r}")
-        arity = np.array([c.arity for c in L.classes], dtype=np.int64)
-        n_count = np.zeros(L.n_vars, dtype=np.int64)
-        if L.n_edges:
-            np.add.at(n_count, L.slot_var, arity[L.edge_class[L.slot_edge]] - 1)
-        has_nbr = (n_count > 0).astype(np.uint8)
-        if frozen is not None:   # 2 = ghost of another rank's variable: never written by the local kernels
-            has_nbr[np.asarray(frozen, dtype=bool)[L.var_order]] = 2
-        var_id = (L.var_order if var_global_id is None
-                  else np.asarray(var_global_id, dtype=np.int32)[L.var_order])
-        if p_mode == "arity":  # dsa.py:257-260: 1 / n_count * 1.2
-            with np.errstate(divide="ignore"):
-                prob = np.where(n_count > 0, 1.0 / np.maximum(n_count, 1) * 1.2, 0.0)
-        else:
-            prob = np.full(L.n_vars, float(probability))
-        # isolated variables (dsa.py:278-289): argopt of (own cost, value), tuple order
-        if isolated_value is not None:   # given in canonical order
-            isolated_value = np.asarray(isolated_value, dtype=np.int32)[L.var_order]
-        else:
-            isolated_value = np.zeros(L.n_vars, dtype=np.int32)
-            for v in np.nonzero(n_count == 0)[0]:  # (frozen ghosts are filled by the exchange)
-                c = L.unary[L.unary_off[v]:L.unary_off[v] + L.dom_size[v]]
-                if mode == "min":
-                    isolated_value[v] = int(np.argmin(c))
-                else:
-                    isolated_value[v] = int(len(c) - 1 - np.argmax(c[::-1]))
-        self.has_nbr_host, self.n_count = has_nbr, n_count
-        with torch.cuda.device(self.device):
-            self.tables = self._dev(L.tables, tdt)
-            self.dom_size = self._dev(L.dom_size, torch.int32)
-            self.var_id = self._dev(var_id, torch.int32)
-            self.edge_var = self._dev(L.edge_var, torch.int32)
-            self.edge_class = self._dev(L.edge_class, torch.int32)
-            self.var_ptr = self._dev(L.var_ptr, torch.int32)
-            self.slot_edge = self._dev(L.slot_edge, torch.int32)
-            self.has_nbr = self._dev(has_nbr, torch.uint8)
-            self.prob = self._dev(prob, torch.float64)
-            z = lambda n, dt: torch.zeros(max(int(n), 1), dtype=dt, device=self.device)  # noqa
-            self.con_opt = z(L.n_factors, tdt)
-            self.value = [self._dev(isolated_value, torch.int32) if L.n_vars else z(1, torch.int32),
-                          z(L.n_vars, torch.int32)]
-            self.value_cost = z(L.n_vars, tdt)
-            self.var_cost = self._dev(L.unary, tdt) if var_costs else None
-            self.unary_off = self._dev(L.unary_off, torch.int64) if var_costs else None
-            self.var_seed = None if var_seed is None else self._dev(_var_seeds(L, var_seed), torch.uint64)
+        inputs, state, scalars = dsa_plan(L, precision, mode, probability, p_mode, variant, stop_cycle, seed,
+                                          isolated_value, var_global_id, frozen, var_costs, var_seed)
+        self.has_nbr_host = inputs["has_nbr"]
+        value0, _ = inputs.pop("value")
+        t = self._upload(inputs, state)
+        with torch.cuda.device(self.device):   # the second buffer starts as zeros on the device, nothing to copy
+            t["value"] = [self._dev(value0, torch.int32), torch.zeros(len(value0), dtype=torch.int32, device=self.device)]
+        self.__dict__.update(t)
         # fast path: every constraint binary over ONE domain size -> oriented tables, one contiguous
         # row per incidence (transposed copy for scope position 0)
         self.tables_or = self.slot_nbr = self.slot_tab = self.slot_opt = None
@@ -535,14 +544,10 @@ class DsaEngine(_CycleEngine):
                 self.row_cache = torch.zeros(max(L.n_edges * fast_dom, 4), dtype=tdt, device=self.device)
                 self.slot_last = torch.full((max(L.n_edges, 1),), 255, dtype=torch.uint8, device=self.device)
         self._classes = _class_array(L)
-        d = fill_header(FgDsaDesc(), precision, L, self._classes)
-        fill_desc(d, {k: getattr(self, k) for k in (
-            "tables", "dom_size", "var_id", "edge_var", "edge_class", "var_ptr", "slot_edge", "has_nbr", "prob",
-            "con_opt", "value", "value_cost", "tables_or", "slot_nbr", "slot_tab", "slot_opt", "var_cost", "unary_off",
-            "row_cache", "slot_last", "var_seed")})
+        d = fill_desc(fill_header(FgDsaDesc(), precision, L, self._classes), t, scalars)
+        fill_desc(d, {k: getattr(self, k) for k in ("tables_or", "slot_nbr", "slot_tab", "slot_opt", "row_cache",
+                                                    "slot_last")})
         d.fast_dom = fast_dom
-        d.mode_max, d.variant = int(mode == "max"), _cabi.DSA_VARIANTS[variant]
-        d.stop_cycle, d.seed = int(stop_cycle), int(seed) & (2 ** 64 - 1)
         self._create(d)
 
     def _assignment(self):

@@ -2,18 +2,8 @@
 // the UTIL launches of the schedule in order, each segment's nodes bottom-up with dpop_util_entry on every
 // UTIL entry, then the VALUE paths top-down with dpop_value_node, so its logic can be compared with the
 // oracle and the reference's messages without a GPU.  Nothing in the product links or calls this.
-//   g++ -O1 -std=c++17 -ffp-contract=off -shared -fPIC -o dpop_host.so dpop_host.cpp
 // The descriptor is the C-ABI's fg_dpop_desc_t with HOST pointers.
-#include <stdint.h>
-#include <string.h>
-
-#define __global__
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
-
+#include "cuda_host.h"
 #include "../../pydcop_b200/csrc/dpop_kernels.cuh"
 
 static DpopNodes nodes(const fg_dpop_desc_t *d) {

@@ -1,71 +1,24 @@
-// TEST INFRASTRUCTURE: runs the generic DSA CUDA kernel SOURCE (pydcop_b200/csrc/dsa_generic.cuh,
-// unmodified) on the CPU in the launch order of dsa_init_t / dsa_compute_t in engine.cu.  Nothing in
-// the product links or calls this.
-#include <math.h>
-#include <stdint.h>
-#include <string.h>
-
-struct Dim3 { unsigned x, y, z; };
-static thread_local Dim3 blockIdx, blockDim, threadIdx;
-#define __launch_bounds__(...)
-static inline float __int_as_float(unsigned x) { float f; memcpy(&f, &x, 4); return f; }
-static inline double __longlong_as_double(unsigned long long x) { double f; memcpy(&f, &x, 8); return f; }
-
+// TEST INFRASTRUCTURE: runs fg_dsa_init / fg_dsa_cycle_compute's generic launch sequence
+// (pydcop_b200/csrc/dsa_generic.cuh) on the CPU.  The descriptor is the C-ABI's fg_dsa_desc_t with HOST pointers.
+// Nothing in the product links or calls this.
+#include "cuda_host.h"
 #include "../../pydcop_b200/csrc/dsa_generic.cuh"
 
-template <typename F>
-static void launch(int64_t n, F body) {
-  blockDim = Dim3{128, 1, 1};
-  for (int64_t b = 0; b < (n + 127) / 128; ++b)
-    for (unsigned t = 0; t < 128; ++t) {
-      blockIdx = Dim3{(unsigned)b, 0, 0};
-      threadIdx = Dim3{t, 0, 0};
-      body();
-    }
-}
-
 extern "C" {
-struct dsa_host {
-  const fg_class_t *classes;
-  int32_t n_classes, n_vars, precision, mode_max, variant;
-  const void *tables;
-  const int32_t *dom_size, *var_id, *edge_var, *edge_class, *var_ptr, *slot_edge;
-  const uint8_t *has_nbr;
-  const double *prob;
-  void *con_opt;
-  int32_t *value[2];
-  void *value_cost;
-  uint64_t seed;
-  const void *var_cost;        // A-DSA: the variables' own costs (NULL: DSA)
-  const int64_t *unary_off;
-};
+int64_t dsa_host_init(const fg_dsa_desc_t *d) {
+  fg_host_launcher launch;
+  if (d->precision == FG_F64) dsa_init<double>(*d, d->classes, launch);
+  else dsa_init<float>(*d, d->classes, launch);
+  return launch.launches;
 }
 
-static DsaSide side(const dsa_host *h) {
-  return DsaSide{h->classes, h->dom_size, h->var_id, h->edge_var, h->edge_class, h->var_ptr, h->slot_edge, h->has_nbr, h->prob};
-}
-
-template <typename T>
-static void init_t(const dsa_host *h) {
-  for (int ci = 0; ci < h->n_classes; ++ci) {
-    const fg_class_t &c = h->classes[ci];
-    if (!c.n_factors) continue;
-    launch(c.n_factors, [&] { k_dsa_con_opt<T>(c, (const T *)h->tables, (T *)h->con_opt, h->mode_max); });
+// round done, from buffer done & 1 (fg_dsa_current's buf_index) into the other one
+int64_t dsa_host_cycle(const fg_dsa_desc_t *d, int64_t done) {
+  fg_host_launcher launch;
+  if (d->n_vars) {
+    if (d->precision == FG_F64) dsa_step<double>(*d, d->classes, (int)(done & 1), (uint32_t)done, launch);
+    else dsa_step<float>(*d, d->classes, (int)(done & 1), (uint32_t)done, launch);
   }
-  launch(h->n_vars, [&] { k_dsa_init(side(h), h->n_vars, h->seed, h->value[0]); });
-  memcpy(h->value[1], h->value[0], sizeof(int32_t) * (size_t)h->n_vars);
+  return launch.launches;
 }
-
-template <typename T>
-static void step_t(const dsa_host *h, int cur, uint32_t cycle) {
-  launch(h->n_vars, [&] {
-    k_dsa_step_generic<T>(side(h), h->n_vars, (const T *)h->tables, (const T *)h->con_opt, h->value[cur],
-                          h->value[cur ^ 1], (T *)h->value_cost, h->mode_max, h->variant, h->seed, cycle,
-                          (const T *)h->var_cost, h->unary_off);
-  });
-}
-
-extern "C" void dsa_host_init(const dsa_host *h) { if (h->precision == FG_F64) init_t<double>(h); else init_t<float>(h); }
-extern "C" void dsa_host_step(const dsa_host *h, int cur, uint32_t cycle) {
-  if (h->precision == FG_F64) step_t<double>(h, cur, cycle); else step_t<float>(h, cur, cycle);
-}
+}  // extern "C"

@@ -3,17 +3,7 @@
 // maxsum_init_t / maxsum_compute_t in engine.cu (generic kernels only, as with PYDCOP_B200_NO_FAST=1).
 // Lets the kernels be compared with the oracle on shapes the GPU tests do not reach.  Nothing in the
 // product links or calls this.
-//   g++ -O1 -std=c++17 -ffp-contract=off -I/usr/local/cuda/include -shared -fPIC ...
-#include <math.h>
-#include <stdint.h>
-#include <string.h>
-
-struct Dim3 { unsigned x, y, z; };
-static thread_local Dim3 blockIdx, blockDim, threadIdx;
-#define __launch_bounds__(...)
-static inline float __int_as_float(unsigned x) { float f; memcpy(&f, &x, 4); return f; }
-static inline double __longlong_as_double(unsigned long long x) { double f; memcpy(&f, &x, 8); return f; }
-
+#include "cuda_host.h"
 #include "../../pydcop_b200/csrc/maxsum_generic.cuh"
 
 template <typename F>

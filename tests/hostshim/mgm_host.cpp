@@ -1,115 +1,30 @@
-// TEST INFRASTRUCTURE: runs the MGM CUDA kernel SOURCE (pydcop_b200/csrc/mgm_kernels.cuh) on the
-// CPU, one "thread" after the other, so its logic can be compared with the oracle and the
-// reference trajectories without a GPU.  Nothing in the product links or calls this.
-//   g++ -O1 -ffp-contract=off -shared -fPIC -o mgm_host.so mgm_host.cpp
-#include <stdint.h>
-
-struct Dim3 { unsigned x, y, z; };
-static thread_local Dim3 blockIdx, blockDim, threadIdx;
-#define __global__
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(n)
-
-struct float4 { float x, y, z, w; };
-struct float2 { float x, y; };
-struct double2 { double x, y; };
-#include "../../pydcop_b200/csrc/mgm_kernels.cuh"
+// TEST INFRASTRUCTURE: runs fg_mgm_init / fg_mgm_step's launch sequence (pydcop_b200/csrc/mgm_fast_kernels.cuh) on
+// the CPU.  The descriptor is the C-ABI's fg_mgm_desc_t with HOST pointers.  Nothing in the product links or calls
+// this.
+#include "cuda_host.h"
 #include "../../pydcop_b200/csrc/mgm_fast_kernels.cuh"
 
-template <typename F>
-static void launch(int n, int block, F body) {
-  blockDim = Dim3{(unsigned)block, 1, 1};
-  for (unsigned b = 0; b < (unsigned)((n + block - 1) / block); ++b)
-    for (unsigned t = 0; t < (unsigned)block; ++t) {
-      blockIdx = Dim3{b, 0, 0};
-      threadIdx = Dim3{t, 0, 0};
-      body();
+extern "C" {
+int64_t mgm_host_init(const fg_mgm_desc_t *d) {
+  fg_host_launcher launch;
+  if (d->n_vars) mgm_init(*d, d->classes, launch);
+  return launch.launches;
+}
+
+// round done + 1; -1 with the active-row arrays (dev_row_cache): that value phase is block-cooperative and has no
+// thread-by-thread run
+int64_t mgm_host_cycle(const fg_mgm_desc_t *d, int64_t done) {
+  if (d->dev_row_cache) return -1;
+  fg_host_launcher launch;
+  if (d->n_vars) {
+    if (d->precision == FG_F64) {
+      mgm_gain<double>(*d, d->classes, done, launch);
+      mgm_decide<double>(*d, d->classes, launch);
+    } else {
+      mgm_gain<float>(*d, d->classes, done, launch);
+      mgm_decide<float>(*d, d->classes, launch);
     }
-}
-
-extern "C" {
-
-struct mgm_host_arrays {
-  const fg_class_t *classes;
-  const int32_t *dom_size, *var_id, *var_rank, *edge_var, *edge_class, *var_ptr, *slot_edge, *nbr_ptr, *nbr_idx;
-  const int64_t *unary_off;
-  const int32_t *init_value;
-  const void *tables, *unary;
-  int32_t *value;
-  void *cost;
-  uint8_t *has_cost;
-  void *gain;
-  int32_t *new_value;
-  int32_t n_vars, precision, mode_max;
-  uint64_t seed;
-};
-
-static MgmSide side(const mgm_host_arrays *a) {
-  return MgmSide{a->classes, a->dom_size, a->var_id, a->var_rank, a->edge_var, a->edge_class,
-                 a->var_ptr, a->slot_edge, a->nbr_ptr, a->nbr_idx, a->unary_off};
-}
-
-void mgm_host_init(const mgm_host_arrays *a) {
-  launch(a->n_vars, 128, [&] { k_mgm_init(side(a), a->n_vars, a->init_value, a->seed, a->value, a->has_cost); });
-}
-
-}  // extern "C"
-
-template <typename T>
-static void cycle_t(const mgm_host_arrays *a, uint32_t cycle) {
-  launch(a->n_vars, 128, [&] {
-    k_mgm_gain<T>(side(a), a->n_vars, (const T *)a->tables, (const T *)a->unary, a->value, (T *)a->cost,
-                  a->has_cost, (T *)a->gain, a->new_value, a->mode_max, a->seed, cycle);
-  });
-  // the decide kernel of the GPU sees a consistent `gain` array (kernel boundary); sequential
-  // execution gives the same because gain / new_value are not written in this phase
-  launch(a->n_vars, 256, [&] {
-    k_mgm_decide<T>(side(a), a->n_vars, (const T *)a->gain, a->new_value, a->value, (T *)a->cost);
-  });
-}
-
-extern "C" {
-void mgm_host_cycle(const mgm_host_arrays *a, uint32_t cycle) {
-  if (a->precision == FG_F64) cycle_t<double>(a, cycle);
-  else cycle_t<float>(a, cycle);
-}
-}
-
-// ---- fast value phase (mgm_fast_kernels.cuh) ------------------------------------------------
-struct mgm_host_fast {
-  const int32_t *slot_nbr;
-  const int64_t *slot_tab;
-  const void *tables_or;
-  int32_t dom, chunk;
-};
-
-template <typename T, int D, int U>
-static void fast_cycle(const mgm_host_arrays *a, const mgm_host_fast *f, uint32_t cycle) {
-  launch(a->n_vars, 128, [&] {
-    k_mgm_gain_bin<T, D, U>(side(a), a->n_vars, f->slot_nbr, f->slot_tab, (const T *)f->tables_or, (const T *)a->unary,
-                            a->value, (T *)a->cost, a->has_cost, (T *)a->gain, a->new_value, a->mode_max, a->seed, cycle);
-  });
-  launch(a->n_vars, 256, [&] {
-    k_mgm_decide<T>(side(a), a->n_vars, (const T *)a->gain, a->new_value, a->value, (T *)a->cost);
-  });
-}
-
-template <typename T, int U>
-static int fast_by_dom(const mgm_host_arrays *a, const mgm_host_fast *f, uint32_t cycle) {
-  switch (f->dom) {
-    case 4: fast_cycle<T, 4, U>(a, f, cycle); return 0;
-    case 8: fast_cycle<T, 8, U>(a, f, cycle); return 0;
-    case 10: fast_cycle<T, 10, U>(a, f, cycle); return 0;
-    case 16: fast_cycle<T, 16, U>(a, f, cycle); return 0;
-    case 20: fast_cycle<T, 20, U>(a, f, cycle); return 0;
   }
-  return 3;
+  return launch.launches;
 }
-
-extern "C" int mgm_host_cycle_fast(const mgm_host_arrays *a, const mgm_host_fast *f, uint32_t cycle) {
-  if (a->precision == FG_F64) return f->chunk == 2 ? fast_by_dom<double, 2>(a, f, cycle) : fast_by_dom<double, 4>(a, f, cycle);
-  return f->chunk == 2 ? fast_by_dom<float, 2>(a, f, cycle) : fast_by_dom<float, 4>(a, f, cycle);
-}
+}  // extern "C"

@@ -2,19 +2,8 @@
 // the CPU, so it can be compared with the oracle and the reference traces without a GPU.  The block-wide selections
 // of k_syncbb become sequential scans over the candidates with the same predicates.  Nothing in the product links or
 // calls this.
-//   g++ -O1 -std=c++17 -ffp-contract=off -shared -fPIC -o syncbb_host.so syncbb_host.cpp
 // The descriptor is the C-ABI's fg_syncbb_desc_t with HOST pointers.
-#include <stdint.h>
-
-struct Dim3 { unsigned x, y, z; };
-static thread_local Dim3 blockIdx, blockDim, threadIdx, gridDim;
-#define __global__
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
-
+#include "cuda_host.h"
 #include "../../pydcop_b200/csrc/syncbb_kernels.cuh"
 
 template <typename T>

@@ -4,11 +4,9 @@
    one union layout with per-problem var_global_id / var_rank: every problem's slice of the state equals its own run
    at every cycle, bit for bit, in f32 and f64.
 2. solve_batch's host logic through the engine seam: grouping, cutting, order, refusals, the CLI."""
-import ctypes as C
 import functools
 import json
 import os
-import subprocess
 from unittest import mock
 
 import numpy as np
@@ -18,8 +16,7 @@ import test_gdba_hostshim as tg
 import test_mgm2_hostshim as tm2
 import test_mgm_hostshim as tm
 import test_mixeddsa_hostshim as tmx
-from conftest import ROOT
-from pydcop_b200 import batch, engine as eng_mod, ingest
+from pydcop_b200 import batch, ingest
 from pydcop_b200.generators import mixed_shape_graph
 from pydcop_b200.layout import build_layout
 from pydcop_b200.solve import main, name_rank, solve, solve_batch
@@ -77,47 +74,19 @@ def batch_problems(n, seed=0, modes=("min",), hard=False, n_range=(6, 40)):
 # ------------------------------------------------------------------------------------------------------------------
 # 1. kernel source: the union against every problem's own run
 # ------------------------------------------------------------------------------------------------------------------
-def _shim(name):
-    """tests/hostshim/<name>_host.cpp built for this file (the kernel headers are its dependencies)."""
-    src = os.path.join(ROOT, "tests", "hostshim", f"{name}_host.cpp")
-    so = os.path.join(ROOT, "tests", "hostshim", "_build", f"batch_{name}_host.so")
-    csrc = os.path.join(ROOT, "pydcop_b200", "csrc")
-    deps = [src, os.path.join(ROOT, "include", "pydcop_b200.h")] + [os.path.join(csrc, f) for f in os.listdir(csrc)]
-    if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-w", "-I", CUDA_INC, "-shared", "-fPIC",
-                        "-o", so, src], check=True, capture_output=True)
-    lib = C.CDLL(so)
-    for fn in ("gdba_host_cycle", "mixeddsa_host_cycle"):
-        if hasattr(lib, fn):
-            getattr(lib, fn).argtypes = [C.c_void_p, C.c_int64]
-    return lib
+_HOSTS = {"mgm": tm.HostMgm, "mgm2": tm2.HostMgm2, "gdba": tg.HostGdba, "mixeddsa": tmx.HostMixedDsa}
 
 
-_PLANS = {"mgm": (tm, "mgm_plan"), "mgm2": (tm2, "mgm2_plan"), "gdba": (tg, "gdba_plan"),
-          "mixeddsa": (tmx, "mixeddsa_plan")}
-_HOSTS = {"mgm": (tm.HostMgm, "mgm"), "mgm2": (tm2.HostMgm2, "mgm2"), "gdba": (tg.HostGdba, "gdba"),
-          "mixeddsa": (tmx.HostMixedDsa, "mixeddsa")}
-
-
-@functools.lru_cache(maxsize=None)
-def shim(name):
-    return _shim(name)
-
-
-def host_engine(kind, layout, inst, precision, mode, params, seed, var_rank=None, var_global_id=None):
-    """The host-shimmed engine of `kind` over `layout`: the engine's own plan (with var_global_id) stepped by the
-    kernel source."""
+def host_engine(kind, layout, inst, precision, mode, params, seed, var_rank=None, var_global_id=None, var_seed=None):
+    """The host-shimmed engine of `kind` over `layout`: the engine's own plan (with var_global_id / var_seed) run by
+    the kernel source."""
     if kind in ("dsa", "adsa"):
         return HostDsa(inst, precision=precision, mode=mode, seed=seed, var_global_id=var_global_id,
-                       var_costs=kind == "adsa", **params)
+                       var_costs=kind == "adsa", var_seed=var_seed, **params)
     if kind == "maxsum":
         return HostMaxSum(layout, precision=precision, mode=mode, **params)
-    module, plan = _PLANS[kind]
-    cls, lib = _HOSTS[kind]
-    with mock.patch.object(module, plan, functools.partial(getattr(eng_mod, plan), var_global_id=var_global_id)):
-        return cls(shim(lib), layout, precision=precision, mode=mode, seed=seed, var_rank=var_rank, **params)
+    return _HOSTS[kind](layout, precision=precision, mode=mode, seed=seed, var_rank=var_rank,
+                        var_global_id=var_global_id, var_seed=var_seed, **params)
 
 
 def _values(e):

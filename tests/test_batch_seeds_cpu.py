@@ -1,11 +1,10 @@
 """Per-problem seeds in a batch (a per-variable Philox key, solve_batch(seed=[...]), --iterations) without a GPU.
 
-1. The kernel source of every Philox family, run on the CPU through the host shims: a union of one problem repeated
-   with several seeds, and a union of distinct problems with distinct seeds, equals every member run alone with its
+1. The kernel source of every Philox family, run on the CPU through the host shims with the keys in each descriptor's
+   dev_var_seed: a union of one problem repeated with several seeds, and a union of distinct problems with distinct seeds, equals every member run alone with its
    own scalar seed, at every cycle, bit for bit; the repeats do not all follow one trajectory.
 2. A key array holding one value is the scalar seed; a plan without keys is the plan the engines always built.
 3. solve_batch and the CLI through the engine seam."""
-import ctypes as C
 import functools
 import json
 from unittest import mock
@@ -17,86 +16,10 @@ import test_batch_cpu as tb
 from pydcop_b200 import batch, engine as eng_mod, ingest
 from pydcop_b200.layout import build_layout
 from pydcop_b200.solve import main, name_rank, solve, solve_batch
-from test_dsa_generic_hostshim import HostDsa
-from test_mgm_hostshim import HostMgm
 
 pytestmark = tb.pytestmark
 
 SEEDS = [0, 1, 7, -5, 2 ** 40 + 3, 2 ** 64 - 1]   # -5 and 2**64 - 1 are keyed as solve() masks them
-
-
-def _p(a):
-    return C.c_void_p(a.ctypes.data if a is not None else 0)
-
-
-class SeededDsa(HostDsa):
-    """HostDsa with DsaSide::var_seed (tests/hostshim/dsa_seeded_host.cpp)."""
-
-    def __init__(self, inst, var_seed=None, **kw):
-        super().__init__(inst, **kw)
-        self.lib = tb.shim("dsa_seeded")
-        self.var_seed = None if var_seed is None else eng_mod._var_seeds(self.L, var_seed)
-
-    def init(self):
-        self.lib.dsa_host_init_seeded(C.byref(self.h), _p(self.var_seed))
-        self.cur, self.cycle = 0, 0
-        return self
-
-    def step(self, n=1):
-        for _ in range(n):
-            if self.stop_cycle and self.cycle >= self.stop_cycle:
-                break
-            self.lib.dsa_host_step_seeded(C.byref(self.h), self.cur, C.c_uint32(self.cycle), _p(self.var_seed))
-            self.cur ^= 1
-            self.cycle += 1
-        return self
-
-
-class SeededMgm(HostMgm):
-    """HostMgm with MgmSide::var_seed (tests/hostshim/mgm_seeded_host.cpp); the shim's array struct has no field for
-    it, so the keys are passed next to it."""
-
-    def __init__(self, lib, layout, var_global_id=None, var_seed=None, **kw):
-        keep = {}
-
-        def plan(*a, **k):
-            inputs, state, scalars = eng_mod.mgm_plan(*a, **k, var_global_id=var_global_id, var_seed=var_seed)
-            keep["var_seed"] = inputs.pop("var_seed", None)
-            return inputs, state, scalars
-        with mock.patch("test_mgm_hostshim.mgm_plan", plan):
-            super().__init__(lib, layout, **kw)
-        self.var_seed = keep["var_seed"]
-
-    def init(self):
-        self.lib.mgm_host_init_seeded(C.byref(self.a), _p(self.var_seed))
-        self.cycle = 0
-        return self
-
-    def step(self, n=1):
-        for _ in range(n):
-            if self.finished:
-                break
-            self.lib.mgm_host_cycle_seeded(C.byref(self.a), C.c_uint32(self.cycle + 1), _p(self.var_seed))
-            self.cycle += 1
-        return self
-
-
-def seeded_engine(kind, layout, inst, precision, mode, params, seed, var_rank=None, var_global_id=None, var_seed=None):
-    """tb.host_engine with the per-variable keys, stepped by tests/hostshim/<family>_seeded_host.cpp: the engine's own
-    plan (mgm2, gdba, mixeddsa: dev_var_seed of the descriptor) or the keys next to the shim's arrays (dsa, adsa,
-    mgm)."""
-    if kind in ("dsa", "adsa"):
-        return SeededDsa(inst, precision=precision, mode=mode, seed=seed, var_global_id=var_global_id,
-                         var_costs=kind == "adsa", var_seed=var_seed, **params)
-    if kind == "mgm":
-        return SeededMgm(tb.shim("mgm_seeded"), layout, precision=precision, mode=mode, seed=seed, var_rank=var_rank,
-                         var_global_id=var_global_id, var_seed=var_seed, **params)
-    module, plan = tb._PLANS[kind]
-    cls, lib = tb._HOSTS[kind]
-    with mock.patch.object(module, plan, functools.partial(getattr(eng_mod, plan), var_global_id=var_global_id,
-                                                           var_seed=var_seed)):
-        return cls(tb.shim(lib + "_seeded"), layout, precision=precision, mode=mode, seed=seed, var_rank=var_rank,
-                   **params)
 
 
 def _trajectory(e, n_cycles):
@@ -115,8 +38,8 @@ def check_seeds(kind, dcops, seeds, precision, params, n_cycles=12):
     assert u.var_seed is not None and u.var_seed.dtype == np.uint64
     L = batch.union_layout(u, dcops)
     # the scalar seed of the union is none of the members': every draw must take its variable's key
-    whole = _trajectory(seeded_engine(kind, L, u.inst, precision, mode, params, 12345, u.var_rank, u.var_global_id,
-                                      u.var_seed).init(), n_cycles)
+    whole = _trajectory(tb.host_engine(kind, L, u.inst, precision, mode, params, 12345, u.var_rank, u.var_global_id,
+                                        u.var_seed).init(), n_cycles)
     per_problem = []
     for i, (d, s) in enumerate(zip(dcops, seeds)):
         inst = d.instance()
@@ -174,7 +97,7 @@ def test_one_key_everywhere_is_the_scalar_seed(kind, params):
     inst = d.instance()
     L = build_layout(**inst)
     p = _host_params(kind, params)
-    keyed = _trajectory(seeded_engine(kind, L, inst, "f64", "min", p, 0, name_rank(d),
+    keyed = _trajectory(tb.host_engine(kind, L, inst, "f64", "min", p, 0, name_rank(d),
                                       var_seed=np.full(d.n_vars, 2 ** 33 + 9)).init(), 10)
     scalar = _trajectory(tb.host_engine(kind, L, inst, "f64", "min", p, 2 ** 33 + 9, name_rank(d)).init(), 10)
     for w, s in zip(keyed, scalar):
@@ -226,7 +149,7 @@ def seeded_factory(kind, layout, inst, params, seen=None):
     p = {k: v for k, v in params.items() if k not in ("mode", "seed", "noise")}
     if kind == "maxsum":
         return tb.factory(kind, layout, inst, params)
-    return seeded_engine(kind, layout, inst, "f64", params["mode"], _host_params(kind, p), params["seed"],
+    return tb.host_engine(kind, layout, inst, "f64", params["mode"], _host_params(kind, p), params["seed"],
                          inst.get("var_rank"), inst.get("var_global_id"), inst.get("var_seed"))
 
 

@@ -1,7 +1,7 @@
-"""The DBA CUDA kernel SOURCE executed on the CPU (tests/hostshim/dba_host.cpp compiles pydcop_b200/csrc/dba_kernels.cuh
-with g++ and loops over the threads) with exactly the arrays DbaEngine uploads (dba_plan): the violation bit rows
-against numpy, and the trajectories against the reference's (tests/golden/dba_*.npz) and the oracle's.  The device
-run is tests/test_gpu_zz_dba.py's."""
+"""The DBA CUDA kernel SOURCE executed on the CPU (tests/hostshim/dba_host.cpp runs fg_dba_init / fg_dba_step's launch
+sequence from pydcop_b200/csrc/dba_kernels.cuh, thread after thread) with exactly the arrays DbaEngine uploads
+(dba_plan): the violation bit rows against numpy, and the trajectories against the reference's
+(tests/golden/dba_*.npz) and the oracle's. The device run is tests/test_gpu_zz_dba.py's."""
 import ctypes as C
 import os
 import subprocess
@@ -11,46 +11,26 @@ import pytest
 
 import _limits as LM
 import oracle as orc
+from _hostshim import HostRun
 from _dba_oracle import LIVE, ROW_KEYS, DbaOracle
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
-from pydcop_b200.engine import _class_array, canonical_slot, dba_plan, fill_desc, fill_header, host_state
+from pydcop_b200.engine import canonical_slot, dba_plan
 from pydcop_b200.layout import layout_from_instance
 from test_dba_cpu import check_trajectory
 from test_mgm2_hostshim import random_mgm2_instance
 
-SHIM_SRC = os.path.join(ROOT, "tests", "hostshim", "dba_host.cpp")
-SHIM_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "dba_host.so")
 P = C.c_void_p
 
 
-@pytest.fixture(scope="module")
-def shim():
-    deps = [SHIM_SRC, os.path.join(ROOT, "include", "pydcop_b200.h")] + [
-        os.path.join(ROOT, "pydcop_b200", "csrc", f) for f in ("dba_kernels.cuh", "mgm_kernels.cuh", "philox.cuh")]
-    if not os.path.exists(SHIM_SO) or any(os.path.getmtime(d) > os.path.getmtime(SHIM_SO) for d in deps):
-        os.makedirs(os.path.dirname(SHIM_SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-o", SHIM_SO,
-                        SHIM_SRC], check=True, capture_output=True)
-    lib = C.CDLL(SHIM_SO)
-    lib.dba_host_cycle.argtypes = [P, C.c_int64]
-    return lib
+class HostDba(HostRun):
+    """DbaEngine's plan (dba_plan) run by tests/hostshim/dba_host.cpp; `cycle` is fg_dba_current's."""
 
-
-class HostDba:
-    """DbaEngine's plan (dba_plan) and driving API over the host-shimmed kernels."""
-
-    def __init__(self, lib, layout, precision="f64", infinity=10000, max_distance=50, stop_cycle=0, seed=0,
+    def __init__(self, layout, precision="f64", infinity=10000, max_distance=50, stop_cycle=0, seed=0,
                  var_rank=None, **_):
-        self.lib, self.L = lib, layout
-        inputs, state, scalars = dba_plan(layout, precision, infinity, max_distance, stop_cycle, seed, var_rank)
-        self.has_nbr = np.diff(inputs["nbr_ptr"]) > 0
-        self.k = dict(inputs, **host_state(state))
-        self.value = self.k["value"]
-        self.classes = _class_array(layout)
-        self.d = fill_desc(fill_header(_cabi.FgDbaDesc(), precision, layout, self.classes), self.k, scalars)
-        self.stop_cycle, self.rounds = scalars["stop_cycle"], 0
+        super().__init__("dba", layout, dba_plan(layout, precision, infinity, max_distance, stop_cycle, seed,
+                                                 var_rank), precision)
+        self.has_nbr = np.diff(self.k["nbr_ptr"]) > 0
 
     @property
     def end_round(self):
@@ -64,24 +44,11 @@ class HostDba:
     def cycle(self):
         return min(self.rounds, self.end_round)
 
-    def init(self):
-        self.lib.dba_host_init(C.byref(self.d))
-        self.rounds = 0
-        return self
-
-    def step(self, n=1):
-        for _ in range(n):
-            if self.finished:
-                break
-            self.lib.dba_host_cycle(C.byref(self.d), self.rounds)
-            self.rounds += 1
-        return self
-
     def values(self):
         L, k = self.L, self.k
         cost = k["cost"][:L.n_vars].astype(np.float64)
         cost[k["has_cost"][:L.n_vars] == 0] = np.nan
-        return L.vars_to_canonical(self.value[self.cycle % 2][:L.n_vars].copy()), L.vars_to_canonical(cost)
+        return L.vars_to_canonical(k["value"][self.cycle % 2][:L.n_vars].copy()), L.vars_to_canonical(cost)
 
     def record(self):
         L, k, n, E = self.L, self.k, self.L.n_vars, self.L.n_edges
@@ -138,9 +105,9 @@ def check_bits(eng, precision, infinity):
 
 @pytest.mark.parametrize("name", golden_names("dba_"))
 @pytest.mark.parametrize("precision", ["f64", "f32"])
-def test_kernel_source_matches_fixture(shim, name, precision):
+def test_kernel_source_matches_fixture(name, precision):
     inst, meta = orc.load_golden(os.path.join(GOLDEN_DIR, name + ".npz"))
-    eng = HostDba(shim, layout_from_instance(inst), precision=precision, seed=meta["seed"], var_rank=inst["var_rank"],
+    eng = HostDba(layout_from_instance(inst), precision=precision, seed=meta["seed"], var_rank=inst["var_rank"],
                   **meta["params"]).init()
     check_bits(eng, precision, meta["params"]["infinity"])
     check_trajectory(eng, inst, meta, name)
@@ -161,18 +128,18 @@ def random_dba_instance(n, d, seed, infinity=10000, frac=0.3):
 
 
 @pytest.mark.parametrize("precision,max_distance,infinity", [("f64", 3, 10000), ("f32", 2, 100), ("f64", 0, 10000)])
-def test_kernel_source_matches_oracle_on_random_graphs(shim, precision, max_distance, infinity):
+def test_kernel_source_matches_oracle_on_random_graphs(precision, max_distance, infinity):
     inst = random_dba_instance(500, 3, seed=13, infinity=infinity)
     dt = np.float64 if precision == "f64" else np.float32
     kw = dict(infinity=infinity, max_distance=max_distance, seed=5)
     o = DbaOracle(inst, dt, **kw).init()
-    eng = HostDba(shim, layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
+    eng = HostDba(layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
     check_bits(eng, precision, infinity)
     compare_with_oracle(eng, o, 12)
     assert o.stats["weight_raises"] > 0 and o.stats["moves"] > 0
 
 
-def test_kernel_source_flood_on_a_solvable_colouring(shim):
+def test_kernel_source_flood_on_a_solvable_colouring():
     """A sparse 3-colouring: variables stop, the End flood reaches every variable with neighbours, and rounds after
     the end change nothing."""
     rng = np.random.default_rng(4)
@@ -189,18 +156,18 @@ def test_kernel_source_flood_on_a_solvable_colouring(shim):
     inst["var_ptr"], inst["var_edge"] = default_var_csr(n, inst["edge_var"])
     kw = dict(max_distance=4, seed=9)
     o = DbaOracle(inst, **kw).init()
-    eng = HostDba(shim, layout_from_instance(inst), **kw).init()
+    eng = HostDba(layout_from_instance(inst), **kw).init()
     compare_with_oracle(eng, o, 80)
     assert o.ended and o.stats["stops"] > 0 and o.stats["floods"] > 0
     c, before = eng.cycle, eng.record()
     for r in range(eng.rounds, eng.rounds + 2):              # rounds enqueued after the end change nothing
-        eng.lib.dba_host_cycle(C.byref(eng.d), r)
+        eng.lib.dba_host_cycle(C.byref(eng.d), C.c_int64(r))
     after = eng.record()
     assert all(np.array_equal(before[k], after[k]) for k in ROW_KEYS) and eng.cycle == c
 
 
 @pytest.mark.parametrize("case", list(LM.LOCAL))
-def test_kernel_source_at_the_limits(shim, case):
+def test_kernel_source_at_the_limits(case):
     """Domain sizes 1 and 256 (8 words per row) and the mix {1, 2, 256} (tests/_limits.py), some entries raised
     to infinity."""
     inst = LM.LOCAL[case]()
@@ -209,7 +176,7 @@ def test_kernel_source_at_the_limits(shim, case):
     inst["tables"] = np.where(rng.random(len(t)) < 0.4, 10000.0, t)
     kw = dict(max_distance=3, seed=23)
     o = DbaOracle(inst, np.float64, **kw).init()
-    eng = HostDba(shim, layout_from_instance(inst), precision="f64", var_rank=inst["var_rank"], **kw).init()
+    eng = HostDba(layout_from_instance(inst), precision="f64", var_rank=inst["var_rank"], **kw).init()
     check_bits(eng, "f64", 10000)
     compare_with_oracle(eng, o, 6)
 
@@ -232,7 +199,7 @@ def test_descriptor_validation():
     import torch
     lib = _cabi.load()
     inst = random_dba_instance(60, 3, seed=1)
-    d = HostDba(None, layout_from_instance(inst)).d
+    d = HostDba(layout_from_instance(inst)).d
 
     def create():
         h = P()
@@ -282,13 +249,13 @@ def unresolved_instance():
     return unit_instance([[0, 1], [0, 1], [0, 1]], [([0, 1], inf), ([1, 2], inf)])
 
 
-def test_kernel_source_unresolved_keeps_the_value(shim):
+def test_kernel_source_unresolved_keeps_the_value():
     """Weights grown past infinity: the kernel keeps the current value, draws nothing, clears can_move and counts
     every such variable in every round, as the oracle does."""
     inst = unresolved_instance()
     kw = dict(infinity=3, max_distance=0, seed=2)
     o = DbaOracle(inst, **kw).init()
-    eng = HostDba(shim, layout_from_instance(inst), **kw).init()
+    eng = HostDba(layout_from_instance(inst), **kw).init()
     o.weight = [[5] * len(c) for c in o.cons]
     eng.k["weight"][:] = 5
     start = o.values()[0].copy()

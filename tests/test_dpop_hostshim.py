@@ -4,34 +4,23 @@ against the reference's messages (tests/golden/dpop_*.npz) and the oracle.  This
 per-node device functions and the host-side descriptors without a GPU; the device run is
 tests/test_gpu_zz_dpop.py's."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import _hostshim as hs
 from _dpop_oracle import DpopOracle
 import _limits as LM
-from conftest import ROOT
 from pydcop_b200 import _cabi, pseudotree as pt
 from pydcop_b200.engine import dpop_plan, fill_desc, host_state
 from pydcop_b200.layout import build_layout
 from test_dpop_cpu import NAMES, _integer_without_sentinel, check_against_golden, load, same, tree_of
 
-SHIM_SRC = os.path.join(ROOT, "tests", "hostshim", "dpop_host.cpp")
-SHIM_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "dpop_host.so")
 
 
 @pytest.fixture(scope="module")
 def shim():
-    deps = [SHIM_SRC, os.path.join(ROOT, "include", "pydcop_b200.h"),
-            os.path.join(ROOT, "pydcop_b200", "csrc", "dpop_kernels.cuh")]
-    if not os.path.exists(SHIM_SO) or any(os.path.getmtime(d) > os.path.getmtime(SHIM_SO) for d in deps):
-        os.makedirs(os.path.dirname(SHIM_SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-o", SHIM_SO,
-                        SHIM_SRC], check=True, capture_output=True)
-    lib = C.CDLL(SHIM_SO)
+    lib = hs.build("dpop_host")
     lib.dpop_host_run.argtypes = [C.c_void_p]
     return lib
 

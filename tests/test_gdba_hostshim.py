@@ -1,8 +1,7 @@
-"""The GDBA CUDA kernel SOURCE executed on the CPU (tests/hostshim/gdba_host.cpp compiles
-pydcop_b200/csrc/gdba_kernels.cuh with g++ and loops over the threads) with exactly the arrays
-GdbaEngine uploads, against the reference trajectories (tests/golden/gdba_*.npz) and the oracle.
-This checks the kernels' logic and the host-side array preparation without a GPU; the device run is
-tests/test_gpu_zz_gdba.py's."""
+"""The GDBA CUDA kernel SOURCE executed on the CPU (tests/hostshim/gdba_host.cpp runs fg_gdba_init / fg_gdba_step's
+launch sequence from pydcop_b200/csrc/gdba_kernels.cuh, thread after thread) with exactly the arrays GdbaEngine
+uploads, against the reference trajectories (tests/golden/gdba_*.npz) and the oracle. This checks the kernels' logic
+and the host-side array preparation without a GPU; the device run is tests/test_gpu_zz_gdba.py's."""
 import ctypes as C
 import os
 import subprocess
@@ -13,72 +12,34 @@ import pytest
 import _limits as LM
 import oracle as orc
 from _gdba_oracle import GdbaOracle
+from _hostshim import HostRun
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
-from pydcop_b200.engine import (_class_array, fill_desc, fill_header, gdba_host_arrays, gdba_modifiers_view,
-                                gdba_plan, host_state, mgm_host_arrays)
+from pydcop_b200.engine import gdba_host_arrays, gdba_modifiers_view, gdba_plan, mgm_host_arrays
 from pydcop_b200.layout import layout_from_instance
 from test_gdba_cpu import check_trajectory
 from test_mgm2_hostshim import random_mgm2_instance
 
-SHIM_SRC = os.path.join(ROOT, "tests", "hostshim", "gdba_host.cpp")
-SHIM_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "gdba_host.so")
 P = C.c_void_p
 
 
-@pytest.fixture(scope="module")
-def shim():
-    deps = [SHIM_SRC, os.path.join(ROOT, "include", "pydcop_b200.h")] + [
-        os.path.join(ROOT, "pydcop_b200", "csrc", f) for f in ("gdba_kernels.cuh", "mgm_kernels.cuh", "philox.cuh")]
-    if not os.path.exists(SHIM_SO) or any(os.path.getmtime(d) > os.path.getmtime(SHIM_SO) for d in deps):
-        os.makedirs(os.path.dirname(SHIM_SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-o", SHIM_SO,
-                        SHIM_SRC], check=True, capture_output=True)
-    lib = C.CDLL(SHIM_SO)
-    lib.gdba_host_cycle.argtypes = [P, C.c_int64]
-    return lib
+class HostGdba(HostRun):
+    """GdbaEngine's plan (gdba_plan) run by tests/hostshim/gdba_host.cpp."""
 
-
-class HostGdba:
-    """GdbaEngine's plan (gdba_plan) and driving API over the host-shimmed kernels."""
-
-    def __init__(self, lib, layout, precision="f64", mode="min", modifier="A", violation="NZ", increase_mode="E",
-                 stop_cycle=0, seed=0, var_rank=None, **_):
-        self.lib, self.L = lib, layout
-        inputs, state, scalars = gdba_plan(layout, precision, mode, modifier, violation, increase_mode, stop_cycle,
-                                           seed, var_rank)
-        self.has_nbr = np.diff(inputs["nbr_ptr"]) > 0
-        self.gh = gdba_host_arrays(layout, inputs["nbr_ptr"], increase_mode, violation)
+    def __init__(self, layout, precision="f64", mode="min", modifier="A", violation="NZ", increase_mode="E",
+                 stop_cycle=0, seed=0, var_rank=None, var_global_id=None, var_seed=None, **_):
+        plan = gdba_plan(layout, precision, mode, modifier, violation, increase_mode, stop_cycle, seed, var_rank,
+                         var_global_id=var_global_id, var_seed=var_seed)
+        super().__init__("gdba", layout, plan, precision)
+        self.has_nbr = np.diff(self.k["nbr_ptr"]) > 0
+        self.gh = gdba_host_arrays(layout, self.k["nbr_ptr"], increase_mode, violation)
         self.base_mod, self.increase_mode = (0 if modifier == "A" else 1), increase_mode
-        self.k = dict(inputs, **host_state(state))
-        self.value = self.k["value"]
-        self.classes = _class_array(layout)
-        self.d = fill_desc(fill_header(_cabi.FgGdbaDesc(), precision, layout, self.classes), self.k, scalars)
-        self.stop_cycle, self.cycle = scalars["stop_cycle"], 0
-
-    @property
-    def finished(self):
-        return bool(self.stop_cycle and self.cycle + 1 >= self.stop_cycle)
-
-    def init(self):
-        self.lib.gdba_host_init(C.byref(self.d))
-        self.cycle = 0
-        return self
-
-    def step(self, n=1):
-        for _ in range(n):
-            if self.finished:
-                break
-            self.lib.gdba_host_cycle(C.byref(self.d), self.cycle)
-            self.cycle += 1
-        return self
 
     def values(self):
         L, k = self.L, self.k
         cost = k["cost"][:L.n_vars].astype(np.float64)
         cost[k["has_cost"][:L.n_vars] == 0] = np.nan
-        return L.vars_to_canonical(self.value[self.cycle % 2][:L.n_vars].copy()), L.vars_to_canonical(cost)
+        return L.vars_to_canonical(self.value[:L.n_vars].copy()), L.vars_to_canonical(cost)
 
     def modifiers(self):
         return gdba_modifiers_view(self.gh, self.k["mod"], self.base_mod, self.increase_mode)
@@ -112,12 +73,12 @@ def compare_with_oracle(eng, o, dt, n_cycles):
 
 @pytest.mark.parametrize("name", golden_names("gdba_"))
 @pytest.mark.parametrize("precision", ["f64", "f32"])
-def test_kernel_source_matches_fixture(shim, name, precision):
+def test_kernel_source_matches_fixture(name, precision):
     """f64 against the reference's trajectory; f32 against the f32 oracle (float fixtures round
     differently in f32) and, for integer costs, against the trajectory as well."""
     inst, meta = orc.load_golden(os.path.join(GOLDEN_DIR, name + ".npz"))
     dt = np.float64 if precision == "f64" else np.float32
-    eng = HostGdba(shim, layout_from_instance(inst), precision=precision, mode=meta["mode"], seed=meta["seed"],
+    eng = HostGdba(layout_from_instance(inst), precision=precision, mode=meta["mode"], seed=meta["seed"],
                    var_rank=inst["var_rank"], **meta["params"]).init()
     if precision == "f64" or "float" not in name:
         check_trajectory(eng, inst, meta, dt, name)
@@ -142,13 +103,13 @@ MODE_GRID = [("A", "E"), ("A", "R"), ("A", "C"), ("A", "T"), ("M", "E"), ("M", "
 @pytest.mark.parametrize("modifier,increase_mode", MODE_GRID)
 @pytest.mark.parametrize("precision,mode,violation,levels", [("f64", "min", "NZ", 0), ("f32", "max", "NM", 3),
                                                              ("f32", "min", "MX", 3)])
-def test_kernel_source_matches_oracle_on_random_graphs(shim, modifier, increase_mode, precision, mode, violation,
+def test_kernel_source_matches_oracle_on_random_graphs(modifier, increase_mode, precision, mode, violation,
                                                        levels):
     inst = random_gdba_instance(400, 3, seed=13, levels=levels)
     dt = np.float64 if precision == "f64" else np.float32
     kw = dict(mode=mode, modifier=modifier, violation=violation, increase_mode=increase_mode, seed=5)
     o = GdbaOracle(inst, dt, **kw).init()
-    eng = HostGdba(shim, layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
+    eng = HostGdba(layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
     compare_with_oracle(eng, o, dt, 8)
     assert o.stats["breakouts"] > 0
     if increase_mode != "T":
@@ -194,7 +155,7 @@ def test_descriptor_validation():
     import torch
     lib = _cabi.load()
     inst = random_gdba_instance(60, 3, seed=1)
-    d = HostGdba(None, layout_from_instance(inst), violation="NM").d
+    d = HostGdba(layout_from_instance(inst), violation="NM").d
 
     def create():
         h = P()
@@ -225,14 +186,14 @@ def test_descriptor_validation():
         assert rc == _cabi.FG_ERR_CUDA and "no CUDA device" in msg
 
 
-def test_kernel_source_isolated_variables(shim):
+def test_kernel_source_isolated_variables():
     """A variable without neighbours keeps optimal_cost_value over its own costs: here the unary
     constraint is NOT part of it (gdba.py:304-315)."""
     from test_mgm2_cpu import unit_instance
     inst = unit_instance([list(range(3))], [([0], lambda x: 5 - x)])
     inst["unary"] = np.array([1.0, 0.5, 0.5])
     for precision, mode, want in (("f64", "min", 1), ("f32", "max", 0)):
-        eng = HostGdba(shim, layout_from_instance(inst), precision=precision, mode=mode).init().step(3)
+        eng = HostGdba(layout_from_instance(inst), precision=precision, mode=mode).init().step(3)
         val, cost = eng.values()
         assert val.tolist() == [want] and cost.tolist() == [inst["unary"][want]]
         o = GdbaOracle(inst, mode=mode).init().step(3)
@@ -241,11 +202,11 @@ def test_kernel_source_isolated_variables(shim):
 
 @pytest.mark.parametrize("modifier,increase_mode", LM.GDBA_MODES)
 @pytest.mark.parametrize("case", list(LM.LOCAL))
-def test_kernel_source_at_the_limits(shim, case, modifier, increase_mode):
+def test_kernel_source_at_the_limits(case, modifier, increase_mode):
     """Domain sizes 1 and 256 and the mix {1, 2, 256} (tests/_limits.py), as tests/test_gpu_limits.py runs them."""
     inst = LM.gdba_instance(case)
     kw = dict(mode="min", modifier=modifier, violation="NZ", increase_mode=increase_mode, seed=23)
     o = GdbaOracle(inst, np.float64, **kw).init()
-    eng = HostGdba(shim, layout_from_instance(inst), precision="f64", var_rank=inst["var_rank"], **kw).init()
+    eng = HostGdba(layout_from_instance(inst), precision="f64", var_rank=inst["var_rank"], **kw).init()
     compare_with_oracle(eng, o, np.float64, 6)
     assert o.stats["breakouts"] > 0

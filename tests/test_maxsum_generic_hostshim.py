@@ -4,24 +4,21 @@ the oracle and the reference trajectories — including shapes the GPU tests do 
 to 6, domain sizes up to 40, hub variables).  Needs the CUDA toolkit headers (not a GPU)."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 from hypothesis import given, settings, strategies as st
 
+import _hostshim as hs
+from _hostshim import CUDA_INC
 import _limits as LM
 import oracle as orc
 from bench import oracle_instance
-from conftest import GOLDEN_DIR, ROOT, golden_names
+from conftest import GOLDEN_DIR, golden_names
 from pydcop_b200 import _cabi
 from pydcop_b200.engine import _class_array, _varclass_array
-from pydcop_b200.generators import random_factor_graph
 from pydcop_b200.layout import build_layout, layout_from_instance
 
-SRC = os.path.join(ROOT, "tests", "hostshim", "maxsum_generic_host.cpp")
-SO = os.path.join(ROOT, "tests", "hostshim", "_build", "maxsum_generic_host.so")
-CUDA_INC = "/usr/local/cuda/include"
 P = C.c_void_p
 
 pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")),
@@ -41,14 +38,7 @@ class _Host(C.Structure):
 
 
 def _lib():
-    deps = [SRC] + [os.path.join(ROOT, "pydcop_b200", "csrc", f) for f in ("maxsum_generic.cuh", "common.cuh")] \
-        + [os.path.join(ROOT, "include", "pydcop_b200.h")]
-    if not os.path.exists(SO) or any(os.path.getmtime(d) > os.path.getmtime(SO) for d in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-I", CUDA_INC, "-shared", "-fPIC",
-                        "-o", SO, SRC], check=True, capture_output=True)
-    return C.CDLL(SO)
+    return hs.build("maxsum_generic_host")
 
 
 class HostMaxSum:

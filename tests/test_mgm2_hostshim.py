@@ -1,73 +1,37 @@
-"""The MGM-2 CUDA kernel SOURCE executed on the CPU (tests/hostshim/mgm2_host.cpp compiles
-pydcop_b200/csrc/mgm2_kernels.cuh with g++ and loops over the threads) with exactly the arrays
-Mgm2Engine uploads, against the reference trajectories (tests/golden/mgm2_*.npz) and the oracle.
-This checks the kernels' logic and the host-side array preparation without a GPU; the device run is
-tests/test_gpu_zz_mgm2.py's."""
+"""The MGM-2 CUDA kernel SOURCE executed on the CPU (tests/hostshim/mgm2_host.cpp runs fg_mgm2_init / fg_mgm2_step's
+launch sequence from pydcop_b200/csrc/mgm2_kernels.cuh, thread after thread) with exactly the arrays Mgm2Engine
+uploads, against the reference trajectories (tests/golden/mgm2_*.npz) and the oracle. This checks the kernels' logic
+and the host-side array preparation without a GPU; the device run is tests/test_gpu_zz_mgm2.py's."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import _limits as LM
 import oracle as orc
+from _hostshim import HostRun
 from _mgm2_oracle import Mgm2Oracle
-from conftest import GOLDEN_DIR, ROOT, golden_names
+from conftest import GOLDEN_DIR, golden_names
 from pydcop_b200 import _cabi
-from pydcop_b200.engine import (_class_array, fill_desc, fill_header, host_state, mgm2_offer_offsets,
-                                mgm2_plan, mgm_host_arrays)
+from pydcop_b200.engine import mgm2_offer_offsets, mgm2_plan, mgm_host_arrays
 from pydcop_b200.generators import random_factor_graph
 from pydcop_b200.layout import default_var_csr, layout_from_instance
 from test_mgm2_cpu import check_trajectory
 
-SHIM_SRC = os.path.join(ROOT, "tests", "hostshim", "mgm2_host.cpp")
-SHIM_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "mgm2_host.so")
 P = C.c_void_p
 
 
-@pytest.fixture(scope="module")
-def shim():
-    deps = [SHIM_SRC, os.path.join(ROOT, "include", "pydcop_b200.h")] + [
-        os.path.join(ROOT, "pydcop_b200", "csrc", f) for f in ("mgm2_kernels.cuh", "mgm_kernels.cuh", "philox.cuh")]
-    if not os.path.exists(SHIM_SO) or any(os.path.getmtime(d) > os.path.getmtime(SHIM_SO) for d in deps):
-        os.makedirs(os.path.dirname(SHIM_SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-o", SHIM_SO,
-                        SHIM_SRC], check=True, capture_output=True)
-    return C.CDLL(SHIM_SO)
+class HostMgm2(HostRun):
+    """Mgm2Engine's plan (mgm2_plan) run by tests/hostshim/mgm2_host.cpp."""
 
-
-class HostMgm2:
-    """Mgm2Engine's plan (mgm2_plan) and driving API over the host-shimmed kernels."""
-
-    def __init__(self, lib, layout, precision="f64", mode="min", threshold=0.5, favor="unilateral",
-                 stop_cycle=0, seed=0, var_rank=None, **_):
-        self.lib, self.L = lib, layout
-        inputs, state, scalars = mgm2_plan(layout, precision, mode, threshold, favor, stop_cycle, seed, var_rank)
-        self.nbr_ptr, self.nbr_idx = inputs["nbr_ptr"], inputs["nbr_idx"]
+    def __init__(self, layout, precision="f64", mode="min", threshold=0.5, favor="unilateral", stop_cycle=0, seed=0,
+                 var_rank=None, var_global_id=None, var_seed=None, **_):
+        plan = mgm2_plan(layout, precision, mode, threshold, favor, stop_cycle, seed, var_rank,
+                         var_global_id=var_global_id, var_seed=var_seed)
+        super().__init__("mgm2", layout, plan, precision)
+        self.nbr_ptr, self.nbr_idx = self.k["nbr_ptr"], self.k["nbr_idx"]
         self.has_nbr = np.diff(self.nbr_ptr) > 0
-        self.k = dict(inputs, **host_state(state))
-        self.classes = _class_array(layout)
-        self.d = fill_desc(fill_header(_cabi.FgMgm2Desc(), precision, layout, self.classes), self.k, scalars)
-        self.stop_cycle, self.cycle = scalars["stop_cycle"], 0
-
-    @property
-    def finished(self):
-        return bool(self.stop_cycle and self.cycle + 1 >= self.stop_cycle)
-
-    def init(self):
-        self.lib.mgm2_host_init(C.byref(self.d))
-        self.cycle = 0
-        return self
-
-    def step(self, n=1):
-        for _ in range(n):
-            if self.finished:
-                break
-            self.lib.mgm2_host_cycle(C.byref(self.d), C.c_uint32(self.cycle + 1))
-            self.cycle += 1
-        return self
 
     def values(self):
         L, k = self.L, self.k
@@ -101,13 +65,13 @@ def _assert_same(a, b, dt, k):
 
 @pytest.mark.parametrize("name", golden_names("mgm2_"))
 @pytest.mark.parametrize("precision", ["f64", "f32"])
-def test_kernel_source_matches_fixture(shim, name, precision):
+def test_kernel_source_matches_fixture(name, precision):
     """f64 against the reference's trajectory; f32 against the f32 oracle (float fixtures round
     differently in f32) and, for integer costs, against the trajectory as well."""
     inst, meta = orc.load_golden(os.path.join(GOLDEN_DIR, name + ".npz"))
     dt = np.float64 if precision == "f64" else np.float32
     L = layout_from_instance(inst)
-    eng = HostMgm2(shim, L, precision=precision, mode=meta["mode"], seed=meta["seed"], var_rank=inst["var_rank"],
+    eng = HostMgm2(L, precision=precision, mode=meta["mode"], seed=meta["seed"], var_rank=inst["var_rank"],
                    **meta["params"]).init()
     if precision == "f64" or "float" not in name:
         check_trajectory(eng, inst, meta, dt, name)
@@ -156,13 +120,13 @@ def random_mgm2_instance(n, d, arities, seed, n_factors=None, levels=0):
                                                                   ("f64", "min", "no", 0.5, 2),
                                                                   ("f64", "max", "coordinated", 0.5, 3),
                                                                   ("f32", "min", "coordinated", 0.5, 2)])
-def test_kernel_source_matches_oracle_on_random_graphs(shim, precision, mode, favor, threshold, levels):
+def test_kernel_source_matches_oracle_on_random_graphs(precision, mode, favor, threshold, levels):
     """Float costs, and integer costs with few levels, where the favor rule decides ties."""
     inst = random_mgm2_instance(600, 4 if not levels else 3, [2, 3, 1], seed=11, levels=levels)
     dt = np.float64 if precision == "f64" else np.float32
     kw = dict(mode=mode, favor=favor, threshold=threshold, seed=5)
     o = Mgm2Oracle(inst, dt, **kw).init()
-    eng = HostMgm2(shim, layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
+    eng = HostMgm2(layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
     assert np.array_equal(eng.values()[0], o.values()[0])
     pairs = 0
     for k in range(1, 9):
@@ -205,7 +169,7 @@ def test_descriptor_validation():
     import torch
     lib = _cabi.load()
     inst = random_mgm2_instance(60, 3, [2], seed=1)
-    d = HostMgm2(None, layout_from_instance(inst)).d
+    d = HostMgm2(layout_from_instance(inst)).d
 
     def create():
         h = P()
@@ -230,26 +194,26 @@ def test_descriptor_validation():
         assert rc == _cabi.FG_ERR_CUDA and "no CUDA device" in msg
 
 
-def test_kernel_source_no_neighbors(shim):
+def test_kernel_source_no_neighbors():
     """The reference's test_no_neighbors through the init kernel: max mode, cost x1 * 2 over 0..9 gives
     value 9 with cost 18."""
     from test_mgm2_cpu import unit_instance
     inst = unit_instance([list(range(10))], [([0], lambda x1: x1 * 2)])
     for precision in ("f64", "f32"):
-        eng = HostMgm2(shim, layout_from_instance(inst), precision=precision, mode="max").init()
+        eng = HostMgm2(layout_from_instance(inst), precision=precision, mode="max").init()
         val, cost = eng.values()
         assert val.tolist() == [9] and cost.tolist() == [18.0]
 
 
 @pytest.mark.parametrize("precision,mode,favor", [("f32", "min", "no"), ("f64", "max", "coordinated")])
 @pytest.mark.parametrize("case", list(LM.LOCAL))
-def test_kernel_source_at_the_limits(shim, case, precision, mode, favor):
+def test_kernel_source_at_the_limits(case, precision, mode, favor):
     """Domain sizes 1 and 256 and the mix {1, 2, 256} (tests/_limits.py), as tests/test_gpu_limits.py runs them."""
     inst = LM.LOCAL[case]()
     dt = np.float64 if precision == "f64" else np.float32
     kw = dict(mode=mode, favor=favor, threshold=0.5, seed=19)
     o = Mgm2Oracle(inst, dt, **kw).init()
-    eng = HostMgm2(shim, layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
+    eng = HostMgm2(layout_from_instance(inst), precision=precision, var_rank=inst["var_rank"], **kw).init()
     assert np.array_equal(eng.values()[0], o.values()[0])
     offers = 0
     for k in range(1, 5):

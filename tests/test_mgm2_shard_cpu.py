@@ -1,11 +1,10 @@
 """Sharded MGM-2 on CPU: the shard builder, and the whole init / five-exchange cycle over torch.distributed (gloo,
-world 2 and 3) with the sharded kernel SOURCE on the CPU (tests/hostshim/mgm2_shard_host.cpp compiles
-pydcop_b200/csrc/mgm2_shard_kernels.cuh with g++) in the engine seam of ShardedMgm2.  Every cycle must equal the
+world 2 and 3) with the sharded kernel SOURCE on the CPU (tests/hostshim/mgm2_shard_host.cpp runs
+the fg_mgm2_shard_* launch sequences of pydcop_b200/csrc/mgm2_shard_kernels.cuh) in the engine seam of ShardedMgm2.  Every cycle must equal the
 single-process run of the kernel source (tests/hostshim/mgm2_host.cpp) and Mgm2Oracle bit for bit."""
 import ctypes as C
 import os
 import socket
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,39 +12,24 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+import _hostshim as hs
 import oracle as orc
 from _mgm2_oracle import Mgm2Oracle
-from conftest import GOLDEN_DIR, ROOT, golden_names
+from conftest import GOLDEN_DIR, golden_names
 from pydcop_b200 import _cabi
 from pydcop_b200.engine import _class_array, distinct_neighbours, fill_desc, fill_header, host_state, mgm2_plan
 from pydcop_b200.layout import layout_from_instance
 from pydcop_b200.multigpu import resolve_owner
 from pydcop_b200.multigpu_mgm2 import EXCHANGES, build_mgm2_shard
+from test_mgm2_hostshim import HostMgm2
 
-SHIM_SRC = os.path.join(ROOT, "tests", "hostshim", "mgm2_shard_host.cpp")
-SHIM_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "mgm2_shard_host.so")
-SINGLE_SRC = os.path.join(ROOT, "tests", "hostshim", "mgm2_host.cpp")
-SINGLE_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "mgm2_host.so")
 KEYS = ("value", "cost", "gain", "committed", "partner", "go")
-
-
-def _compile(src, so, headers):
-    deps = [src, os.path.join(ROOT, "include", "pydcop_b200.h")] + [
-        os.path.join(ROOT, "pydcop_b200", "csrc", f) for f in headers]
-    if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        tmp = f"{so}.{os.getpid()}"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-o", tmp, src],
-                       check=True, capture_output=True)
-        os.replace(tmp, so)
-    return so
 
 
 @pytest.fixture(scope="module")
 def shims():
-    base = ("mgm2_kernels.cuh", "mgm_kernels.cuh", "philox.cuh")
-    return (_compile(SHIM_SRC, SHIM_SO, base + ("mgm2_shard_kernels.cuh",)), _compile(SINGLE_SRC, SINGLE_SO, base))
+    """Both shims built before the gloo workers start (they load the cached libraries)."""
+    return hs.build("mgm2_shard_host"), hs.build("mgm2_host")
 
 
 class HostShardMgm2:
@@ -53,11 +37,11 @@ class HostShardMgm2:
     buffers are torch CPU tensors for gloo)."""
 
     def __init__(self, layout, inst=None, precision="f64", mode="min", threshold=0.5, favor="unilateral",
-                 stop_cycle=0, seed=0, var_rank=None, var_global_id=None, so=SHIM_SO):
-        self.lib = C.CDLL(so)
+                 stop_cycle=0, seed=0, var_rank=None, var_global_id=None):
+        self.lib = hs.build("mgm2_shard_host")
         self.layout, self.precision = layout, precision
         inputs, state, scalars = mgm2_plan(layout, precision, mode, threshold, favor, stop_cycle, seed, var_rank,
-                                           var_global_id)
+                                           var_global_id=var_global_id)
         self.k = dict(inputs, **host_state(state))
         self.classes = _class_array(layout)
         self.d = fill_desc(fill_header(_cabi.FgMgm2Desc(), precision, layout, self.classes), self.k, scalars)
@@ -91,7 +75,7 @@ class HostShardMgm2:
         self.cycle = 0
 
     def shard_phase(self, x):
-        self.lib.mgm2_shard_host_phase(C.byref(self.d), C.byref(self.plan), C.c_int32(x), C.c_uint32(self.cycle + 1))
+        self.lib.mgm2_shard_host_phase(C.byref(self.d), C.byref(self.plan), C.c_int32(x), C.c_int64(self.cycle))
         if x == EXCHANGES - 1:
             self.cycle += 1
 
@@ -103,25 +87,8 @@ class HostShardMgm2:
         return L.vars_to_canonical(self.k["value"][:L.n_vars].copy()), None
 
 
-class HostMgm2Single:
-    """The single-process kernel source (tests/hostshim/mgm2_host.cpp): every variable's state per cycle."""
-
-    def __init__(self, layout, precision, so=SINGLE_SO, **kw):
-        self.lib, self.L = C.CDLL(so), layout
-        inputs, state, scalars = mgm2_plan(layout, precision, **kw)
-        self.k = dict(inputs, **host_state(state))
-        self.classes = _class_array(layout)
-        self.d = fill_desc(fill_header(_cabi.FgMgm2Desc(), precision, layout, self.classes), self.k, scalars)
-        self.stop_cycle, self.cycle = scalars["stop_cycle"], 0
-
-    def init(self):
-        self.lib.mgm2_host_init(C.byref(self.d))
-        return self
-
-    def step(self):
-        if not (self.stop_cycle and self.cycle + 1 >= self.stop_cycle):
-            self.lib.mgm2_host_cycle(C.byref(self.d), C.c_uint32(self.cycle + 1))
-            self.cycle += 1
+class HostMgm2Single(HostMgm2):
+    """The single-process run (tests/hostshim/mgm2_host.cpp): every variable's state per cycle."""
 
     def state(self):
         L, n = self.L, self.L.n_vars
@@ -291,7 +258,7 @@ def _check(shims, world, cases):
         dt = np.float64 if precision == "f64" else np.float32
         L = layout_from_instance(inst)
         kw = dict(params, var_rank=inst.get("var_rank"))
-        single = HostMgm2Single(L, precision, so=shims[1], **kw).init()
+        single = HostMgm2Single(L, precision, **kw).init()
         o = Mgm2Oracle(inst, dt, **params).init()
         V = L.n_vars
         moved = 0
@@ -380,7 +347,7 @@ def test_distributed_solve_mgm2_equals_single_process(shims, params, kw):
     assert a["assignment"] == b["assignment"] and a["n_gpus"] == 2
 
     def single_engine(kind, layout, inst, p):
-        e = HostMgm2Single(layout, "f64", so=shims[1], mode=p["mode"], threshold=p["threshold"], favor=p["favor"],
+        e = HostMgm2Single(layout, "f64", mode=p["mode"], threshold=p["threshold"], favor=p["favor"],
                            stop_cycle=p["stop_cycle"], seed=p["seed"], var_rank=inst["var_rank"])
 
         class Run:

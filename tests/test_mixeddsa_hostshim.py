@@ -1,7 +1,7 @@
-"""The MixedDSA CUDA kernel SOURCE executed on the CPU (tests/hostshim/mixeddsa_host.cpp compiles
-pydcop_b200/csrc/mixeddsa_kernels.cuh with g++ and loops over the threads) with exactly the arrays MixedDsaEngine
-uploads (engine.mixeddsa_plan), against the reference trajectories (tests/golden/mixeddsa_*.npz) and the oracle, in
-f64 and f32.  The device run is tests/test_gpu_zz_mixeddsa.py's."""
+"""The MixedDSA CUDA kernel SOURCE executed on the CPU (tests/hostshim/mixeddsa_host.cpp runs fg_mixeddsa_init /
+fg_mixeddsa_step's launch sequence from pydcop_b200/csrc/mixeddsa_kernels.cuh, thread after thread) with exactly the
+arrays MixedDsaEngine uploads (engine.mixeddsa_plan), against the reference trajectories
+(tests/golden/mixeddsa_*.npz) and the oracle, in f64 and f32. The device run is tests/test_gpu_zz_mixeddsa.py's."""
 import ctypes as C
 import os
 import subprocess
@@ -11,71 +11,31 @@ import pytest
 
 import _limits as LM
 import oracle as orc
+from _hostshim import HostRun
 from _mixeddsa_oracle import MixedDsaOracle
 from conftest import GOLDEN_DIR, ROOT, golden_names
 from pydcop_b200 import _cabi
-from pydcop_b200.engine import (_class_array, fill_desc, fill_header, host_state, mixeddsa_hard_factors,
-                                mixeddsa_plan, mixeddsa_slots)
+from pydcop_b200.engine import mixeddsa_hard_factors, mixeddsa_plan, mixeddsa_slots
 from pydcop_b200.layout import layout_from_instance
 from test_mixeddsa_cpu import EXACT_F32, check_trajectory
 
-SHIM_SRC = os.path.join(ROOT, "tests", "hostshim", "mixeddsa_host.cpp")
-SHIM_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "mixeddsa_host.so")
-CUDA_INC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include")
 P = C.c_void_p
 
 
-@pytest.fixture(scope="module")
-def shim():
-    deps = [SHIM_SRC, os.path.join(ROOT, "include", "pydcop_b200.h")] + [
-        os.path.join(ROOT, "pydcop_b200", "csrc", f)
-        for f in ("mixeddsa_kernels.cuh", "dsa_generic.cuh", "mgm_kernels.cuh", "philox.cuh")]
-    if not os.path.exists(SHIM_SO) or any(os.path.getmtime(d) > os.path.getmtime(SHIM_SO) for d in deps):
-        os.makedirs(os.path.dirname(SHIM_SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-w", "-I", CUDA_INC, "-shared", "-fPIC", "-o",
-                        SHIM_SO, SHIM_SRC], check=True, capture_output=True)
-    lib = C.CDLL(SHIM_SO)
-    lib.mixeddsa_host_cycle.argtypes = [P, C.c_int64]
-    return lib
+class HostMixedDsa(HostRun):
+    """MixedDsaEngine's plan (mixeddsa_plan) run by tests/hostshim/mixeddsa_host.cpp."""
 
-
-class HostMixedDsa:
-    """MixedDsaEngine's plan (mixeddsa_plan) and driving API over the host-shimmed kernels."""
-
-    def __init__(self, lib, layout, precision="f64", mode="min", proba_hard=0.7, proba_soft=0.5, variant="B",
-                 stop_cycle=0, seed=0, **_):
-        self.lib, self.L = lib, layout
-        inputs, state, scalars = mixeddsa_plan(layout, precision, mode, proba_hard, proba_soft, variant, stop_cycle,
-                                               seed)
-        self.k = dict(inputs, **host_state(state))
-        self.value = self.k["value"]
-        self.classes = _class_array(layout)
-        self.d = fill_desc(fill_header(_cabi.FgMixedDsaDesc(), precision, layout, self.classes), self.k, scalars)
-        self.stop_cycle, self.cycle = scalars["stop_cycle"], 0
-
-    @property
-    def finished(self):
-        return bool(self.stop_cycle and self.cycle >= self.stop_cycle)
-
-    def init(self):
-        self.lib.mixeddsa_host_init(C.byref(self.d))
-        self.cycle = 0
-        return self
-
-    def step(self, n=1):
-        for _ in range(n):
-            if self.finished:
-                break
-            self.lib.mixeddsa_host_cycle(C.byref(self.d), self.cycle)
-            self.cycle += 1
-        return self
+    def __init__(self, layout, precision="f64", mode="min", proba_hard=0.7, proba_soft=0.5, variant="B",
+                 stop_cycle=0, seed=0, var_global_id=None, var_seed=None, **_):
+        plan = mixeddsa_plan(layout, precision, mode, proba_hard, proba_soft, variant, stop_cycle, seed,
+                             var_global_id=var_global_id, var_seed=var_seed)
+        super().__init__("mixeddsa", layout, plan, precision)
 
     def values(self):
         L, k = self.L, self.k
         cost = k["cost"][:L.n_vars].astype(np.float64)
         cost[k["has_cost"][:L.n_vars] == 0] = np.nan
-        return L.vars_to_canonical(self.value[self.cycle % 2][:L.n_vars].copy()), L.vars_to_canonical(cost)
+        return L.vars_to_canonical(self.value[:L.n_vars].copy()), L.vars_to_canonical(cost)
 
     def record(self):
         L, k, n = self.L, self.k, self.L.n_vars
@@ -97,12 +57,12 @@ def compare_with_oracle(eng, o, dt, n_cycles):
 
 @pytest.mark.parametrize("name", golden_names("mixeddsa_"))
 @pytest.mark.parametrize("precision", ["f64", "f32"])
-def test_kernel_source_matches_fixture(shim, name, precision):
+def test_kernel_source_matches_fixture(name, precision):
     """f64 against the reference's trajectory; f32 against it on the exact-cost fixtures, else against the f32
     oracle."""
     inst, meta = orc.load_golden(os.path.join(GOLDEN_DIR, name + ".npz"))
     dt = np.float64 if precision == "f64" else np.float32
-    eng = HostMixedDsa(shim, layout_from_instance(inst), precision=precision, mode=meta["mode"], seed=meta["seed"],
+    eng = HostMixedDsa(layout_from_instance(inst), precision=precision, mode=meta["mode"], seed=meta["seed"],
                        **meta["params"]).init()
     if precision == "f64" or name in EXACT_F32:
         check_trajectory(eng, inst, meta, dt, name)
@@ -147,12 +107,12 @@ RANDOM_RUNS = [("f64", "min", "B", 0, False), ("f64", "max", "A", 4, False), ("f
 
 
 @pytest.mark.parametrize("precision,mode,variant,levels,neg", RANDOM_RUNS)
-def test_kernel_source_matches_oracle_on_random_graphs(shim, precision, mode, variant, levels, neg):
+def test_kernel_source_matches_oracle_on_random_graphs(precision, mode, variant, levels, neg):
     inst = random_mixed(300, seed=17 + levels, levels=levels, neg=neg)
     dt = np.float64 if precision == "f64" else np.float32
     kw = dict(mode=mode, variant=variant, proba_hard=0.8, proba_soft=0.6, seed=9)
     o = MixedDsaOracle(inst, dt, **kw).init()
-    eng = HostMixedDsa(shim, layout_from_instance(inst), precision=precision, **kw).init()
+    eng = HostMixedDsa(layout_from_instance(inst), precision=precision, **kw).init()
     compare_with_oracle(eng, o, dt, 6)
 
 
@@ -171,13 +131,13 @@ def limits_instance(case):
 
 
 @pytest.mark.parametrize("case", list(LIMITS))
-def test_kernel_source_at_the_limits(shim, case):
+def test_kernel_source_at_the_limits(case):
     """Domain sizes 1 and 256, arity 8, a degree-2400 hub, unary-only and factor-free graphs."""
     inst = limits_instance(case)
     kw = dict(mode="min", variant="B", proba_hard=0.9, proba_soft=0.9, seed=23)
     for precision, dt in (("f64", np.float64), ("f32", np.float32)):
         o = MixedDsaOracle(inst, dt, **kw).init()
-        eng = HostMixedDsa(shim, layout_from_instance(inst), precision=precision, **kw).init()
+        eng = HostMixedDsa(layout_from_instance(inst), precision=precision, **kw).init()
         compare_with_oracle(eng, o, dt, 3 if case == "hub2400" else 4)
 
 
@@ -212,7 +172,7 @@ def test_descriptor_validation():
     every check, and without a device create reports FG_ERR_CUDA — never a CPU path."""
     import torch
     lib = _cabi.load()
-    d = HostMixedDsa(None, layout_from_instance(random_mixed(60, seed=1))).d
+    d = HostMixedDsa(layout_from_instance(random_mixed(60, seed=1))).d
 
     def create():
         h = P()

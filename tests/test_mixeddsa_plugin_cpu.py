@@ -189,7 +189,7 @@ def test_plan_passes_every_create_check():
     for inst in (random_mixed(80, seed=4), limits_instance("no_factors"), limits_instance("d256")):
         for precision in ("f32", "f64"):
             for variant in "ABC":
-                d = HostMixedDsa(None, layout_from_instance(inst), precision=precision, variant=variant,
+                d = HostMixedDsa(layout_from_instance(inst), precision=precision, variant=variant,
                                  mode="max", stop_cycle=3).d
                 h = C.c_void_p()
                 rc = lib.fg_mixeddsa_create(C.byref(d), C.byref(h))

@@ -9,6 +9,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import _hostshim as hs
 import oracle as orc
 from _syncbb_oracle import SyncbbOracle
 from conftest import GOLDEN_DIR, ROOT
@@ -17,21 +18,12 @@ from pydcop_b200.engine import fill_desc, host_state, syncbb_plan
 from pydcop_b200.layout import layout_from_instance
 from test_syncbb_cpu import INTEGER, RUNNABLE
 
-SHIM_SRC = os.path.join(ROOT, "tests", "hostshim", "syncbb_host.cpp")
-SHIM_SO = os.path.join(ROOT, "tests", "hostshim", "_build", "syncbb_host.so")
 P = C.c_void_p
 
 
 @pytest.fixture(scope="module")
 def shim():
-    deps = [SHIM_SRC, os.path.join(ROOT, "include", "pydcop_b200.h"),
-            os.path.join(ROOT, "pydcop_b200", "csrc", "syncbb_kernels.cuh")]
-    if not os.path.exists(SHIM_SO) or any(os.path.getmtime(d) > os.path.getmtime(SHIM_SO) for d in deps):
-        os.makedirs(os.path.dirname(SHIM_SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O1", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-o", SHIM_SO,
-                        SHIM_SRC], check=True, capture_output=True)
-    lib = C.CDLL(SHIM_SO)
+    lib = hs.build("syncbb_host")
     lib.syncbb_host_step.argtypes = [P, C.c_int64]
     lib.syncbb_host_init.argtypes = [P]
     return lib
