@@ -909,6 +909,55 @@ int fg_solution_cost_segmented(int32_t precision, int32_t n_classes, const fg_cl
                                const int32_t *dev_var_seg, int32_t n_seg, double infinity, double *dev_out,
                                void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Cost trace (pydcop solve --collect_on cycle_change, orchestrator.py:802-884): with a trace attached to an
+ * iterative family's handle, its fg_<family>_step enqueues, after every committed cycle and on the step's stream,
+ * one record of fg_solution_cost(_segmented)'s sums over the family's current values: record k (k = 0, 1, ...)
+ * adds into row k, dev_rows[(k * n_seg + s) * 2] = cost and [... + 1] = violations of segment s, and stamps
+ * dev_stamp[k + 1] with the device's global timer (ns) when the whole row is summed.  A record is ONE launch over a
+ * block map built at create (the factor ranges of every non-ghost class, then the variables); it never
+ * synchronises.  Once `capacity` rows are recorded no more are: the caller attaches a fresh trace to go on.
+ * Records count in neither the family's launch count nor its cycles.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t abi_version, precision;
+  int32_t n_vars, n_classes;
+  const fg_class_t *classes;      /* HOST [n_classes], copied by fg_trace_create */
+  const void *dev_tables;         /* T[...] the family's tables */
+  const int32_t *dev_edge_var;    /* [n_edges] */
+  const void *dev_unary;          /* T[...] the variables' OWN costs, internal order (MaxSum: without noise); NULL:
+                                     variable costs are not added */
+  const int64_t *dev_unary_off;   /* [n_vars+1] */
+  const int32_t *dev_factor_seg;  /* [n_factors] optional, as fg_solution_cost_segmented; NULL (both): one segment */
+  const int32_t *dev_var_seg;     /* [n_vars] */
+  int32_t n_seg, reserved0;
+  double infinity;                /* an entry equal to it counts as a violation */
+  double *dev_rows;               /* [capacity * n_seg * 2] */
+  int64_t *dev_stamp;             /* [capacity + 1] stamp 0 written by fg_trace_start */
+  int64_t capacity;               /* rows */
+} fg_trace_desc_t;
+
+typedef struct fg_trace *fg_trace_t;
+
+int fg_trace_create(const fg_trace_desc_t *desc, fg_trace_t *out);
+/* a trace still attached to a handle must be detached first */
+int fg_trace_destroy(fg_trace_t tr);
+const char *fg_trace_last_error(fg_trace_t tr);
+/* zeroes every row, writes stamp 0 and the row count back to 0, on `stream` */
+int fg_trace_start(fg_trace_t tr, void *stream);
+/* rows enqueued since fg_trace_start (a host count: no synchronisation) */
+int fg_trace_rows(fg_trace_t tr, int64_t *n_rows);
+/* Attach `tr` (NULL: detach) to a handle of the same device, precision and variable count.  Records the values of
+ * MaxSum's dev_value, DSA's dev_value[cur], MGM's and MGM-2's dev_value, and GDBA's, DBA's and MixedDSA's
+ * dev_value[cycle % 2]; the sharded step loops record nothing. */
+int fg_maxsum_set_trace(fg_maxsum_t h, fg_trace_t tr);
+int fg_dsa_set_trace(fg_dsa_t h, fg_trace_t tr);
+int fg_mgm_set_trace(fg_mgm_t h, fg_trace_t tr);
+int fg_mgm2_set_trace(fg_mgm2_t h, fg_trace_t tr);
+int fg_gdba_set_trace(fg_gdba_t h, fg_trace_t tr);
+int fg_dba_set_trace(fg_dba_t h, fg_trace_t tr);
+int fg_mixeddsa_set_trace(fg_mixeddsa_t h, fg_trace_t tr);
+
 /* Row permutation on the device (engine creation): dev_dst[i * row_elems + k] = dev_src[dev_rows[i] * row_elems + k]
  * for i < n_rows, k < row_elems, elements of the given precision.  MaxSumEngine packs a one-class layout's tables with it
  * when the factor order permutes them (layout.FactorGraphLayout.table_rows): the caller's array is uploaded as it is and

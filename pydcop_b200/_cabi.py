@@ -208,6 +208,14 @@ class FgHaloPlan(C.Structure):
                 ("dev_edge_dst_r", P * 2), ("dev_slot_dst_q", P * 2)]
 
 
+class FgTraceDesc(C.Structure):
+    _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32), ("n_vars", C.c_int32), ("n_classes", C.c_int32),
+                ("classes", C.POINTER(FgClass)), ("dev_tables", P), ("dev_edge_var", P), ("dev_unary", P),
+                ("dev_unary_off", P), ("dev_factor_seg", P), ("dev_var_seg", P),
+                ("n_seg", C.c_int32), ("reserved0", C.c_int32), ("infinity", C.c_double),
+                ("dev_rows", P), ("dev_stamp", P), ("capacity", C.c_int64)]
+
+
 FG_MGM2_EXCHANGES = 5
 
 
@@ -329,6 +337,18 @@ SYMBOLS = {
     "fg_solution_cost_segmented": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(FgClass), P, P, P, P, P,
                                              C.c_int32, P, P, P, P, C.c_int32, C.c_double, P, P]),
     "fg_gather_rows": (C.c_int, [C.c_int32, P, P, P, C.c_int64, C.c_int64, P]),
+    "fg_trace_create": (C.c_int, [C.POINTER(FgTraceDesc), C.POINTER(P)]),
+    "fg_trace_destroy": (C.c_int, [P]),
+    "fg_trace_last_error": (C.c_char_p, [P]),
+    "fg_trace_start": (C.c_int, [P, P]),
+    "fg_trace_rows": (C.c_int, [P, C.POINTER(C.c_int64)]),
+    "fg_maxsum_set_trace": (C.c_int, [P, P]),
+    "fg_dsa_set_trace": (C.c_int, [P, P]),
+    "fg_mgm_set_trace": (C.c_int, [P, P]),
+    "fg_mgm2_set_trace": (C.c_int, [P, P]),
+    "fg_gdba_set_trace": (C.c_int, [P, P]),
+    "fg_dba_set_trace": (C.c_int, [P, P]),
+    "fg_mixeddsa_set_trace": (C.c_int, [P, P]),
 }
 
 _lib = None

@@ -96,7 +96,7 @@ static int dba_round(fg_dba *h, cudaStream_t st) {
   if (h->d.n_vars) dba_cycle(h->d, h->dev_classes, h->eval_dmax, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
-  return FG_OK;
+  return fg_trace_cycle(h, h->d.dev_value[h->cycle % 2], st);
 }
 
 extern "C" int fg_dba_step(fg_dba_t h, int32_t n_cycles, void *stream) {
@@ -134,3 +134,5 @@ extern "C" int fg_dba_current(fg_dba_t h, int64_t *cycle, int32_t *finished) {
 }
 
 extern "C" int64_t fg_dba_launch_count(fg_dba_t h) { return fg_launch_count(h); }
+
+extern "C" int fg_dba_set_trace(fg_dba_t h, fg_trace_t tr) { return fg_set_trace(h, tr); }

@@ -4,6 +4,7 @@
 #include <type_traits>
 
 #include "handle.cuh"
+#include "cost.cuh"
 #include "dsa_generic.cuh"
 #include "maxsum_generic.cuh"
 #include "maxsum_fast.cuh"
@@ -348,6 +349,7 @@ extern "C" int fg_maxsum_step(fg_maxsum_t h, int32_t n_cycles, void *stream) {
     int rc = fg_maxsum_cycle_compute(h, stream);
     if (rc != FG_OK) return rc;
     fg_maxsum_cycle_commit(h);
+    if ((rc = fg_trace_cycle(h, h->d.dev_value, (cudaStream_t)stream)) != FG_OK) return rc;
   }
   return FG_OK;
 }
@@ -780,6 +782,7 @@ extern "C" int fg_dsa_step(fg_dsa_t h, int32_t n_cycles, void *stream) {
     int rc = fg_dsa_cycle_compute(h, stream);
     if (rc != FG_OK) return rc;
     fg_dsa_cycle_commit(h);
+    if ((rc = fg_trace_cycle(h, h->d.dev_value[h->cur], (cudaStream_t)stream)) != FG_OK) return rc;
   }
   return FG_OK;
 }
@@ -864,20 +867,9 @@ template <typename T>
 __global__ void k_cost_factors(const fg_class_t c, const T *__restrict__ tables, const int32_t *__restrict__ edge_var,
                                const int32_t *__restrict__ value, const uint8_t *__restrict__ skip, T infinity,
                                const int32_t *__restrict__ seg, int32_t n_seg, double *__restrict__ out) {
-  int f = blockIdx.x * blockDim.x + threadIdx.x;
   double cst = 0.0, viol = 0.0;
-  int s = -1;
-  if (f < c.n_factors) {
-    s = seg ? seg[c.first_factor + f] : 0;
-    if (s >= n_seg) s = -1;
-  }
-  if (s >= 0 && !(skip && skip[c.first_factor + f])) {
-    int64_t idx = 0, stride = 1;
-    const int e0 = c.first_edge + f * c.arity;
-    for (int i = c.arity - 1; i >= 0; --i) { idx += (int64_t)value[edge_var[e0 + i]] * stride; stride *= c.dom[i]; }
-    const T t = tables[c.table_base + (int64_t)f * c.table_size + idx];
-    if (t != infinity) cst = (double)t; else viol = 1.0;   // `r_cost != infinity`, dcop.py:355
-  }
+  const int s = cost_factor_lane<T>(c, blockIdx.x * blockDim.x + threadIdx.x, tables, edge_var, value, skip, infinity,
+                                    seg, n_seg, cst, viol);
   cost_warp_add(cst, viol, s, seg != nullptr, out);
 }
 
@@ -885,17 +877,9 @@ template <typename T>
 __global__ void k_cost_unary(const T *__restrict__ unary, const int64_t *__restrict__ unary_off,
                              const int32_t *__restrict__ value, int n_vars, const uint8_t *__restrict__ skip,
                              T infinity, const int32_t *__restrict__ seg, int32_t n_seg, double *__restrict__ out) {
-  int v = blockIdx.x * blockDim.x + threadIdx.x;
   double cst = 0.0, viol = 0.0;
-  int s = -1;
-  if (v < n_vars) {
-    s = seg ? seg[v] : 0;
-    if (s >= n_seg) s = -1;
-  }
-  if (s >= 0 && !(skip && skip[v])) {
-    const T t = unary[unary_off[v] + value[v]];
-    if (t != infinity) cst = (double)t; else viol = 1.0;   // `cost_for_val != infinity`, dcop.py:363
-  }
+  const int s = cost_var_lane<T>(blockIdx.x * blockDim.x + threadIdx.x, n_vars, unary, unary_off, value, skip, infinity,
+                                 seg, n_seg, cst, viol);
   cost_warp_add(cst, viol, s, seg != nullptr, out);
 }
 
@@ -941,6 +925,150 @@ extern "C" int fg_solution_cost_segmented(int32_t precision, int32_t n_classes, 
                               dev_unary_off, n_vars, dev_factor_skip, dev_var_skip, dev_factor_seg, dev_var_seg, n_seg,
                               infinity, dev_out, stream);
 }
+
+// ---------------------------------------------------------------------------------------------
+// cost trace: fg_solution_cost(_segmented)'s sums once per cycle, in ONE launch (a batch union has many classes, and
+// its cycles take a few tens of microseconds)
+// ---------------------------------------------------------------------------------------------
+constexpr int kTraceBlock = 128;
+
+struct fg_trace : fg_handle_base {
+  fg_trace_desc_t d;
+  int2 *dev_map = nullptr;       // per block: (class, first factor), or (-1, first variable)
+  unsigned *dev_ticket = nullptr;
+  unsigned n_blocks = 0;
+  int64_t rows = 0;              // records enqueued since fg_trace_start
+};
+
+// Every block covers kTraceBlock factors of one class or kTraceBlock variables (map[blockIdx.x]) and adds its warps'
+// runs into `row` as fg_solution_cost's kernels do; the last block to finish stamps the row and resets the ticket.
+template <typename T>
+__global__ void __launch_bounds__(kTraceBlock)
+k_trace_record(const fg_class_t *__restrict__ classes, const int2 *__restrict__ map, const T *__restrict__ tables,
+               const int32_t *__restrict__ edge_var, const int32_t *__restrict__ value, const T *__restrict__ unary,
+               const int64_t *__restrict__ unary_off, int n_vars, T infinity, const int32_t *__restrict__ factor_seg,
+               const int32_t *__restrict__ var_seg, int32_t n_seg, double *__restrict__ row,
+               int64_t *__restrict__ stamp, unsigned *__restrict__ ticket) {
+  const int2 b = map[blockIdx.x];
+  double cst = 0.0, viol = 0.0;
+  const int s = b.x >= 0 ? cost_factor_lane<T>(classes[b.x], b.y + (int)threadIdx.x, tables, edge_var, value, nullptr,
+                                               infinity, factor_seg, n_seg, cst, viol)
+                         : cost_var_lane<T>(b.y + (int)threadIdx.x, n_vars, unary, unary_off, value, nullptr, infinity,
+                                            var_seg, n_seg, cst, viol);
+  cost_warp_add(cst, viol, s, factor_seg != nullptr, row);
+  __threadfence();   // this thread's adds are visible before its block takes a ticket
+  __syncthreads();
+  if (threadIdx.x == 0 && atomicAdd(ticket, 1u) == gridDim.x - 1) {
+    __threadfence();
+    *stamp = (int64_t)global_timer_ns();
+    *ticket = 0;
+  }
+}
+
+__global__ void k_trace_stamp(int64_t *stamp) { *stamp = (int64_t)global_timer_ns(); }
+
+extern "C" int fg_trace_create(const fg_trace_desc_t *desc, fg_trace_t *out) {
+  if (desc && (desc->n_classes < 0 || (desc->n_classes > 0 && !desc->classes))) {
+    if (out) *out = nullptr;
+    return FG_ERR_ARG;
+  }
+  int rc = fg_open(desc, out);
+  if (rc != FG_OK) return rc;
+  fg_trace *h = *out;
+  const fg_trace_desc_t &d = *desc;
+  auto refuse = [&](const char *why) { snprintf(h->err, sizeof(h->err), "%s", why); return FG_ERR_ARG; };
+  if (d.n_vars < 0) return refuse("negative n_vars");
+  if (d.capacity < 1) return refuse("capacity must be at least one row");
+  if (d.n_seg < 1) return refuse("n_seg must be at least 1");
+  if (!d.dev_factor_seg != !d.dev_var_seg) return refuse("give both segment arrays or neither");
+  if (!d.dev_factor_seg && d.n_seg != 1) return refuse("n_seg > 1 needs the segment arrays");
+  if (d.capacity > (INT64_MAX / 16) / d.n_seg) return refuse("capacity * n_seg rows overflow");
+  if (!d.dev_rows || !d.dev_stamp) return refuse("missing dev_rows or dev_stamp");
+  if (d.dev_unary && !d.dev_unary_off) return refuse("dev_unary needs dev_unary_off");
+  std::vector<int2> map;
+  for (size_t i = 0; i < h->classes.size(); ++i) {
+    const fg_class_t &c = h->classes[i];
+    if (!c.n_factors || (c.flags & FG_CLASS_GHOST)) continue;   // as fg_solution_cost
+    if (!d.dev_tables || !d.dev_edge_var) return refuse("missing dev_tables or dev_edge_var");
+    for (int f = 0; f < c.n_factors; f += kTraceBlock) map.push_back(make_int2((int)i, f));
+  }
+  if (d.dev_unary)
+    for (int v = 0; v < d.n_vars; v += kTraceBlock) map.push_back(make_int2(-1, v));
+  if (map.empty()) map.push_back(make_int2(-1, d.n_vars));   // nothing to sum: one block still stamps the row
+  if (map.size() > (size_t)INT32_MAX) return refuse("block map exceeds the grid");
+  if ((rc = fg_require_device(h)) != FG_OK) return rc;
+  rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_edge_var), FG_FIELD(d, dev_unary),
+                             FG_FIELD(d, dev_unary_off), FG_FIELD(d, dev_factor_seg), FG_FIELD(d, dev_var_seg),
+                             FG_FIELD(d, dev_rows), FG_FIELD(d, dev_stamp)});
+  if (rc != FG_OK) return rc;
+  if ((rc = fg_upload_classes(h)) != FG_OK) return rc;
+  h->n_blocks = (unsigned)map.size();
+  CUDA_TRY(h, cudaMalloc(&h->dev_map, sizeof(int2) * map.size()));
+  CUDA_TRY(h, cudaMemcpy(h->dev_map, map.data(), sizeof(int2) * map.size(), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, cudaMalloc(&h->dev_ticket, sizeof(unsigned)));
+  CUDA_TRY(h, cudaMemset(h->dev_ticket, 0, sizeof(unsigned)));
+  return FG_OK;
+}
+
+extern "C" int fg_trace_destroy(fg_trace_t h) {
+  if (h) {
+    fg_device_scope on(h);
+    if (h->dev_map) cudaFree(h->dev_map);
+    if (h->dev_ticket) cudaFree(h->dev_ticket);
+  }
+  return fg_close(h);
+}
+
+extern "C" const char *fg_trace_last_error(fg_trace_t h) { return fg_last_error(h); }
+
+extern "C" int fg_trace_start(fg_trace_t h, void *stream) {
+  if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_TRY(h, cudaMemsetAsync(h->d.dev_rows, 0, sizeof(double) * 2 * (size_t)h->d.n_seg * (size_t)h->d.capacity, st));
+  CUDA_TRY(h, cudaMemsetAsync(h->dev_ticket, 0, sizeof(unsigned), st));
+  k_trace_stamp<<<1, 1, 0, st>>>(h->d.dev_stamp);
+  ++h->launches;
+  CUDA_TRY(h, cudaGetLastError());
+  h->rows = 0;
+  return FG_OK;
+}
+
+extern "C" int fg_trace_rows(fg_trace_t h, int64_t *n_rows) {
+  if (!h || !n_rows) return FG_ERR_ARG;
+  *n_rows = h->rows;
+  return FG_OK;
+}
+
+int fg_trace_check(const fg_trace *tr, int device, int32_t precision, int32_t n_vars, char *err, size_t n) {
+  if (tr->device != device) { snprintf(err, n, "the trace belongs to device %d, the handle to %d", tr->device, device); return FG_ERR_ARG; }
+  if (tr->d.precision != precision) { snprintf(err, n, "trace precision differs from the handle's"); return FG_ERR_ARG; }
+  if (tr->d.n_vars != n_vars) { snprintf(err, n, "trace over %d variables, the handle has %d", tr->d.n_vars, n_vars); return FG_ERR_ARG; }
+  return FG_OK;
+}
+
+template <typename T>
+static void trace_record_t(fg_trace *h, const int32_t *value, cudaStream_t st) {
+  const fg_trace_desc_t &d = h->d;
+  k_trace_record<T><<<h->n_blocks, kTraceBlock, 0, st>>>(
+      h->dev_classes, h->dev_map, (const T *)d.dev_tables, d.dev_edge_var, value, (const T *)d.dev_unary,
+      d.dev_unary_off, d.n_vars, (T)d.infinity, d.dev_factor_seg, d.dev_var_seg, d.n_seg,
+      d.dev_rows + 2 * (int64_t)d.n_seg * h->rows, d.dev_stamp + h->rows + 1, h->dev_ticket);
+}
+
+// runs on the trace's device, which fg_trace_check made sure is the calling handle's
+int fg_trace_record(fg_trace *h, const int32_t *value, cudaStream_t st) {
+  if (h->rows >= h->d.capacity) return FG_OK;   // full: the caller attaches a fresh trace
+  if (h->d.precision == FG_F64) trace_record_t<double>(h, value, st);
+  else trace_record_t<float>(h, value, st);
+  CUDA_TRY(h, cudaGetLastError());
+  ++h->rows;
+  ++h->launches;
+  return FG_OK;
+}
+
+extern "C" int fg_maxsum_set_trace(fg_maxsum_t h, fg_trace_t tr) { return fg_set_trace(h, tr); }
+extern "C" int fg_dsa_set_trace(fg_dsa_t h, fg_trace_t tr) { return fg_set_trace(h, tr); }
 
 // one 16-, 8- or 4-byte word per thread and step: rows of C2's f32 tables (400 bytes) move as 25 16-byte words
 template <typename W>

@@ -84,7 +84,7 @@ static int gdba_cycle_t(fg_gdba *h, cudaStream_t st) {
   if (h->d.n_vars) gdba_cycle<T>(h->d, h->dev_classes, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
-  return FG_OK;
+  return fg_trace_cycle(h, h->d.dev_value[h->cycle % 2], st);
 }
 
 extern "C" int fg_gdba_step(fg_gdba_t h, int32_t n_cycles, void *stream) {
@@ -94,3 +94,5 @@ extern "C" int fg_gdba_step(fg_gdba_t h, int32_t n_cycles, void *stream) {
 extern "C" int fg_gdba_current(fg_gdba_t h, int64_t *cycle, int32_t *finished) { return fg_current(h, cycle, finished); }
 
 extern "C" int64_t fg_gdba_launch_count(fg_gdba_t h) { return fg_launch_count(h); }
+
+extern "C" int fg_gdba_set_trace(fg_gdba_t h, fg_trace_t tr) { return fg_set_trace(h, tr); }

@@ -11,14 +11,22 @@
 
 #include "common.cuh"
 
+struct fg_trace;
+
 struct fg_handle_base {
   std::vector<fg_class_t> classes;      // the descriptor's class table, copied (d.classes points here)
   fg_class_t *dev_classes = nullptr;    // its device copy (fg_upload_classes)
   int device = -1;                      // the device current at create (fg_require_device); -1 before
   int64_t cycle = 0;
   int64_t launches = 0;
+  fg_trace *trace = nullptr;            // fg_<family>_set_trace: a record after every cycle of the step loop
   mutable char err[512] = {0};        // written by const readers too (fg_device_scope)
 };
+
+// engine.cu: the checks of fg_<family>_set_trace (FG_ERR_ARG, the reason in err) and one record of `value` on the
+// stream, counted by the trace alone
+int fg_trace_check(const fg_trace *tr, int device, int32_t precision, int32_t n_vars, char *err, size_t n);
+int fg_trace_record(fg_trace *tr, const int32_t *value, cudaStream_t st);
 
 // Runs the rest of an entry point on the handle's device and gives the caller's device back on exit, so a handle
 // works whichever device the calling thread has current.  No-op for a null handle or one without a device yet.
@@ -205,6 +213,24 @@ struct fg_launcher {
 static inline const char *fg_last_error(const fg_handle_base *h) { return h ? h->err : "invalid handle"; }
 
 static inline int64_t fg_launch_count(const fg_handle_base *h) { return h ? h->launches : -1; }
+
+template <class H>
+static inline int fg_set_trace(H *h, fg_trace *tr) {
+  if (!h) return FG_ERR_ARG;
+  FG_ON_DEVICE(h);
+  if (tr && fg_trace_check(tr, h->device, h->d.precision, h->d.n_vars, h->err, sizeof(h->err)) != FG_OK)
+    return FG_ERR_ARG;
+  h->trace = tr;
+  return FG_OK;
+}
+
+// the record of a committed cycle whose values are `value`, when a trace is attached
+static inline int fg_trace_cycle(fg_handle_base *h, const int32_t *value, cudaStream_t st) {
+  if (!h->trace) return FG_OK;
+  int rc = fg_trace_record(h->trace, value, st);
+  if (rc != FG_OK) snprintf(h->err, sizeof(h->err), "trace record: %s", fg_trace_last_error(h->trace));
+  return rc;
+}
 
 // MGM, MGM-2 and GDBA: rounds stop once cycle + 1 >= stop_cycle (0 = never)
 template <class H>

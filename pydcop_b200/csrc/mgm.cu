@@ -93,7 +93,7 @@ static int mgm_cycle_t(fg_mgm *h, cudaStream_t st) {
   }
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
-  return FG_OK;
+  return fg_trace_cycle(h, d.dev_value, st);
 }
 
 extern "C" int fg_mgm_step(fg_mgm_t h, int32_t n_cycles, void *stream) {
@@ -103,3 +103,5 @@ extern "C" int fg_mgm_step(fg_mgm_t h, int32_t n_cycles, void *stream) {
 extern "C" int fg_mgm_current(fg_mgm_t h, int64_t *cycle, int32_t *finished) { return fg_current(h, cycle, finished); }
 
 extern "C" int64_t fg_mgm_launch_count(fg_mgm_t h) { return fg_launch_count(h); }
+
+extern "C" int fg_mgm_set_trace(fg_mgm_t h, fg_trace_t tr) { return fg_set_trace(h, tr); }

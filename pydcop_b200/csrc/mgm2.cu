@@ -94,7 +94,7 @@ static int mgm2_cycle_t(fg_mgm2 *h, cudaStream_t st) {
   if (h->d.n_vars) mgm2_cycle<T>(h->d, h->dev_classes, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
-  return FG_OK;
+  return fg_trace_cycle(h, h->d.dev_value, st);
 }
 
 extern "C" int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream) {
@@ -104,6 +104,8 @@ extern "C" int fg_mgm2_step(fg_mgm2_t h, int32_t n_cycles, void *stream) {
 extern "C" int fg_mgm2_current(fg_mgm2_t h, int64_t *cycle, int32_t *finished) { return fg_current(h, cycle, finished); }
 
 extern "C" int64_t fg_mgm2_launch_count(fg_mgm2_t h) { return fg_launch_count(h); }
+
+extern "C" int fg_mgm2_set_trace(fg_mgm2_t h, fg_trace_t tr) { return fg_set_trace(h, tr); }
 
 // ---------------------------------------------------------------------------------------------
 // Sharded MGM-2 (include/pydcop_b200.h: fg_mgm2_shard_*; kernels in csrc/mgm2_shard_kernels.cuh)

@@ -86,7 +86,7 @@ static int mixeddsa_round_t(fg_mixeddsa *h, cudaStream_t st) {
   if (h->d.n_vars) mixeddsa_cycle<T>(h->d, h->dev_classes, h->dmax, h->cycle, launch);
   CUDA_TRY(h, cudaGetLastError());
   ++h->cycle;
-  return FG_OK;
+  return fg_trace_cycle(h, h->d.dev_value[h->cycle % 2], st);
 }
 
 extern "C" int fg_mixeddsa_step(fg_mixeddsa_t h, int32_t n_cycles, void *stream) {
@@ -110,3 +110,5 @@ extern "C" int fg_mixeddsa_current(fg_mixeddsa_t h, int64_t *cycle, int32_t *fin
 }
 
 extern "C" int64_t fg_mixeddsa_launch_count(fg_mixeddsa_t h) { return fg_launch_count(h); }
+
+extern "C" int fg_mixeddsa_set_trace(fg_mixeddsa_t h, fg_trace_t tr) { return fg_set_trace(h, tr); }

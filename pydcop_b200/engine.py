@@ -152,7 +152,10 @@ class _EngineBase:
         if getattr(self, "_h", None) and self._h.value:
             with torch.cuda.device(self.device):   # __del__ may run with any device current
                 self._fn("destroy")(self._h)
+                if getattr(self, "_trace", None) is not None and self._trace["h"] is not None:
+                    self.lib.fg_trace_destroy(self._trace["h"])
             self._h = C.c_void_p()
+            self._trace = None
 
     def __del__(self):
         try:
@@ -166,8 +169,21 @@ class _EngineBase:
         return self
 
     def step(self, n_cycles=1):
+        """n_cycles cycles of fg_<FAMILY>_step.  With a trace started, a full trace block is moved aside and the trace
+        restarted whenever more cycles follow, so every cycle is recorded."""
+        n = int(n_cycles)
         with torch.cuda.device(self.device):
-            self._check(self._fn("step")(self._h, int(n_cycles), self._stream()), f"fg_{self.FAMILY}_step")
+            while True:
+                k = n
+                tr = getattr(self, "_trace", None)
+                if tr is not None and tr["h"] is not None:
+                    if self._trace_rows() >= tr["capacity"] and n > 0:
+                        self._trace_rotate()
+                    k = min(n, tr["capacity"] - self._trace_rows())
+                self._check(self._fn("step")(self._h, k, self._stream()), f"fg_{self.FAMILY}_step")
+                n -= k
+                if n <= 0:
+                    break
         return self
 
     @property
@@ -186,14 +202,99 @@ class _EngineBase:
         """(cost float64[n_seg], violations int64[n_seg]) of the current assignment per segment, reduced on the device
         (fg_solution_cost_segmented): what solution_cost computes over the factors and variables of each segment.
         seg_factor / seg_var: the segment (problem of a batch) of every factor and variable, canonical order."""
+        with torch.cuda.device(self.device):
+            seg = self._segments(seg_factor, seg_var, n_seg)
+            out = self._solution_cost(self._assignment(), infinity, unary, seg=seg).cpu().numpy().reshape(-1, 2)
+        return out[:, 0].copy(), out[:, 1].astype(np.int64)
+
+    def _segments(self, seg_factor, seg_var, n_seg):
+        """(factor segment, variable segment, n_seg) on the device in internal order, from canonical seg_factor /
+        seg_var."""
         L = self.layout
         f_int = np.zeros(max(L.n_factors, 1), dtype=np.int32)
         f_int[L.factor_perm] = np.asarray(seg_factor, dtype=np.int32)
         v_int = _per_var(L, np.asarray(seg_var, dtype=np.int32)[L.var_order], np.int32)
+        return self._dev(f_int, torch.int32), self._dev(v_int, torch.int32), int(n_seg)
+
+    def start_trace(self, capacity, infinity=float("inf"), unary=None, seg=None):
+        """Record (cost, violations) of the current values after every cycle step() runs from now on, on the device
+        and without synchronising (fg_trace_*): solution_cost's sums, or with seg = (seg_factor, seg_var, n_seg) as
+        in solution_costs_segmented, solution_costs_segmented's.  `capacity`: rows per trace block; a full block is
+        moved aside on the device and the trace goes on, so any number of cycles is recorded."""
+        self.stop_trace()
+        L = self.layout
         with torch.cuda.device(self.device):
-            seg = (self._dev(f_int, torch.int32), self._dev(v_int, torch.int32), int(n_seg))
-            out = self._solution_cost(self._assignment(), infinity, unary, seg=seg).cpu().numpy().reshape(-1, 2)
-        return out[:, 0].copy(), out[:, 1].astype(np.int64)
+            self._cost_inputs()
+            segd = None if seg is None else self._segments(*seg)
+            n_seg = 1 if seg is None else segd[2]
+            capacity = max(1, int(capacity))
+            rows = torch.zeros(capacity * n_seg * 2, dtype=torch.float64, device=self.device)
+            stamp = torch.zeros(capacity + 1, dtype=torch.int64, device=self.device)
+            un = self._unary_dev(unary)
+            d = _cabi.FgTraceDesc()
+            d.abi_version, d.precision = _cabi.FG_ABI_VERSION, PRECISIONS[self.precision][0]
+            d.n_vars, d.n_classes = L.n_vars, len(L.classes)
+            d.classes = C.cast(self._classes, C.POINTER(FgClass))
+            fill_desc(d, {"tables": self.tables, "edge_var": self._edge_var_dev, "unary": un,
+                          "unary_off": self._cost_unary_off, "factor_seg": None if segd is None else segd[0],
+                          "var_seg": None if segd is None else segd[1], "rows": rows, "stamp": stamp},
+                      {"n_seg": n_seg, "infinity": float(infinity), "capacity": capacity})
+            h = C.c_void_p()
+            rc = self.lib.fg_trace_create(C.byref(d), C.byref(h))
+            if rc != _cabi.FG_OK:
+                msg = (self.lib.fg_trace_last_error(h) or b"").decode()
+                self.lib.fg_trace_destroy(h)
+                raise EngineError(f"fg_trace_create failed (rc={rc}): {msg}")
+            self._trace = {"h": h, "capacity": capacity, "n_seg": n_seg, "rows": rows, "stamp": stamp,
+                           "keep": (un, segd), "done": []}
+            self._trace_check(self.lib.fg_trace_start(h, self._stream()), "fg_trace_start")
+            self._check(self._fn("set_trace")(self._h, h), f"fg_{self.FAMILY}_set_trace")
+        return self
+
+    def _trace_check(self, rc, what):
+        if rc != _cabi.FG_OK:
+            raise EngineError(f"{what} failed (rc={rc}): "
+                              f"{(self.lib.fg_trace_last_error(self._trace['h']) or b'').decode()}")
+
+    def _trace_rows(self):
+        if self._trace["h"] is None:   # stopped
+            return self._trace["stopped_rows"]
+        n = C.c_int64()
+        self.lib.fg_trace_rows(self._trace["h"], C.byref(n))
+        return n.value
+
+    def _trace_rotate(self):
+        """A full block: its rows and stamps copied aside on the stream, the trace restarted behind them."""
+        tr = self._trace
+        tr["done"].append((tr["rows"].clone(), tr["stamp"].clone(), self._trace_rows()))
+        self._trace_check(self.lib.fg_trace_start(tr["h"], self._stream()), "fg_trace_start")
+
+    def trace(self):
+        """The cycles recorded since start_trace: cost float64[rows, n_seg], violation int64[rows, n_seg] and time
+        float64[rows], seconds on the device's global timer from start_trace to the end of each row's record.
+        Synchronises (it is the only call of a trace that does)."""
+        tr = self._trace
+        if tr is None:
+            raise EngineError("no trace started")
+        with torch.cuda.device(self.device):
+            blocks = tr["done"] + [(tr["rows"], tr["stamp"], self._trace_rows())]
+            t0 = int(blocks[0][1][0].item())
+            rows = [r.view(-1, tr["n_seg"], 2)[:n].cpu().numpy() for r, _, n in blocks]
+            stamps = [s[1:n + 1].cpu().numpy() for _, s, n in blocks]
+        out = np.concatenate(rows) if rows else np.zeros((0, tr["n_seg"], 2))
+        return {"cost": out[:, :, 0].copy(), "violation": out[:, :, 1].astype(np.int64),
+                "time": (np.concatenate(stamps).astype(np.int64) - t0) * 1e-9}
+
+    def stop_trace(self):
+        """Detach the trace: the step loop is the plain one again.  trace() still reads what was recorded."""
+        tr = getattr(self, "_trace", None)
+        if tr is None or tr["h"] is None:
+            return
+        with torch.cuda.device(self.device):
+            self._check(self._fn("set_trace")(self._h, None), f"fg_{self.FAMILY}_set_trace")
+            tr["stopped_rows"] = self._trace_rows()
+            self.lib.fg_trace_destroy(tr["h"])
+        tr["h"] = None
 
     def _dev(self, a, dtype):
         a = np.ascontiguousarray(a)
@@ -236,24 +337,10 @@ class _EngineBase:
         (cost, violations) pairs (fg_solution_cost_segmented)."""
         L = self.layout
         prec = PRECISIONS[self.precision][0]
-        tdt = PRECISIONS[self.precision][1]
         with torch.cuda.device(self.device):
-            if not hasattr(self, "_cost_out"):
-                self._edge_var_dev = self._dev(L.edge_var, torch.int32)
-                self._cost_out = torch.zeros(2, dtype=torch.float64, device=self.device)
-                self._cost_unary_off = self._dev(L.unary_off, torch.int64)
+            self._cost_inputs()
             out = self._cost_out if seg is None else torch.zeros(2 * seg[2], dtype=torch.float64, device=self.device)
-            un = None
-            if unary is not None:   # canonical (variable-major) -> internal (class-major, padded bases)
-                un_host = np.zeros(max(int(L.unary_off[-1]), 1))
-                cu = np.asarray(unary, dtype=np.float64).reshape(-1)
-                dom = L.dom_size.astype(np.int64)
-                c_off = np.concatenate([[0], np.cumsum(dom[L.var_perm])])[:-1]   # canonical offsets
-                if len(cu):
-                    src = np.repeat(c_off[L.var_order], dom) + (np.arange(int(dom.sum())) - np.repeat(np.cumsum(dom) - dom, dom))
-                    dst = np.repeat(L.unary_off[:-1], dom) + (np.arange(int(dom.sum())) - np.repeat(np.cumsum(dom) - dom, dom))
-                    un_host[dst] = cu[src]
-                un = self._dev(un_host, tdt)
+            un = self._unary_dev(unary)
             args = (prec, len(L.classes), C.cast(self._classes, C.POINTER(FgClass)), _ptr(self.tables),
                     _ptr(self._edge_var_dev), _ptr(value_tensor), _ptr(un), _ptr(self._cost_unary_off),
                     int(L.n_vars if n_vars is None else n_vars), _ptr(factor_skip), _ptr(var_skip))
@@ -264,6 +351,31 @@ class _EngineBase:
                                                          _ptr(out), self._stream())
             self._check(rc, "fg_solution_cost" if seg is None else "fg_solution_cost_segmented")
             return out
+
+
+    def _cost_inputs(self):
+        """The device arrays of the cost reductions the engine's descriptor does not hold, made once."""
+        if not hasattr(self, "_cost_out"):
+            L = self.layout
+            self._edge_var_dev = self._dev(L.edge_var, torch.int32)
+            self._cost_out = torch.zeros(2, dtype=torch.float64, device=self.device)
+            self._cost_unary_off = self._dev(L.unary_off, torch.int64)
+
+    def _unary_dev(self, unary):
+        """The variables' own costs `unary` (canonical order) on the device in internal order (class-major, padded
+        bases), in the engine's precision; None for None."""
+        if unary is None:
+            return None
+        L = self.layout
+        un_host = np.zeros(max(int(L.unary_off[-1]), 1))
+        cu = np.asarray(unary, dtype=np.float64).reshape(-1)
+        dom = L.dom_size.astype(np.int64)
+        c_off = np.concatenate([[0], np.cumsum(dom[L.var_perm])])[:-1]   # canonical offsets
+        if len(cu):
+            src = np.repeat(c_off[L.var_order], dom) + (np.arange(int(dom.sum())) - np.repeat(np.cumsum(dom) - dom, dom))
+            dst = np.repeat(L.unary_off[:-1], dom) + (np.arange(int(dom.sum())) - np.repeat(np.cumsum(dom) - dom, dom))
+            un_host[dst] = cu[src]
+        return self._dev(un_host, PRECISIONS[self.precision][1])
 
 
 class _CycleEngine(_EngineBase):

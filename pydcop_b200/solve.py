@@ -225,7 +225,8 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
           seed: Optional[int] = None, infinity: float = float("inf"), chunk: int = 50,
           on_cycle: Optional[Callable[[int, np.ndarray], None]] = None,
           engine_factory: Optional[Callable] = None, distributed: Optional[bool] = None,
-          partition="auto", halo: str = "auto", sharded_kwargs: Optional[Dict[str, Any]] = None) -> Dict[str, Any]:
+          partition="auto", halo: str = "auto", sharded_kwargs: Optional[Dict[str, Any]] = None,
+          trace: bool = False) -> Dict[str, Any]:
     """Run `algo` on `problem` and return pyDcop's result dict.
 
     Under `torchrun` (torch.distributed initialised, world size > 1; `distributed` None = detect)
@@ -244,12 +245,19 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     precision    f32 | f64 (f64 reproduces the reference's double arithmetic bit for bit)
     seed         MaxSum: the U(0, noise) draws; DSA: the Philox stream of the random choices
     on_cycle     callback(cycle, value_index) after every chunk (metrics collection)
+    trace        the result gains "trace": {"cycle", "time", "cost", "violation"}, one entry per cycle the engine ran
+                 (pydcop solve --collect_on cycle_change): each cycle's solution cost recorded on the device inside
+                 the step loop, without a host round trip; "time" is seconds on the device timer since the first
+                 cycle was enqueued.  The last entry's cost and violation are the result's.  Single-GPU iterative
+                 algorithms only (not dpop, syncbb or torchrun).
     SyncBB has no cycles to chunk: it ignores `chunk` and never calls `on_cycle` (a variable may have no value
     until the search ends).
     """
     kind, params, stop_cycle = _algorithm(algo, algo_params, timeout)
     if distributed is None:
         distributed = _under_torchrun()
+    if trace:
+        _check_trace(kind, distributed)
     if distributed and seed is None:
         seed = 0
     t0 = time.perf_counter()
@@ -285,7 +293,10 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     deadline = None if timeout is None else t0 + float(timeout)
     if kind == "syncbb":
         return _finish_syncbb(engine, dcop, deadline, infinity, precision, t0, t_packed)
-    cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline, distributed, on_cycle, kind == "dba")
+    tracer = _Trace(engine, stop_cycle, infinity, dcop.arrays["unary"], None,
+                    lambda idx: [solution_cost(dcop, idx, infinity)]) if trace else None
+    cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline, distributed, on_cycle, kind == "dba",
+                                tracer.after_cycle if tracer else None)
     if kind == "dba":                      # the rounds that changed the state
         cycle = engine.cycle
     idx = _indices(engine)
@@ -293,14 +304,17 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
         cost, violation = engine.solution_cost(infinity, dcop.arrays["unary"])
     else:                                  # engine seam of the CPU tests
         violation, cost = solution_cost(dcop, idx, infinity)
-    return {"status": status, "assignment": dcop.assignment(idx), "cost": cost,
-            "violation": violation, "time": time.perf_counter() - t0, "cycle": 0 if kind == "dpop" else cycle,
-            "msg_count": 0, "msg_size": 0,  # nothing crosses an agent boundary
-            "algo": kind, "precision": precision, "n_gpus": n_gpus,
-            "ingest_time": t_packed - t0,
-            # bytes this process moved host -> device (problem arrays) and device -> host (assignment, costs)
-            "h2d_bytes": int(getattr(getattr(engine, "engine", engine), "h2d_bytes", 0)),
-            "d2h_bytes": int(len(idx) * 12 + 16)}
+    out = {"status": status, "assignment": dcop.assignment(idx), "cost": cost,
+           "violation": violation, "time": time.perf_counter() - t0, "cycle": 0 if kind == "dpop" else cycle,
+           "msg_count": 0, "msg_size": 0,  # nothing crosses an agent boundary
+           "algo": kind, "precision": precision, "n_gpus": n_gpus,
+           "ingest_time": t_packed - t0,
+           # bytes this process moved host -> device (problem arrays) and device -> host (assignment, costs)
+           "h2d_bytes": int(getattr(getattr(engine, "engine", engine), "h2d_bytes", 0)),
+           "d2h_bytes": int(len(idx) * 12 + 16)}
+    if tracer is not None:
+        out["trace"] = tracer.result(cycle if kind == "dba" else None)[0]
+    return out
 
 
 def _algorithm(algo, algo_params, timeout):
@@ -323,10 +337,12 @@ def _under_torchrun():
         return False
 
 
-def _run_cycles(engine, stop_cycle, chunk, deadline, distributed=False, on_cycle=None, stops_itself=False):
+def _run_cycles(engine, stop_cycle, chunk, deadline, distributed=False, on_cycle=None, stops_itself=False,
+                after_cycle=None):
     """Step an initialised engine `chunk` cycles at a time until stop_cycle (0: none) or the deadline (checked before
     every chunk; under torchrun every rank leaves in the same round), or, with `stops_itself`, until engine.finished.
-    Returns (cycles run, FINISHED | TIMEOUT)."""
+    `after_cycle`: called after every single step(1) of a chunk stepped one cycle at a time (the host trace of the
+    engine seam).  Returns (cycles run, FINISHED | TIMEOUT)."""
     cycle, status = 0, "FINISHED"
     while True:
         n = chunk if not stop_cycle else min(chunk, stop_cycle - cycle)
@@ -342,13 +358,69 @@ def _run_cycles(engine, stop_cycle, chunk, deadline, distributed=False, on_cycle
         if expired:
             status = "TIMEOUT"
             break
-        engine.step(n)
+        if after_cycle is None:
+            engine.step(n)
+        else:
+            for _ in range(n):
+                engine.step(1)
+                after_cycle()
         cycle += n
         if on_cycle is not None:
             on_cycle(cycle, _indices(engine))
         if stops_itself and engine.finished:   # DBA: every variable with neighbours finished, or stop_cycle
             break
     return cycle, status
+
+
+TRACE_BYTES = 64 << 20   # device rows of one trace block, at most: a block of n_seg problems holds fewer cycles
+
+
+def _check_trace(kind, distributed):
+    if kind in ("dpop", "syncbb"):
+        raise ValueError(f"trace: {kind} has no cycles to trace")
+    if distributed:
+        raise ValueError("trace: traces are recorded on one GPU: start the run without torchrun")
+
+
+class _Trace:
+    """The cost of every cycle of one engine run: recorded on the device (engine.start_trace), or for an engine
+    without one (the CPU tests' engine seam) on the host after every single cycle: host_costs(value_index) ->
+    [(violation, cost)] per segment, with solution_cost."""
+
+    def __init__(self, engine, stop_cycle, infinity, unary, seg, host_costs):
+        self.engine, self.rows, self.t0 = engine, [], time.perf_counter()
+        self.n_seg = 1 if seg is None else seg[2]
+        self.device = hasattr(engine, "start_trace")
+        if self.device:
+            want = stop_cycle or 1024
+            engine.start_trace(max(1, min(want, TRACE_BYTES // (16 * self.n_seg))), infinity, unary, seg)
+        else:
+            self.host_costs, self.cycle = host_costs, getattr(engine, "cycle", 0)
+        # what _run_cycles calls after every single cycle: nothing when the device records inside the step loop
+        self.after_cycle = None if self.device else self._host_row
+
+    def _host_row(self):
+        c = getattr(self.engine, "cycle", None)
+        if c is not None and c == self.cycle:   # the engine stopped: no cycle ran
+            return
+        self.cycle = c
+        t = time.perf_counter() - self.t0
+        self.rows.append((t, self.host_costs(_indices(self.engine))))
+
+    def result(self, n_cycles=None):
+        """One trace dict per segment; `n_cycles`: keep the first n (DBA: the rounds that changed the state)."""
+        if self.device:
+            tr = self.engine.trace()
+            self.engine.stop_trace()
+            t, cost, viol = tr["time"], tr["cost"], tr["violation"]
+        else:
+            t = np.array([r[0] for r in self.rows], dtype=np.float64)
+            cost = np.array([[c for _, c in r[1]] for r in self.rows], dtype=np.float64).reshape(-1, self.n_seg)
+            viol = np.array([[v for v, _ in r[1]] for r in self.rows], dtype=np.int64).reshape(-1, self.n_seg)
+        n = len(t) if n_cycles is None else min(len(t), int(n_cycles))
+        return [{"cycle": list(range(1, n + 1)), "time": [float(x) for x in t[:n]],
+                 "cost": [float(x) for x in cost[:n, k]], "violation": [int(x) for x in viol[:n, k]]}
+                for k in range(self.n_seg)]
 
 
 BATCHED = ("maxsum", "dsa", "adsa", "mgm", "mgm2", "gdba", "mixeddsa")
@@ -361,7 +433,7 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
                 precision: str = "f32", device=None, seed: Union[None, int, Sequence[int]] = None,
                 infinity: float = float("inf"),
                 chunk: int = 50, max_vars: int = batch.MAX_BATCH_VARS,
-                engine_factory: Optional[Callable] = None) -> List[Dict[str, Any]]:
+                engine_factory: Optional[Callable] = None, trace: bool = False) -> List[Dict[str, Any]]:
     """Run `algo` on every problem of `problems` and return one result dict per problem, in input order, with
     solve()'s keys.
 
@@ -383,6 +455,8 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
     algo: maxsum | dsa | adsa | mgm | mgm2 | gdba | mixeddsa (the fixed-length families; dba, dpop and syncbb are
     refused).  engine_factory(kind, layout, inst, params): as in solve(), `inst` with var_rank, var_global_id and
     var_seed (None when the group's problems share one seed, params["seed"]).
+    trace: every result gains solve()'s "trace", cut out of its group's per-problem record (its times are the
+    group's); the trace of a problem whose group never started is empty.
     """
     kind = ALGOS.get(algo)
     if kind in NOT_BATCHED:
@@ -429,7 +503,14 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
                                  var_seed=var_seed)
         ingest_time += time.perf_counter() - t_group
         engine.init()
-        cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline)
+        tracer = None
+        if trace:
+            tracer = _Trace(engine, stop_cycle, infinity, u.unary, (u.seg_factor, u.seg_var, len(members)),
+                            lambda idx: [solution_cost(dcops[i], idx[u.var_start[k]:u.var_start[k + 1]], infinity)
+                                         for k, i in enumerate(members)])
+        cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline,
+                                    after_cycle=tracer.after_cycle if tracer else None)
+        traces = tracer.result() if tracer is not None else None
         idx = _indices(engine)
         if hasattr(engine, "solution_costs_segmented"):   # reduced per problem on the device
             costs, violations = engine.solution_costs_segmented(u.seg_factor, u.seg_var, len(members), infinity,
@@ -444,6 +525,8 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
                           "violation": int(violations[k]), "cycle": cycle, "msg_count": 0, "msg_size": 0,
                           "algo": kind, "precision": precision, "n_gpus": 1, "h2d_bytes": h2d,
                           "d2h_bytes": int(len(v) * 12 + 16)}
+            if traces is not None:
+                results[i]["trace"] = traces[k]
     total = time.perf_counter() - t0
     for r in results:
         r.update(time=total, ingest_time=ingest_time)
@@ -519,6 +602,9 @@ def main(argv=None):
                     help="CSV of cycle,time,cost,violation,msg_count,msg_size,status every --metrics_every "
                          "cycles (the columns of `pydcop solve --run_metrics`, commands/solve.py:356-375)")
     ap.add_argument("--metrics_every", type=int, default=10, metavar="CYCLES")
+    ap.add_argument("--collect_on", choices=["cycle_change"], default=None,
+                    help="cycle_change: the solution cost of EVERY cycle, recorded on the device inside the step loop "
+                         "(solve(trace=True)): --run_metrics gets one row per cycle, --batch entries a \"trace\"")
     ap.add_argument("--partition", default="auto", choices=["auto", "blocks", "multilevel"],
                     help="under torchrun: how the variables are split over the GPUs")
     ap.add_argument("--batch", action="store_true",
@@ -539,6 +625,7 @@ def main(argv=None):
         if args.run_metrics or args.save or world > 1:
             ap.error("--batch runs on one GPU and takes neither --run_metrics, --save nor torchrun")
         return _main_batch(args, _algo_params(ap, args))
+    trace = args.collect_on == "cycle_change"
     if world > 1:   # launched by torchrun: one process per GPU over NCCL
         import torch
         import torch.distributed as dist
@@ -555,10 +642,15 @@ def main(argv=None):
         violation, cost = solution_cost(dcop, idx, args.infinity)
         rows.append((cycle, time.perf_counter() - t_start, cost, violation, 0, 0, "RUNNING"))
 
+    host_rows = args.run_metrics and not trace
     res = solve(dcop, args.algo, params, args.timeout, args.precision, seed=args.seed,
                 infinity=args.infinity, partition=args.partition,
-                chunk=max(1, args.metrics_every) if args.run_metrics else 50,
-                on_cycle=collect if args.run_metrics else None)
+                chunk=max(1, args.metrics_every) if host_rows else 50,
+                on_cycle=collect if host_rows else None, trace=trace)
+    if trace and args.run_metrics:
+        tr = res.pop("trace")
+        rows = [(c, t, cost, v, 0, 0, "RUNNING")
+                for c, t, cost, v in zip(tr["cycle"], tr["time"], tr["cost"], tr["violation"])]
     if args.run_metrics and rank == 0:
         import csv
         with open(args.run_metrics, "w", newline="") as f:
@@ -588,7 +680,7 @@ def _algo_params(ap, args):
 def _main_batch(args, params):
     if args.iterations is None:
         res = solve_batch(args.dcop_files, args.algo, params, args.timeout, args.precision, seed=args.seed,
-                          infinity=args.infinity)
+                          infinity=args.infinity, trace=args.collect_on == "cycle_change")
         for path, r in zip(args.dcop_files, res):
             r["problem"] = path
     else:
@@ -596,7 +688,8 @@ def _main_batch(args, params):
         base, n = args.seed or 0, args.iterations
         dcops = [load(path, base) for path in args.dcop_files]
         res = solve_batch([d for d in dcops for _ in range(n)], args.algo, params, args.timeout, args.precision,
-                          seed=[base + r for _ in dcops for r in range(n)], infinity=args.infinity)
+                          seed=[base + r for _ in dcops for r in range(n)], infinity=args.infinity,
+                          trace=args.collect_on == "cycle_change")
         for k, r in enumerate(res):
             r.update(problem=args.dcop_files[k // n], iteration=k % n, seed=base + k % n)
     for r in res:
