@@ -54,7 +54,7 @@
 extern "C" {
 #endif
 
-#define FG_ABI_VERSION 2
+#define FG_ABI_VERSION 3
 #define FG_MAX_ARITY 8
 #define FG_MAX_DOM 256
 
@@ -62,6 +62,7 @@ enum { FG_OK = 0, FG_ERR_ARG = 1, FG_ERR_CUDA = 2, FG_ERR_UNSUPPORTED = 3 };
 enum { FG_F32 = 0, FG_F64 = 1 };
 enum { FG_START_LEAFS = 0, FG_START_LEAFS_VARS = 1, FG_START_ALL = 2 }; /* maxsum.py:219 */
 enum { FG_DSA_A = 0, FG_DSA_B = 1, FG_DSA_C = 2 };                      /* dsa.py:133 */
+#define FG_MAX_PSETS 65535   /* parameter sets of one handle: indices are uint16 */
 enum { FG_CLASS_GHOST = 1, FG_CLASS_BOUNDARY = 2 };
 
 /* One class of same-shaped factors (constraints). */
@@ -225,6 +226,11 @@ int fg_halo_push(int32_t precision, const void *dev_r, const void *dev_q, const 
  * relations.py:1367-1400 — for ALL variables at once).  Random draws are Philox4x32-10 keyed by
  * (seed; variable, cycle): u = 53-bit uniform, choice = (word*n)>>32 (oracle/philox.py).
  * ------------------------------------------------------------------------------------------ */
+/* one parameter set of a DSA / A-DSA handle: the decision rule (the probability reaches the kernels as dev_prob) */
+typedef struct {
+  int32_t variant;               /* FG_DSA_* */
+} fg_dsa_pset_t;
+
 typedef struct {
   int32_t abi_version, precision;
   int32_t n_vars, n_factors, n_edges, n_classes;
@@ -268,6 +274,13 @@ typedef struct {
   uint8_t *dev_slot_last;        /* [n_edges] */
   const uint64_t *dev_var_seed;  /* [n_vars] optional: the Philox key of internal variable v, in place of `seed`
                                    (a batch of problems, each run with its own seed); NULL = `seed` for all */
+  /* optional parameter sets (a batch of problems, each with its own algorithm parameters): dev_var_pset[v] is the
+   * set of internal variable v, an index into the HOST table psets[0 .. n_psets).  create validates every set and
+   * copies the table into device memory the handle owns; the kernels read it there.  Both NULL (n_psets 0, anything
+   * else is refused): every variable takes the scalar fields above. */
+  const uint16_t *dev_var_pset;  /* [n_vars] */
+  const fg_dsa_pset_t *psets;
+  int32_t n_psets, reserved_ps;
 } fg_dsa_desc_t;
 
 typedef struct fg_dsa *fg_dsa_t;
@@ -440,6 +453,13 @@ int64_t fg_mgm_launch_count(fg_mgm_t h);
  * ------------------------------------------------------------------------------------------ */
 enum { FG_MGM2_FAVOR_UNILATERAL = 0, FG_MGM2_FAVOR_NO = 1, FG_MGM2_FAVOR_COORDINATED = 2 };
 
+/* one parameter set of an MGM-2 handle */
+typedef struct {
+  double threshold;               /* finite, in [0, 1] */
+  int32_t favor;                  /* FG_MGM2_FAVOR_* */
+  int32_t reserved0;
+} fg_mgm2_pset_t;
+
 typedef struct {
   int32_t abi_version, precision;
   int32_t n_vars, n_factors, n_edges, n_classes;
@@ -479,6 +499,10 @@ typedef struct {
   int32_t reserved0;
   uint64_t seed;
   const uint64_t *dev_var_seed;   /* [n_vars] optional: Philox key of internal variable v; NULL = `seed` */
+  /* optional parameter sets, as fg_dsa_desc_t's */
+  const uint16_t *dev_var_pset;  /* [n_vars] */
+  const fg_mgm2_pset_t *psets;
+  int32_t n_psets, reserved_ps;
 } fg_mgm2_desc_t;
 
 typedef struct fg_mgm2 *fg_mgm2_t;
@@ -567,6 +591,13 @@ enum { FG_GDBA_MODIFIER_A = 0, FG_GDBA_MODIFIER_M = 1 };
 enum { FG_GDBA_VIOLATION_NZ = 0, FG_GDBA_VIOLATION_NM = 1, FG_GDBA_VIOLATION_MX = 2 };
 enum { FG_GDBA_INCREASE_E = 0, FG_GDBA_INCREASE_R = 1, FG_GDBA_INCREASE_C = 2, FG_GDBA_INCREASE_T = 3 };
 
+/* one parameter set of a GDBA handle (increase_mode stays one per handle: it decides the modifier layout); with
+ * NM / MX the factors of the variables of a set read their dev_viol_ref entry of that set's mode */
+typedef struct {
+  int32_t modifier;               /* FG_GDBA_MODIFIER_* */
+  int32_t violation;              /* FG_GDBA_VIOLATION_* */
+} fg_gdba_pset_t;
+
 typedef struct {
   int32_t abi_version, precision;
   int32_t n_vars, n_factors, n_edges, n_classes;
@@ -606,6 +637,10 @@ typedef struct {
   int64_t mod_size;               /* elements of dev_mod */
   uint64_t seed;
   const uint64_t *dev_var_seed;   /* [n_vars] optional: Philox key of internal variable v; NULL = `seed` */
+  /* optional parameter sets, as fg_dsa_desc_t's */
+  const uint16_t *dev_var_pset;  /* [n_vars] */
+  const fg_gdba_pset_t *psets;
+  int32_t n_psets, reserved_ps;
 } fg_gdba_desc_t;
 
 typedef struct fg_gdba *fg_gdba_t;
@@ -834,6 +869,13 @@ enum { FG_MIXEDDSA_BRANCH_NONE = 0, FG_MIXEDDSA_BRANCH_HARD = 1, FG_MIXEDDSA_BRA
        FG_MIXEDDSA_BRANCH_STUCK_HARD = 3, FG_MIXEDDSA_BRANCH_STUCK_SOFT = 4, FG_MIXEDDSA_BRANCH_IDLE = 5,
        FG_MIXEDDSA_MOVED = 8 };
 
+/* one parameter set of a MixedDSA handle */
+typedef struct {
+  double proba_hard, proba_soft;  /* finite, in [0, 1] */
+  int32_t variant;                /* FG_DSA_* */
+  int32_t reserved0;
+} fg_mixeddsa_pset_t;
+
 typedef struct {
   int32_t abi_version, precision;
   int32_t n_vars, n_factors, n_edges, n_classes;
@@ -864,6 +906,10 @@ typedef struct {
   int32_t reserved0;
   uint64_t seed;
   const uint64_t *dev_var_seed;   /* [n_vars] optional: Philox key of internal variable v; NULL = `seed` */
+  /* optional parameter sets, as fg_dsa_desc_t's */
+  const uint16_t *dev_var_pset;  /* [n_vars] */
+  const fg_mixeddsa_pset_t *psets;
+  int32_t n_psets, reserved_ps;
 } fg_mixeddsa_desc_t;
 
 typedef struct fg_mixeddsa *fg_mixeddsa_t;

@@ -5,13 +5,14 @@ Fails loudly when the library is missing: there is no Python/CPU fallback for th
 import ctypes as C
 import os
 
-FG_ABI_VERSION = 2
+FG_ABI_VERSION = 3
 FG_MAX_ARITY = 8
 FG_MAX_DOM = 256
 FG_OK, FG_ERR_ARG, FG_ERR_CUDA, FG_ERR_UNSUPPORTED = 0, 1, 2, 3
 FG_F32, FG_F64 = 0, 1
 START_MESSAGES = {"leafs": 0, "leafs_vars": 1, "all": 2}
 DSA_VARIANTS = {"A": 0, "B": 1, "C": 2}
+FG_MAX_PSETS = 65535   # parameter sets of one handle (uint16 indices)
 
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libpydcop_b200.so")
 
@@ -54,6 +55,10 @@ class FgMaxSumDesc(C.Structure):
                 ("start_messages", C.c_int32), ("damping", C.c_double), ("stability", C.c_double)]
 
 
+class FgDsaPset(C.Structure):
+    _fields_ = [("variant", C.c_int32)]
+
+
 class FgDsaDesc(C.Structure):
     _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
                 ("n_vars", C.c_int32), ("n_factors", C.c_int32), ("n_edges", C.c_int32),
@@ -67,7 +72,9 @@ class FgDsaDesc(C.Structure):
                 ("mode_max", C.c_int32), ("variant", C.c_int32), ("stop_cycle", C.c_int32),
                 ("seed", C.c_uint64), ("dev_var_cost", P), ("dev_unary_off", P),
                 ("dev_row_cache", P), ("dev_slot_last", P),
-                ("dev_var_seed", P)]
+                ("dev_var_seed", P),
+                ("dev_var_pset", P), ("psets", C.POINTER(FgDsaPset)), ("n_psets", C.c_int32),
+                ("reserved_ps", C.c_int32)]
 
 
 class FgMgmDesc(C.Structure):
@@ -86,6 +93,10 @@ class FgMgmDesc(C.Structure):
                 ("dev_var_seed", P)]
 
 
+class FgMgm2Pset(C.Structure):
+    _fields_ = [("threshold", C.c_double), ("favor", C.c_int32), ("reserved0", C.c_int32)]
+
+
 class FgMgm2Desc(C.Structure):
     _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
                 ("n_vars", C.c_int32), ("n_factors", C.c_int32), ("n_edges", C.c_int32),
@@ -99,10 +110,16 @@ class FgMgm2Desc(C.Structure):
                 ("dev_answer_gain", P), ("dev_offer_off", P), ("dev_offer", P),
                 ("mode_max", C.c_int32), ("favor", C.c_int32), ("threshold", C.c_double),
                 ("stop_cycle", C.c_int32), ("reserved0", C.c_int32), ("seed", C.c_uint64),
-                ("dev_var_seed", P)]
+                ("dev_var_seed", P),
+                ("dev_var_pset", P), ("psets", C.POINTER(FgMgm2Pset)), ("n_psets", C.c_int32),
+                ("reserved_ps", C.c_int32)]
 
 
 MGM2_FAVORS = {"unilateral": 0, "no": 1, "coordinated": 2}
+
+
+class FgGdbaPset(C.Structure):
+    _fields_ = [("modifier", C.c_int32), ("violation", C.c_int32)]
 
 
 class FgGdbaDesc(C.Structure):
@@ -118,7 +135,9 @@ class FgGdbaDesc(C.Structure):
                 ("mode_max", C.c_int32), ("modifier", C.c_int32), ("violation", C.c_int32),
                 ("increase_mode", C.c_int32), ("stop_cycle", C.c_int32), ("reserved0", C.c_int32),
                 ("mod_size", C.c_int64), ("seed", C.c_uint64),
-                ("dev_var_seed", P)]
+                ("dev_var_seed", P),
+                ("dev_var_pset", P), ("psets", C.POINTER(FgGdbaPset)), ("n_psets", C.c_int32),
+                ("reserved_ps", C.c_int32)]
 
 
 class FgDpopLaunch(C.Structure):
@@ -166,6 +185,11 @@ class FgSyncbbDesc(C.Structure):
                 ("dev_cycles", P), ("n_elts", C.c_int64), ("n_pair", C.c_int64)]
 
 
+class FgMixedDsaPset(C.Structure):
+    _fields_ = [("proba_hard", C.c_double), ("proba_soft", C.c_double), ("variant", C.c_int32),
+                ("reserved0", C.c_int32)]
+
+
 class FgMixedDsaDesc(C.Structure):
     _fields_ = [("abi_version", C.c_int32), ("precision", C.c_int32),
                 ("n_vars", C.c_int32), ("n_factors", C.c_int32), ("n_edges", C.c_int32),
@@ -177,7 +201,9 @@ class FgMixedDsaDesc(C.Structure):
                 ("dev_h_best", P), ("dev_branch", P),
                 ("proba_hard", C.c_double), ("proba_soft", C.c_double),
                 ("mode_max", C.c_int32), ("variant", C.c_int32), ("stop_cycle", C.c_int32),
-                ("reserved0", C.c_int32), ("seed", C.c_uint64), ("dev_var_seed", P)]
+                ("reserved0", C.c_int32), ("seed", C.c_uint64), ("dev_var_seed", P),
+                ("dev_var_pset", P), ("psets", C.POINTER(FgMixedDsaPset)), ("n_psets", C.c_int32),
+                ("reserved_ps", C.c_int32)]
 
 
 MIXEDDSA_VARIANTS = {"A": 0, "B": 1, "C": 2}

@@ -7,7 +7,9 @@ mechanism the sharded engines use the other way round, DESIGN.md §6), the name 
 neighbours) and the start value of a variable without neighbours.  The union's canonical variable order is the
 concatenation of the problems', so problem k's values are one slice of the result.  Problems with seeds of their own
 also carry their own Philox key (`var_seed`: the problem's seed on each of its variables), so one problem can run many
-times in one union, once per seed.
+times in one union, once per seed.  Problems with algorithm parameters of their own carry the index of their parameter
+set (`var_pset`) on each of their variables, for the parameters the kernels read per variable; the others split
+groups (`groups`' keys).
 """
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Union as AnyOf
@@ -19,6 +21,7 @@ from .layout import FactorGraphLayout, build_layout
 
 INDEX_LIMIT = 2 ** 31 - 1      # variables, factors and edges of one engine are int32 indices
 MAX_BATCH_VARS = 1 << 20       # default bound on the variables of one engine: C4's size
+MAX_PSETS = 65535              # parameter sets of one engine: uint16 indices (FG_MAX_PSETS)
 
 
 def _front_door_consistent(a: Dict[str, np.ndarray]) -> bool:
@@ -47,23 +50,30 @@ def layout_of(index: int, inst) -> FactorGraphLayout:
         raise ValueError(f"problem {index}: {e}") from e
 
 
-def groups(dcops: List[ingest.DcopArrays], max_vars: int = MAX_BATCH_VARS) -> List[List[int]]:
-    """Problem indices per engine: one objective per group (mode_max is one scalar per engine), min before max in
-    order of first appearance, input order inside; a group is cut before it would exceed `max_vars` variables or an
-    int32 index range (a problem larger than that runs alone)."""
+def groups(dcops: List[ingest.DcopArrays], max_vars: int = MAX_BATCH_VARS, keys: Optional[Sequence] = None,
+           sets: Optional[Sequence] = None) -> List[List[int]]:
+    """Problem indices per engine: one objective and one group key per group (mode_max and the parameters the kernels
+    cannot take per variable are one scalar per engine; keys: one hashable per problem, None: one for all), groups in
+    order of first appearance, input order inside; a group is cut before it would exceed `max_vars` variables, an
+    int32 index range (a problem larger than that runs alone) or MAX_PSETS distinct parameter sets (sets: one hashable
+    per problem, None: one for all)."""
+    keys = [None] * len(dcops) if keys is None else list(keys)
+    sets = [None] * len(dcops) if sets is None else list(sets)
     out = []
-    for mode in dict.fromkeys(d.objective for d in dcops):
-        cur, size = [], np.zeros(3, dtype=np.int64)
+    for group in dict.fromkeys(zip((d.objective for d in dcops), keys)):
+        cur, size, seen = [], np.zeros(3, dtype=np.int64), set()
         for i, d in enumerate(dcops):
-            if d.objective != mode:
+            if (d.objective, keys[i]) != group:
                 continue
             a = d.arrays
             s = np.array([d.n_vars, len(a["factor_ptr"]) - 1, len(a["edge_var"])], dtype=np.int64)
             t = size + s
-            if cur and (t[0] > max_vars or (t > INDEX_LIMIT).any()):
+            new_set = sets[i] not in seen
+            if cur and (t[0] > max_vars or (t > INDEX_LIMIT).any() or (new_set and len(seen) >= MAX_PSETS)):
                 out.append(cur)
-                cur, t = [], s
+                cur, t, seen = [], s, set()
             cur.append(i)
+            seen.add(sets[i])
             size = t
         out.append(cur)
     return out
@@ -78,22 +88,32 @@ class Union:
     var_start: np.ndarray                # [n + 1] first variable of every problem, then the total
     var_global_id: np.ndarray            # each variable's index in its own problem
     var_seed: Optional[np.ndarray]       # each variable's problem's seed (uint64), None when all problems share one
+    var_pset: Optional[np.ndarray]       # each variable's problem's parameter set, None when all problems share one
+    psets: List[dict]                    # the distinct parameter sets, in order of first appearance
     var_rank: Optional[np.ndarray]       # each variable's name rank in its own problem
     isolated_value: Optional[np.ndarray]  # start value of the variables without neighbours, per problem
     seg_factor: np.ndarray               # problem (0..n-1) of every canonical factor
     seg_var: np.ndarray                  # problem of every canonical variable
 
 
-def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs, noise: float = 0.0,
-                seed: AnyOf[None, int, Sequence[int]] = None) -> Union:
+def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs,
+                noise: AnyOf[float, Sequence[float]] = 0.0, seed: AnyOf[None, int, Sequence[int]] = None,
+                params: Optional[Sequence[dict]] = None) -> Union:
     """Concatenate the problems `members` of `dcops`: variable, edge and table indices are offset by the problems
     before.  var_inputs(dcop) -> (var_rank or None, isolated_value or None), each problem's own; `seed`: one for every
-    member, or a sequence with one per member; `noise`: MaxSum's, drawn per problem with its seed exactly as solve()
-    draws it."""
+    member, or a sequence with one per member; `noise`: MaxSum's, one for every member or one per member, drawn per
+    problem with its seed exactly as solve() draws it; `params`: one parameter dict per member (None: one set for
+    all), whose distinct dicts become `psets`."""
     parts = [dcops[i].arrays for i in members]
     seeds = [seed] * len(members) if seed is None or isinstance(seed, (int, np.integer)) else list(seed)
     if len(seeds) != len(members):
         raise ValueError(f"{len(seeds)} seeds for {len(members)} problems")
+    noises = list(noise) if isinstance(noise, (list, tuple, np.ndarray)) else [noise] * len(members)
+    if len(noises) != len(members):
+        raise ValueError(f"{len(noises)} noise levels for {len(members)} problems")
+    ids = {}
+    member_set = [ids.setdefault(pset_key(p), len(ids)) for p in params] if params is not None else [0] * len(members)
+    psets = [dict(params[member_set.index(k)]) for k in range(len(ids))] if params is not None else []
     n_var = np.array([len(a["dom_size"]) for a in parts], dtype=np.int64)
     n_fac = np.array([len(a["factor_ptr"]) - 1 for a in parts], dtype=np.int64)
     n_edge = np.array([len(a["edge_var"]) for a in parts], dtype=np.int64)
@@ -110,8 +130,8 @@ def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs, 
                 edge_var=np.concatenate([np.asarray(a["edge_var"], dtype=np.int64) + o
                                          for a, o in zip(parts, v0[:-1])]).astype(np.int32),
                 table_off=ptr("table_off", t0), tables=np.concatenate([np.asarray(a["tables"]) for a in parts]),
-                unary=(np.concatenate([ingest.add_noise(a["unary"], noise, s) for a, s in zip(parts, seeds)])
-                       if noise else unary),
+                unary=(np.concatenate([ingest.add_noise(a["unary"], nz, s) for a, nz, s in zip(parts, noises, seeds)])
+                       if any(noises) else unary),
                 var_ptr=ptr("var_ptr", e0).astype(np.int32),
                 var_edge=np.concatenate([np.asarray(a["var_edge"], dtype=np.int64) + o
                                          for a, o in zip(parts, e0[:-1])]).astype(np.int32),
@@ -122,9 +142,16 @@ def build_union(dcops: List[ingest.DcopArrays], members: List[int], var_inputs, 
                  var_global_id=np.concatenate([np.arange(n, dtype=np.int32) for n in n_var]),
                  var_seed=(None if len(set(seeds)) == 1 else
                            np.repeat(np.array([int(s) & (2 ** 64 - 1) for s in seeds], dtype=np.uint64), n_var)),
+                 var_pset=None if len(psets) <= 1 else np.repeat(np.array(member_set, dtype=np.int32), n_var),
+                 psets=psets,
                  var_rank=None if ranks[0] is None else np.concatenate(ranks).astype(np.int32),
                  isolated_value=None if isos[0] is None else np.concatenate(isos).astype(np.int32),
                  seg_factor=np.repeat(seg, n_fac), seg_var=np.repeat(seg, n_var))
+
+
+def pset_key(params: dict):
+    """A hashable identity of one parameter dict."""
+    return tuple(sorted(params.items()))
 
 
 def union_layout(u: Union, dcops: List[ingest.DcopArrays]) -> FactorGraphLayout:

@@ -29,13 +29,15 @@ struct DsaCachedCfg {
   static constexpr bool VEC = (D * sizeof(T)) % 16 == 0;
 };
 
-template <typename T, int D>
+// PS: every variable reads its variant from its parameter set (var_pset), as k_dsa_step_generic
+template <typename T, int D, bool PS>
 __global__ void __launch_bounds__(DsaCachedCfg<T, D>::THREADS)
 k_dsa_step_cached(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *__restrict__ slot_nbr,
                   const int64_t *__restrict__ slot_tab, const T *__restrict__ slot_opt, const T *__restrict__ tables_or,
                   const uint8_t *__restrict__ has_nbr, const double *__restrict__ prob, const int32_t *__restrict__ var_id,
-                  const uint64_t *__restrict__ var_seed,
-                  const int32_t *__restrict__ val, int32_t *__restrict__ val_next, T *__restrict__ val_cost, int mode_max,
+                  const uint64_t *__restrict__ var_seed, const uint16_t *__restrict__ var_pset,
+                  const fg_dsa_pset_t *__restrict__ psets, const int32_t *__restrict__ val,
+                  int32_t *__restrict__ val_next, T *__restrict__ val_cost, int mode_max,
                   int variant, uint64_t seed, uint32_t cycle, const T *__restrict__ var_cost,
                   const int64_t *__restrict__ unary_off, T *row_cache, uint8_t *slot_last) {
   using Cfg = DsaCachedCfg<T, D>;
@@ -55,6 +57,7 @@ k_dsa_step_cached(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t
   const int v = v0 + tid;
   const bool mine = tid < nv;
   const int cur = mine ? val[v] : 0;
+  if (PS && mine) variant = fg_pset(var_pset, psets, v).variant;
   __syncthreads();
   const int sb = sptr[0], se = sptr[nv];
   const int my_a = mine ? sptr[tid] : 0, my_b = mine ? sptr[tid + 1] : 0;
@@ -198,9 +201,11 @@ inline bool dsa_cached_step(const fg_dsa_desc_t &d, const int32_t *val, int32_t 
     using Cfg = DsaCachedCfg<T, n>;                                                                                   \
     static_assert(sizeof(T) * Cfg::CH * (n + 1) + 2 * Cfg::CH + 4 * (Cfg::NV + 1) <= 48 * 1024, "static shared memory");    \
     const unsigned blocks = (unsigned)((d.n_vars + Cfg::NV - 1) / Cfg::NV);                                           \
-    k_dsa_step_cached<T, n><<<blocks, Cfg::THREADS, 0, st>>>(                                                         \
+    (d.dev_var_pset ? k_dsa_step_cached<T, n, true>                                                                   \
+                    : k_dsa_step_cached<T, n, false>)<<<blocks, Cfg::THREADS, 0, st>>>(                               \
         d.n_vars, d.dev_var_ptr, d.dev_slot_nbr, d.dev_slot_tab, (const T *)d.dev_slot_opt, (const T *)d.dev_tables_or, \
-        d.dev_has_nbr, d.dev_prob, d.dev_var_id, d.dev_var_seed, val, val_next, (T *)d.dev_value_cost, d.mode_max,       \
+        d.dev_has_nbr, d.dev_prob, d.dev_var_id, d.dev_var_seed, d.dev_var_pset, d.psets, val, val_next,               \
+        (T *)d.dev_value_cost, d.mode_max,                                                                            \
         d.variant, d.seed, cycle, (const T *)d.dev_var_cost, d.dev_unary_off, (T *)d.dev_row_cache, d.dev_slot_last);                     \
     ++launches;                                                                                                       \
     return true;                                                                                                      \

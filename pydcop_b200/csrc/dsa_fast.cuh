@@ -11,14 +11,16 @@
 #include "philox.cuh"
 #include "row_load.cuh"
 
-template <typename T, int D>
+// PS: every variable reads its variant from its parameter set (var_pset), as k_dsa_step_generic
+template <typename T, int D, bool PS>
 __global__ void __launch_bounds__(128)
 k_dsa_step_bin(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *__restrict__ slot_nbr,
                const int64_t *__restrict__ slot_tab, const T *__restrict__ slot_opt,
                const T *__restrict__ tables_or, const uint8_t *__restrict__ has_nbr,
                const double *__restrict__ prob, const int32_t *__restrict__ var_id,
-               const uint64_t *__restrict__ var_seed,
-               const int32_t *__restrict__ val, int32_t *__restrict__ val_next, T *__restrict__ val_cost,
+               const uint64_t *__restrict__ var_seed, const uint16_t *__restrict__ var_pset,
+               const fg_dsa_pset_t *__restrict__ psets, const int32_t *__restrict__ val,
+               int32_t *__restrict__ val_next, T *__restrict__ val_cost,
                int mode_max, int variant, uint64_t seed, uint32_t cycle, const T *__restrict__ var_cost,
                const int64_t *__restrict__ unary_off) {
   constexpr int RS = fg_row_stride<T, D>();   // rows on their own line slots
@@ -30,6 +32,7 @@ k_dsa_step_bin(int n_vars, const int32_t *__restrict__ var_ptr, const int32_t *_
     if (hn == 0) val_next[v] = cur;
     return;
   }
+  if (PS) variant = fg_pset(var_pset, psets, v).variant;
   T cost[D];
 #pragma unroll
   for (int x = 0; x < D; ++x) cost[x] = (T)0;
@@ -103,12 +106,11 @@ inline bool dsa_fast_step(const fg_dsa_desc_t &d, const std::vector<fg_class_t> 
   switch (d.fast_dom) {
 #define X(n)                                                                                               \
   case n:                                                                                                  \
-    k_dsa_step_bin<T, n><<<blocks, 128, 0, st>>>(d.n_vars, d.dev_var_ptr, d.dev_slot_nbr, d.dev_slot_tab,   \
-                                                 (const T *)d.dev_slot_opt, (const T *)d.dev_tables_or,     \
-                                                 d.dev_has_nbr, d.dev_prob, d.dev_var_id, d.dev_var_seed,   \
-                                                 val, val_next, (T *)d.dev_value_cost, d.mode_max, d.variant,   \
-                                                 d.seed, cycle,                                                 \
-                                                 (const T *)d.dev_var_cost, d.dev_unary_off);               \
+    (d.dev_var_pset ? k_dsa_step_bin<T, n, true> : k_dsa_step_bin<T, n, false>)<<<blocks, 128, 0, st>>>(    \
+        d.n_vars, d.dev_var_ptr, d.dev_slot_nbr, d.dev_slot_tab, (const T *)d.dev_slot_opt,                  \
+        (const T *)d.dev_tables_or, d.dev_has_nbr, d.dev_prob, d.dev_var_id, d.dev_var_seed, d.dev_var_pset,   \
+        d.psets, val, val_next, (T *)d.dev_value_cost, d.mode_max, d.variant, d.seed, cycle,                   \
+        (const T *)d.dev_var_cost, d.dev_unary_off);                                                         \
     ++launches;                                                                                            \
     return true;
     FG_FAST_DOMS(X)

@@ -9,6 +9,8 @@ struct DsaSide {
   const uint8_t *has_nbr;
   const double *prob;
   const uint64_t *var_seed;  // [n_vars] Philox key of each variable, NULL: the run's seed
+  const uint16_t *var_pset;  // [n_vars] parameter set of each variable, NULL: the descriptor's scalars
+  const fg_dsa_pset_t *psets;
 };
 
 // find_optimum (relations.py:1367-1400): optimum of the whole table of each constraint
@@ -35,8 +37,9 @@ __global__ void k_dsa_init(DsaSide g, int n_vars, uint64_t seed, int32_t *__rest
   value[v] = philox_choice(b, g.dom_size[v]);
 }
 
-// evaluate_cycle (dsa.py:320-357) for every variable.
-template <typename T>
+// evaluate_cycle (dsa.py:320-357) for every variable.  PS: every variable reads its variant from its parameter set
+// (g.var_pset); without, the instantiation is the one the runs without sets have always had.
+template <typename T, bool PS>
 __global__ void __launch_bounds__(128)
 k_dsa_step_generic(DsaSide g, int n_vars, const T *__restrict__ tables,
                    const T *__restrict__ con_opt, const int32_t *__restrict__ val,
@@ -51,6 +54,7 @@ k_dsa_step_generic(DsaSide g, int n_vars, const T *__restrict__ tables,
     if (hn == 0) val_next[v] = cur;
     return;
   }
+  if (PS) variant = fg_pset(g.var_pset, g.psets, v).variant;
   const int d = g.dom_size[v];
   T cost[FG_MAX_DOM];
   for (int x = 0; x < d; ++x) cost[x] = (T)0;
@@ -123,7 +127,7 @@ k_dsa_step_generic(DsaSide g, int n_vars, const T *__restrict__ tables,
 
 static inline DsaSide dsa_side(const fg_dsa_desc_t &d, const fg_class_t *classes) {
   return DsaSide{classes, d.dev_dom_size, d.dev_var_id, d.dev_edge_var, d.dev_edge_class, d.dev_var_ptr,
-                 d.dev_slot_edge, d.dev_has_nbr, d.dev_prob, d.dev_var_seed};
+                 d.dev_slot_edge, d.dev_has_nbr, d.dev_prob, d.dev_var_seed, d.dev_var_pset, d.psets};
 }
 
 // constraint optima, start values into both buffers, and the active-row array's "no row read yet"
@@ -144,7 +148,8 @@ static void dsa_init(const fg_dsa_desc_t &d, const fg_class_t *classes, L &launc
 // evaluate_cycle of round `cycle` from buffer cur into buffer cur ^ 1, on the generic kernel
 template <typename T, class L>
 static void dsa_step(const fg_dsa_desc_t &d, const fg_class_t *classes, int cur, uint32_t cycle, L &launch) {
-  launch(d.n_vars, 128, k_dsa_step_generic<T>, dsa_side(d, classes), d.n_vars, (const T *)d.dev_tables,
+  launch(d.n_vars, 128, d.dev_var_pset ? k_dsa_step_generic<T, true> : k_dsa_step_generic<T, false>,
+         dsa_side(d, classes), d.n_vars, (const T *)d.dev_tables,
          (const T *)d.dev_con_opt, d.dev_value[cur], d.dev_value[cur ^ 1], (T *)d.dev_value_cost, d.mode_max,
          d.variant, d.seed, cycle, (const T *)d.dev_var_cost, d.dev_unary_off);
 }

@@ -707,6 +707,10 @@ extern "C" int fg_dsa_create(const fg_dsa_desc_t *desc, fg_dsa_t *out) {
   int rc = fg_open(desc, out);
   if (rc != FG_OK) return rc;
   fg_dsa *h = *out;
+  rc = fg_check_psets(h, [](const fg_dsa_pset_t &p) -> const char * {
+    return p.variant < FG_DSA_A || p.variant > FG_DSA_C ? "variant is not an FG_DSA_* value" : nullptr;
+  });
+  if (rc != FG_OK) return rc;
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
   const fg_dsa_desc_t &d = *desc;
   rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_var_id),
@@ -716,8 +720,8 @@ extern "C" int fg_dsa_create(const fg_dsa_desc_t *desc, fg_dsa_t *out) {
                              FG_FIELD(d, dev_slot_tab), FG_FIELD(d, dev_slot_opt), FG_FIELD(d, dev_value[0]),
                              FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_value_cost), FG_FIELD(d, dev_var_cost),
                              FG_FIELD(d, dev_unary_off), FG_FIELD(d, dev_row_cache), FG_FIELD(d, dev_slot_last),
-                             FG_FIELD(d, dev_var_seed)});
-  if (rc != FG_OK) return rc;
+                             FG_FIELD(d, dev_var_seed), FG_FIELD(d, dev_var_pset)});
+  if (rc != FG_OK || (rc = fg_upload_psets(h)) != FG_OK) return rc;
   {  // experiment knob: L2 -> DRAM fetch granularity hint (32 | 64 | 128 bytes) for the sparse row reads
     const int g = fg_env_int("PYDCOP_B200_L2_FETCH", 0);
     if (g == 32 || g == 64 || g == 128) { cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)g); cudaGetLastError(); }

@@ -48,6 +48,15 @@ extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
     snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
     return FG_ERR_ARG;
   }
+  rc = fg_check_psets(h, [desc](const fg_gdba_pset_t &p) -> const char * {
+    if (p.modifier != FG_GDBA_MODIFIER_A && p.modifier != FG_GDBA_MODIFIER_M) return "modifier is not A (0) or M (1)";
+    if (p.violation < FG_GDBA_VIOLATION_NZ || p.violation > FG_GDBA_VIOLATION_MX)
+      return "violation is not NZ (0), NM (1) or MX (2)";
+    if (p.violation != FG_GDBA_VIOLATION_NZ && desc->n_edges > 0 && !desc->dev_viol_ref)
+      return "violation NM / MX needs dev_viol_ref";
+    return nullptr;
+  });
+  if (rc != FG_OK) return rc;
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
   const fg_gdba_desc_t &d = *desc;
   rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_unary), FG_FIELD(d, dev_unary_off),
@@ -58,8 +67,8 @@ extern "C" int fg_gdba_create(const fg_gdba_desc_t *desc, fg_gdba_t *out) {
                              FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_cost), FG_FIELD(d, dev_has_cost),
                              FG_FIELD(d, dev_improve), FG_FIELD(d, dev_new_value), FG_FIELD(d, dev_violated),
                              FG_FIELD(d, dev_breakout), FG_FIELD(d, dev_mod), FG_FIELD(d, dev_mod_off),
-                             FG_FIELD(d, dev_var_seed)});
-  if (rc != FG_OK) return rc;
+                             FG_FIELD(d, dev_var_seed), FG_FIELD(d, dev_var_pset)});
+  if (rc != FG_OK || (rc = fg_upload_psets(h)) != FG_OK) return rc;
   return fg_upload_classes(h);
 }
 

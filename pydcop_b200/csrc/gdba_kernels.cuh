@@ -53,19 +53,27 @@ __device__ __forceinline__ int64_t gdba_base_index(const MgmSide &g, const GdbaS
 // ok phase (gdba.py:352-387): evaluation of every value, violations at the current value, improve and
 // the value an improving variable would take.  Modifier counts: increase_mode T, one per slot at
 // mod[s] (mod_off == NULL); E / R / C, a table of the constraint's entries at mod + mod_off[s] for a
-// slot whose constraint spans the variable's neighbourhood, none (mod_off[s] < 0) elsewhere.
-template <typename T>
+// slot whose constraint spans the variable's neighbourhood, none (mod_off[s] < 0) elsewhere.  PS: every variable reads
+// its modifier and violation mode from its parameter set (var_pset); without, the instantiation is the one the runs
+// without sets have always had.
+template <typename T, bool PS>
 __global__ void __launch_bounds__(128, 8)
 k_gdba_eval(MgmSide g, int n_vars, const T *__restrict__ tables, const T *__restrict__ unary,
             const int64_t *__restrict__ unary_off, const T *__restrict__ viol_ref,
             const int32_t *__restrict__ mod, const int64_t *__restrict__ mod_off, int modifier_m, int violation,
             const int32_t *__restrict__ val, T *__restrict__ cost, uint8_t *__restrict__ has_cost,
             T *__restrict__ improve, int32_t *__restrict__ new_value, uint8_t *__restrict__ violated,
-            int mode_max, uint64_t seed, uint32_t cycle) {
+            int mode_max, uint64_t seed, uint32_t cycle, const uint16_t *__restrict__ var_pset,
+            const fg_gdba_pset_t *__restrict__ psets) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= n_vars) return;
   const int n0 = g.nbr_ptr[v], n1 = g.nbr_ptr[v + 1];
   if (n0 == n1) return;
+  if (PS) {
+    const fg_gdba_pset_t &p = fg_pset(var_pset, psets, v);
+    modifier_m = p.modifier;
+    violation = p.violation;
+  }
   const int cur = val[v];
   const int d = g.dom_size[v];
   const int base_mod = modifier_m ? 1 : 0;
@@ -218,9 +226,10 @@ static void gdba_cycle(const fg_gdba_desc_t &d, const fg_class_t *classes, int64
   const int n = d.n_vars;
   int32_t *vin = d.dev_value[done & 1], *vout = d.dev_value[(done + 1) & 1];
   const int64_t *mod_off = d.increase_mode == FG_GDBA_INCREASE_T ? nullptr : d.dev_mod_off;
-  launch(n, 128, k_gdba_eval<T>, g, n, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_unary_off,
-         (const T *)d.dev_viol_ref, d.dev_mod, mod_off, d.modifier, d.violation, vin, (T *)d.dev_cost, d.dev_has_cost,
-         (T *)d.dev_improve, d.dev_new_value, d.dev_violated, d.mode_max, d.seed, cyc);
+  launch(n, 128, d.dev_var_pset ? k_gdba_eval<T, true> : k_gdba_eval<T, false>, g, n, (const T *)d.dev_tables,
+         (const T *)d.dev_unary, d.dev_unary_off, (const T *)d.dev_viol_ref, d.dev_mod, mod_off, d.modifier,
+         d.violation, vin, (T *)d.dev_cost, d.dev_has_cost, (T *)d.dev_improve, d.dev_new_value, d.dev_violated,
+         d.mode_max, d.seed, cyc, d.dev_var_pset, d.psets);
   launch(n, 256, k_gdba_decide<T>, g, n, (const T *)d.dev_improve, d.dev_new_value, d.dev_violated, d.dev_mod,
          mod_off, d.increase_mode, d.mode_max, vin, vout, (T *)d.dev_cost, d.dev_breakout);
 }

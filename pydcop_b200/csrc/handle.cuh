@@ -20,6 +20,7 @@ struct fg_handle_base {
   int64_t cycle = 0;
   int64_t launches = 0;
   fg_trace *trace = nullptr;            // fg_<family>_set_trace: a record after every cycle of the step loop
+  void *dev_psets = nullptr;            // device copy of the descriptor's parameter sets (fg_upload_psets)
   mutable char err[512] = {0};        // written by const readers too (fg_device_scope)
 };
 
@@ -160,7 +161,7 @@ static inline int fg_require_device(fg_handle_base *h) {
   return FG_OK;
 }
 
-// the class table is the one device allocation the library owns (a few hundred bytes)
+// the class table is a device allocation the library owns (a few hundred bytes), as the parameter sets are
 static inline int fg_upload_classes(fg_handle_base *h) {
   size_t bytes = sizeof(fg_class_t) * (h->classes.empty() ? 1 : h->classes.size());
   CUDA_TRY(h, cudaMalloc(&h->dev_classes, bytes));
@@ -169,11 +170,45 @@ static inline int fg_upload_classes(fg_handle_base *h) {
   return FG_OK;
 }
 
+// The descriptor's parameter sets (dev_var_pset, psets[n_psets]): both or neither, at most FG_MAX_PSETS, and every
+// set accepted by valid(set) -> NULL or the reason it is refused.  Host memory only: runs before fg_require_device.
+template <class H, class V>
+static inline int fg_check_psets(H *h, V valid) {
+  const auto &d = h->d;
+  if (!d.dev_var_pset && !d.psets && !d.n_psets) return FG_OK;
+  if (!d.dev_var_pset || !d.psets || d.n_psets < 1 || d.n_psets > FG_MAX_PSETS) {
+    snprintf(h->err, sizeof(h->err), "dev_var_pset and psets go together, with 1 <= n_psets <= %d (n_psets %d)",
+             FG_MAX_PSETS, d.n_psets);
+    return FG_ERR_ARG;
+  }
+  for (int i = 0; i < d.n_psets; ++i) {
+    if (const char *why = valid(d.psets[i])) {
+      snprintf(h->err, sizeof(h->err), "parameter set %d: %s", i, why);
+      return FG_ERR_ARG;
+    }
+  }
+  return FG_OK;
+}
+
+// the checked parameter sets into device memory the handle owns; the handle's descriptor points at that copy
+template <class H>
+static inline int fg_upload_psets(H *h) {
+  if (!h->d.psets) return FG_OK;
+  const size_t bytes = sizeof(*h->d.psets) * (size_t)h->d.n_psets;
+  CUDA_TRY(h, cudaMalloc(&h->dev_psets, bytes));
+  CUDA_TRY(h, cudaMemcpy(h->dev_psets, h->d.psets, bytes, cudaMemcpyHostToDevice));
+  h->d.psets = (decltype(h->d.psets))h->dev_psets;
+  return FG_OK;
+}
+
+static inline bool fg_unit_interval(double p) { return p >= 0.0 && p <= 1.0; }   // false for NaN too
+
 template <class H>
 static inline int fg_close(H *h) {
   {
     fg_device_scope on(h);
     if (h && h->dev_classes) cudaFree(h->dev_classes);
+    if (h && h->dev_psets) cudaFree(h->dev_psets);
   }
   delete h;
   return FG_OK;

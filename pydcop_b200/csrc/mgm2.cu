@@ -56,6 +56,12 @@ extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
     snprintf(h->err, sizeof(h->err), "missing device array in the descriptor");
     return FG_ERR_ARG;
   }
+  rc = fg_check_psets(h, [](const fg_mgm2_pset_t &p) -> const char * {
+    if (p.favor < FG_MGM2_FAVOR_UNILATERAL || p.favor > FG_MGM2_FAVOR_COORDINATED)
+      return "favor is not one of unilateral (0), no (1), coordinated (2)";
+    return fg_unit_interval(p.threshold) ? nullptr : "threshold is not in [0, 1]";
+  });
+  if (rc != FG_OK) return rc;
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
   const fg_mgm2_desc_t &d = *desc;
   rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_dom_size), FG_FIELD(d, dev_var_id),
@@ -66,8 +72,9 @@ extern "C" int fg_mgm2_create(const fg_mgm2_desc_t *desc, fg_mgm2_t *out) {
                              FG_FIELD(d, dev_potential_value), FG_FIELD(d, dev_local_cost), FG_FIELD(d, dev_offerer),
                              FG_FIELD(d, dev_partner), FG_FIELD(d, dev_committed), FG_FIELD(d, dev_go),
                              FG_FIELD(d, dev_answer), FG_FIELD(d, dev_answer_value), FG_FIELD(d, dev_answer_gain),
-                             FG_FIELD(d, dev_offer_off), FG_FIELD(d, dev_offer), FG_FIELD(d, dev_var_seed)});
-  if (rc != FG_OK) return rc;
+                             FG_FIELD(d, dev_offer_off), FG_FIELD(d, dev_offer), FG_FIELD(d, dev_var_seed),
+                             FG_FIELD(d, dev_var_pset)});
+  if (rc != FG_OK || (rc = fg_upload_psets(h)) != FG_OK) return rc;
   return fg_upload_classes(h);
 }
 

@@ -198,16 +198,20 @@ __device__ __forceinline__ void mgm2_value_at(int v, const MgmSide &g, const T *
   }
 }
 
-template <typename T>
+// PS: every variable reads its threshold from its parameter set (var_pset); without, the instantiation is the one the
+// runs without sets have always had.  The sharded kernels call mgm2_value_at with the scalar.
+template <typename T, bool PS>
 __global__ void __launch_bounds__(128, 8)
 k_mgm2_value(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ val,
              T *__restrict__ cost, uint8_t *__restrict__ has_cost, T *__restrict__ local_cost,
              T *__restrict__ gain, int32_t *__restrict__ pvalue, uint8_t *__restrict__ offerer,
              int32_t *__restrict__ partner, uint8_t *__restrict__ committed, uint8_t *__restrict__ answer,
              const int64_t *__restrict__ offer_off, T *__restrict__ offer, int mode_max, double threshold,
-             uint64_t seed, uint32_t cycle) {
+             uint64_t seed, uint32_t cycle, const uint16_t *__restrict__ var_pset,
+             const fg_mgm2_pset_t *__restrict__ psets) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= n_vars) return;
+  if (PS) threshold = fg_pset(var_pset, psets, v).threshold;
   mgm2_value_at<T>(v, g, tables, val, cost, has_cost, local_cost, gain, pvalue, offerer, partner, committed, answer,
                    offer_off, offer, mode_max, threshold, seed, cycle);
 }
@@ -291,16 +295,19 @@ __device__ __forceinline__ void mgm2_answer_at(int v, const MgmSide &g, const T 
   answer_gain[acc_u] = best;
 }
 
-template <typename T>
+// PS: every variable reads its favor from its parameter set, as k_mgm2_value
+template <typename T, bool PS>
 __global__ void __launch_bounds__(128)
 k_mgm2_answer(MgmSide g, int n_vars, const T *__restrict__ tables, const int32_t *__restrict__ val,
               const T *__restrict__ local_cost, T *__restrict__ gain, int32_t *__restrict__ pvalue,
               const uint8_t *__restrict__ offerer, int32_t *__restrict__ partner, uint8_t *__restrict__ committed,
               uint8_t *__restrict__ answer, int32_t *__restrict__ answer_value, T *__restrict__ answer_gain,
               const int64_t *__restrict__ offer_off, const T *__restrict__ offer, int mode_max, int favor,
-              uint64_t seed, uint32_t cycle) {
+              uint64_t seed, uint32_t cycle, const uint16_t *__restrict__ var_pset,
+              const fg_mgm2_pset_t *__restrict__ psets) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= n_vars) return;
+  if (PS) favor = fg_pset(var_pset, psets, v).favor;
   mgm2_answer_at<T>(v, g, tables, val, local_cost, gain, pvalue, offerer, partner, committed, answer, answer_value,
                     answer_gain, offer_off, offer, mode_max, favor, seed, cycle);
 }
@@ -428,12 +435,15 @@ static void mgm2_cycle(const fg_mgm2_desc_t &d, const fg_class_t *classes, int64
   const uint32_t cyc = (uint32_t)(done + 1);
   const int n = d.n_vars;
   T *cost = (T *)d.dev_cost, *local = (T *)d.dev_local_cost, *gain = (T *)d.dev_gain;
-  launch(n, 128, k_mgm2_value<T>, g, n, (const T *)d.dev_tables, d.dev_value, cost, d.dev_has_cost, local, gain,
-         d.dev_potential_value, d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_offer_off,
-         (T *)d.dev_offer, d.mode_max, d.threshold, d.seed, cyc);
-  launch(n, 128, k_mgm2_answer<T>, g, n, (const T *)d.dev_tables, d.dev_value, local, gain, d.dev_potential_value,
-         d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer, d.dev_answer_value, (T *)d.dev_answer_gain,
-         d.dev_offer_off, (const T *)d.dev_offer, d.mode_max, d.favor, d.seed, cyc);
+  const bool ps = d.dev_var_pset != nullptr;
+  launch(n, 128, ps ? k_mgm2_value<T, true> : k_mgm2_value<T, false>, g, n, (const T *)d.dev_tables, d.dev_value,
+         cost, d.dev_has_cost, local, gain, d.dev_potential_value, d.dev_offerer, d.dev_partner, d.dev_committed,
+         d.dev_answer, d.dev_offer_off, (T *)d.dev_offer, d.mode_max, d.threshold, d.seed, cyc, d.dev_var_pset,
+         d.psets);
+  launch(n, 128, ps ? k_mgm2_answer<T, true> : k_mgm2_answer<T, false>, g, n, (const T *)d.dev_tables, d.dev_value,
+         local, gain, d.dev_potential_value, d.dev_offerer, d.dev_partner, d.dev_committed, d.dev_answer,
+         d.dev_answer_value, (T *)d.dev_answer_gain, d.dev_offer_off, (const T *)d.dev_offer, d.mode_max, d.favor,
+         d.seed, cyc, d.dev_var_pset, d.psets);
   launch(n, 256, k_mgm2_commit<T>, n, d.dev_offerer, d.dev_answer, d.dev_answer_value, (const T *)d.dev_answer_gain,
          gain, d.dev_potential_value, d.dev_committed);
   launch(n, 256, k_mgm2_gain<T>, g, n, gain, d.dev_potential_value, d.dev_committed, d.dev_partner, d.dev_go,

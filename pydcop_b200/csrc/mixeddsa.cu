@@ -52,6 +52,12 @@ extern "C" int fg_mixeddsa_create(const fg_mixeddsa_desc_t *desc, fg_mixeddsa_t 
     return FG_ERR_ARG;
   }
   h->dmax = mixeddsa_dmax(h->classes.data(), (int)h->classes.size());
+  rc = fg_check_psets(h, [](const fg_mixeddsa_pset_t &p) -> const char * {
+    if (p.variant < FG_DSA_A || p.variant > FG_DSA_C) return "variant is not an FG_DSA_* value";
+    if (!fg_unit_interval(p.proba_hard)) return "proba_hard is not in [0, 1]";
+    return fg_unit_interval(p.proba_soft) ? nullptr : "proba_soft is not in [0, 1]";
+  });
+  if (rc != FG_OK) return rc;
   if ((rc = fg_require_device(h)) != FG_OK) return rc;
   const fg_mixeddsa_desc_t &d = *desc;
   rc = fg_check_resident(h, {FG_FIELD(d, dev_tables), FG_FIELD(d, dev_unary), FG_FIELD(d, dev_unary_off),
@@ -60,8 +66,9 @@ extern "C" int fg_mixeddsa_create(const fg_mixeddsa_desc_t *desc, fg_mixeddsa_t 
                              FG_FIELD(d, dev_soft_end), FG_FIELD(d, dev_nbr_ptr), FG_FIELD(d, dev_nbr_idx),
                              FG_FIELD(d, dev_init_value), FG_FIELD(d, dev_con_opt), FG_FIELD(d, dev_value[0]),
                              FG_FIELD(d, dev_value[1]), FG_FIELD(d, dev_cost), FG_FIELD(d, dev_has_cost),
-                             FG_FIELD(d, dev_h_best), FG_FIELD(d, dev_branch), FG_FIELD(d, dev_var_seed)});
-  if (rc != FG_OK) return rc;
+                             FG_FIELD(d, dev_h_best), FG_FIELD(d, dev_branch), FG_FIELD(d, dev_var_seed),
+                             FG_FIELD(d, dev_var_pset)});
+  if (rc != FG_OK || (rc = fg_upload_psets(h)) != FG_OK) return rc;
   return fg_upload_classes(h);
 }
 

@@ -75,13 +75,16 @@ __device__ __forceinline__ const T *mixeddsa_row(const MgmSide &g, int s, const 
 // One round (_on_neighbors_values :272-373) for every variable; every dom_size of a variable with a constraint is
 // <= DMAX.  `inf` is +infinity in T (the hard test is `entry == INFINITY`, :438).  Writes the next value of every
 // variable to val_out, so nothing read in this launch is written in it.
-template <typename T, int DMAX>
+// PS: every variable reads its probabilities and variant from its parameter set (var_pset); without, the instantiation
+// is the one the runs without sets have always had.
+template <typename T, int DMAX, bool PS>
 __global__ void __launch_bounds__(128)
 k_mixeddsa_step(MgmSide g, int n_vars, const T *__restrict__ tables, const T *__restrict__ unary,
                 const int32_t *__restrict__ soft_end, const T *__restrict__ con_opt, const int32_t *__restrict__ val,
                 int32_t *__restrict__ val_out, T *__restrict__ cost, uint8_t *__restrict__ has_cost,
                 int32_t *__restrict__ h_best, uint8_t *__restrict__ branch, int mode_max, int variant,
-                double proba_hard, double proba_soft, T inf, uint64_t seed, uint32_t cycle) {
+                double proba_hard, double proba_soft, T inf, uint64_t seed, uint32_t cycle,
+                const uint16_t *__restrict__ var_pset, const fg_mixeddsa_pset_t *__restrict__ psets) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= n_vars) return;
   const int cur = val[v];
@@ -141,6 +144,12 @@ k_mixeddsa_step(MgmSide g, int n_vars, const T *__restrict__ tables, const T *__
       if (mode_max ? (c[x] > cb) : (c[x] < cb)) { cb = c[x]; first = x; nbest = 1; }
       else if (c[x] == cb) ++nbest;
     }
+  }
+  if (PS) {   // read where the decision needs them, so they hold no register over the cost loops
+    const fg_mixeddsa_pset_t &p = fg_pset(var_pset, psets, v);
+    variant = p.variant;
+    proba_hard = p.proba_hard;
+    proba_soft = p.proba_soft;
   }
   const int dh = nh[cur] - hb;
   const T dc = c[cur] - cb;
@@ -217,8 +226,12 @@ static void mixeddsa_init(const fg_mixeddsa_desc_t &d, const fg_class_t *classes
 template <typename T, class L>
 static void mixeddsa_cycle(const fg_mixeddsa_desc_t &d, const fg_class_t *classes, int dmax, int64_t done, L &launch) {
   int32_t *vin = d.dev_value[done & 1], *vout = d.dev_value[(done + 1) & 1];
-  launch(d.n_vars, 128, dmax <= 32 ? k_mixeddsa_step<T, 32> : k_mixeddsa_step<T, FG_MAX_DOM>,
+  const bool ps = d.dev_var_pset != nullptr;
+  launch(d.n_vars, 128,
+         dmax <= 32 ? (ps ? k_mixeddsa_step<T, 32, true> : k_mixeddsa_step<T, 32, false>)
+                    : (ps ? k_mixeddsa_step<T, FG_MAX_DOM, true> : k_mixeddsa_step<T, FG_MAX_DOM, false>),
          mixeddsa_side(d, classes), d.n_vars, (const T *)d.dev_tables, (const T *)d.dev_unary, d.dev_soft_end,
          (const T *)d.dev_con_opt, vin, vout, (T *)d.dev_cost, d.dev_has_cost, d.dev_h_best, d.dev_branch, d.mode_max,
-         d.variant, d.proba_hard, d.proba_soft, std::numeric_limits<T>::infinity(), d.seed, (uint32_t)(done + 1));
+         d.variant, d.proba_hard, d.proba_soft, std::numeric_limits<T>::infinity(), d.seed, (uint32_t)(done + 1),
+         d.dev_var_pset, d.psets);
 }

@@ -38,3 +38,11 @@ __host__ __device__ __forceinline__ void philox_draw(uint32_t var, uint32_t cycl
 __host__ __device__ __forceinline__ uint64_t fg_var_seed(const uint64_t *var_seed, int v, uint64_t seed) {
   return var_seed ? var_seed[v] : seed;
 }
+
+// Parameter set of internal variable v: its entry of the set table (a batch of problems, each with its own algorithm
+// parameters; the table is the device copy fg_upload_psets made).  Callers read it only when var_pset is not NULL and
+// take the descriptor's scalars otherwise.
+template <class P>
+__host__ __device__ __forceinline__ const P &fg_pset(const uint16_t *var_pset, const P *psets, int v) {
+  return psets[var_pset[v]];
+}

@@ -104,7 +104,7 @@ def host_state(state):
 
 _TORCH_DTYPES = {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64,
                  np.dtype(np.int32): torch.int32, np.dtype(np.int64): torch.int64, np.dtype(np.uint8): torch.uint8,
-                 np.dtype(np.uint64): torch.uint64}
+                 np.dtype(np.uint64): torch.uint64, np.dtype(np.uint16): torch.uint16}
 
 
 class _EngineBase:
@@ -572,12 +572,15 @@ def dsa_fast_arrays(layout: FactorGraphLayout, tables: torch.Tensor, mode="min")
 
 def dsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", probability=0.7, p_mode="fixed", variant="B",
              stop_cycle=0, seed=0, isolated_value=None, var_global_id=None, frozen=None, var_costs=False,
-             var_seed=None):
+             var_seed=None, var_pset=None, psets=None):
     """DsaEngine's host-array plan for the generic kernels (inputs, state, scalar descriptor fields), as mgm_plan;
     `value` is the double buffer, its second half uploaded as zeros.  The oriented-table and active-row arrays are
     DsaEngine's own.  frozen (canonical order): ghost variables of a shard, has_nbr = 2 (never written by the local
-    kernels); var_costs: A-DSA's var_cost / unary_off."""
+    kernels); var_costs: A-DSA's var_cost / unary_off.  var_pset (canonical order) / psets (checked parameter dicts):
+    the parameter set of every variable of a union; `prob` then holds each variable's own set's probability and
+    p_mode, and the kernels read its variant."""
     L = layout
+    pset = _pset_index(L, var_pset, psets)
     dt = PRECISIONS[precision][2]
     if variant not in _cabi.DSA_VARIANTS:
         raise ValueError(f"invalid variant {variant!r}")
@@ -590,9 +593,13 @@ def dsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", probability
     has_nbr = (n_count > 0).astype(np.uint8)
     if frozen is not None:   # 2 = ghost of another rank's variable: never written by the local kernels
         has_nbr[np.asarray(frozen, dtype=bool)[L.var_order]] = 2
-    if p_mode == "arity":  # dsa.py:257-260: 1 / n_count * 1.2
-        with np.errstate(divide="ignore"):
-            prob = np.where(n_count > 0, 1.0 / np.maximum(n_count, 1) * 1.2, 0.0)
+    with np.errstate(divide="ignore"):   # p_mode arity, dsa.py:257-260: 1 / n_count * 1.2
+        by_count = np.where(n_count > 0, 1.0 / np.maximum(n_count, 1) * 1.2, 0.0)
+    if pset is not None:   # each variable's own set's p_mode and probability
+        by_arity = np.array([p.get("p_mode", "fixed") == "arity" for p in psets])[pset[:L.n_vars]]
+        prob = np.where(by_arity, by_count, np.array([float(p["probability"]) for p in psets])[pset[:L.n_vars]])
+    elif p_mode == "arity":
+        prob = by_count
     else:
         prob = np.full(L.n_vars, float(probability))
     # isolated variables (dsa.py:278-289): argopt of (own cost, value), tuple order
@@ -615,8 +622,10 @@ def dsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", probability
                   unary_off=np.ascontiguousarray(L.unary_off, np.int64) if var_costs else None)
     _set_global_ids(inputs, L, var_global_id, var_seed)
     state = dict(con_opt=(L.n_factors, dt, 0), value_cost=(L.n_vars, dt, 0))
-    return inputs, state, dict(mode_max=int(mode == "max"), variant=_cabi.DSA_VARIANTS[variant],
-                               stop_cycle=int(stop_cycle), seed=_seed(seed))
+    scalars = dict(mode_max=int(mode == "max"), variant=_cabi.DSA_VARIANTS[variant], stop_cycle=int(stop_cycle),
+                   seed=_seed(seed))
+    _set_psets(inputs, scalars, pset, psets, _cabi.FgDsaPset, lambda p: dict(variant=_cabi.DSA_VARIANTS[p["variant"]]))
+    return inputs, state, scalars
 
 
 class DsaEngine(_CycleEngine):
@@ -625,18 +634,21 @@ class DsaEngine(_CycleEngine):
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
                  probability=0.7, p_mode="fixed", variant="B", stop_cycle=0, seed=0,
-                 isolated_value=None, var_global_id=None, frozen=None, var_costs=False, var_seed=None):
+                 isolated_value=None, var_global_id=None, frozen=None, var_costs=False, var_seed=None,
+                 var_pset=None, psets=None):
         """var_costs: A-DSA's decision (pydcop/algorithms/adsa.py:344-377: every candidate value carries the
         variable's own cost, the current cost does not); False: DSA.
         var_global_id / frozen (canonical order) serve the multi-GPU partition
         (pydcop_b200/multigpu_dsa.py): the Philox counter of each variable when the layout is a
         shard of a larger problem, and the ghost variables whose value is only copied through.
         var_seed (canonical order): the Philox key of each variable when the layout holds several problems with
-        seeds of their own (pydcop_b200.batch); default: `seed` for every variable."""
+        seeds of their own (pydcop_b200.batch); default: `seed` for every variable.
+        var_pset / psets: the parameter set of each variable (canonical order) when the layout holds several problems
+        with parameters of their own, as dsa_plan; default: the scalar parameters for every variable."""
         L = layout
         tdt = self._open(layout, device, precision)
         inputs, state, scalars = dsa_plan(L, precision, mode, probability, p_mode, variant, stop_cycle, seed,
-                                          isolated_value, var_global_id, frozen, var_costs, var_seed)
+                                          isolated_value, var_global_id, frozen, var_costs, var_seed, var_pset, psets)
         self.has_nbr_host = inputs["has_nbr"]
         value0, _ = inputs.pop("value")
         t = self._upload(inputs, state)
@@ -770,6 +782,31 @@ def _set_global_ids(inputs, layout, var_global_id, var_seed=None):
     return inputs
 
 
+def _pset_index(layout, var_pset, psets):
+    """var_pset (canonical order): the parameter set of every variable, an index into `psets` (a list of checked
+    parameter dicts), as uint16 in internal order; None when neither is given."""
+    if var_pset is None and psets is None:
+        return None
+    if var_pset is None or psets is None or not 1 <= len(psets) <= _cabi.FG_MAX_PSETS:
+        raise ValueError(f"var_pset and psets go together, with 1 to {_cabi.FG_MAX_PSETS} parameter sets")
+    vp = np.asarray(var_pset, dtype=np.int64)
+    if vp.shape != (layout.n_vars,) or (vp < 0).any() or (vp >= len(psets)).any():
+        raise ValueError(f"var_pset must hold one index into the {len(psets)} parameter sets per variable")
+    return _per_var(layout, vp[layout.var_order], np.uint16)
+
+
+def _set_psets(inputs, scalars, index, psets, struct, fields):
+    """Add a union's parameter sets to a plan: `index` (_pset_index) as dev_var_pset, and the host table of `struct`
+    (fields(params) -> its field values) as psets / n_psets.  Nothing without an index: the plan is the plan of the
+    scalar parameters."""
+    if index is None:
+        return inputs, scalars
+    inputs["var_pset"] = index
+    table = (struct * len(psets))(*[struct(**fields(p)) for p in psets])
+    scalars.update(psets=table, n_psets=len(psets))   # a descriptor holding the table keeps it alive (ctypes)
+    return inputs, scalars
+
+
 def mgm_plan(layout: FactorGraphLayout, precision="f32", mode="min", stop_cycle=0, seed=0, var_rank=None,
              isolated_value=None, var_global_id=None, var_seed=None):
     """MgmEngine's host-array plan: (inputs: name -> array in its final dtype, in upload order; state: name ->
@@ -899,11 +936,12 @@ def mgm2_offer_offsets(layout: FactorGraphLayout, nbr_ptr, nbr_idx):
 
 
 def mgm2_plan(layout: FactorGraphLayout, precision="f32", mode="min", threshold=0.5, favor="unilateral",
-              stop_cycle=0, seed=0, var_rank=None, var_global_id=None, var_seed=None):
+              stop_cycle=0, seed=0, var_rank=None, var_global_id=None, var_seed=None, var_pset=None, psets=None):
     """Mgm2Engine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan.  var_global_id (canonical
     order): the Philox counter of every variable when the layout is a shard of a larger problem; var_seed as
-    mgm_plan."""
+    mgm_plan; var_pset / psets as dsa_plan (the kernels read each variable's threshold and favor)."""
     L = layout
+    pset = _pset_index(L, var_pset, psets)
     dt = PRECISIONS[precision][2]
     h = mgm_host_arrays(L, mode, var_rank)
     offer_off, offer_size = mgm2_offer_offsets(L, h["nbr_ptr"], h["nbr_idx"])
@@ -915,8 +953,11 @@ def mgm2_plan(layout: FactorGraphLayout, precision="f32", mode="min", threshold=
                  answer_gain=(n, dt, 0), has_cost=(n, np.uint8, 0), offerer=(n, np.uint8, 0),
                  committed=(n, np.uint8, 0), go=(n, np.uint8, 0), answer=(n, np.uint8, 0),
                  offer=(offer_size, dt, 0))
-    return inputs, state, dict(mode_max=int(mode == "max"), favor=_cabi.MGM2_FAVORS[favor], threshold=float(threshold),
-                               stop_cycle=int(stop_cycle or 0), seed=_seed(seed))
+    scalars = dict(mode_max=int(mode == "max"), favor=_cabi.MGM2_FAVORS[favor], threshold=float(threshold),
+                   stop_cycle=int(stop_cycle or 0), seed=_seed(seed))
+    _set_psets(inputs, scalars, pset, psets, _cabi.FgMgm2Pset,
+               lambda p: dict(threshold=float(p["threshold"]), favor=_cabi.MGM2_FAVORS[p["favor"]]))
+    return inputs, state, scalars
 
 
 class Mgm2Engine(_LocalSearchEngine):
@@ -930,6 +971,7 @@ class Mgm2Engine(_LocalSearchEngine):
     var_global_id  canonical order: the Philox counter of each variable when the layout is one rank's shard
                of a larger problem (pydcop_b200/multigpu_mgm2.py; default: the canonical index)
     var_seed   canonical order: the Philox key of each variable, as MgmEngine (default: `seed` for every variable)
+    var_pset, psets  the parameter set of each variable (canonical order) and the sets, as DsaEngine
     Variable costs are not part of MGM-2's costs (assignment_cost without them); a variable without
     neighbours takes a drawn value among its best over its unary constraints on the device.
     """
@@ -937,7 +979,7 @@ class Mgm2Engine(_LocalSearchEngine):
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min",
                  threshold=0.5, favor="unilateral", stop_cycle=0, seed=0, var_rank=None, var_global_id=None,
-                 var_seed=None):
+                 var_seed=None, var_pset=None, psets=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -945,7 +987,7 @@ class Mgm2Engine(_LocalSearchEngine):
         if favor not in _cabi.MGM2_FAVORS:
             raise ValueError(f"invalid favor {favor!r}: expected one of {sorted(_cabi.MGM2_FAVORS)}")
         inputs, state, scalars = mgm2_plan(L, precision, mode, threshold, favor, stop_cycle, seed, var_rank,
-                                           var_global_id, var_seed)
+                                           var_global_id, var_seed, var_pset, psets)
         self.nbr_ptr_host, self.nbr_idx_host = inputs["nbr_ptr"], inputs["nbr_idx"]
         self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
         self.offer_bytes = state["offer"][0] * np.dtype(self.np_dtype).itemsize
@@ -1083,13 +1125,18 @@ def gdba_modifiers_view(h, mods, base_mod, increase_mode):
 
 
 def gdba_plan(layout: FactorGraphLayout, precision="f32", mode="min", modifier="A", violation="NZ", increase_mode="E",
-              stop_cycle=0, seed=0, var_rank=None, isolated_value=None, var_global_id=None, var_seed=None):
+              stop_cycle=0, seed=0, var_rank=None, isolated_value=None, var_global_id=None, var_seed=None,
+              var_pset=None, psets=None):
     """GdbaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
-    buffer, and viol_ref / mod_off are None where the modes do not read them."""
+    buffer, and viol_ref / mod_off are None where the modes do not read them.  var_pset / psets as dsa_plan (the
+    kernels read each variable's modifier and violation mode; a factor's viol_ref is its variables' set's)."""
     L = layout
     dt = PRECISIONS[precision][2]
+    pset = _pset_index(L, var_pset, psets)
     h = mgm_host_arrays(L, mode, var_rank, isolated_value)
     g = gdba_host_arrays(L, h["nbr_ptr"], increase_mode, violation)
+    if pset is not None:
+        g["viol_ref"] = _gdba_viol_ref(L, pset, [p["violation"] for p in psets])
     nb = _neighbourhood_inputs(L, dt, h)
     value0 = _per_var(L, h["value0"], np.int32)
     inputs = dict(tables=nb.pop("tables"), unary=np.ascontiguousarray(L.unary, dt),
@@ -1101,10 +1148,30 @@ def gdba_plan(layout: FactorGraphLayout, precision="f32", mode="min", modifier="
     n = L.n_vars
     state = dict(improve=(n, dt, 0), new_value=(n, np.int32, 0), breakout=(n, np.uint8, 0),
                  violated=(L.n_edges, np.uint8, 0), mod=(g["mod_size"], np.int32, 0))
-    return inputs, state, dict(mode_max=int(mode == "max"), modifier=_cabi.GDBA_MODIFIERS[modifier],
-                               violation=_cabi.GDBA_VIOLATIONS[violation],
-                               increase_mode=_cabi.GDBA_INCREASE_MODES[increase_mode], mod_size=g["mod_size"],
-                               stop_cycle=int(stop_cycle or 0), seed=_seed(seed))
+    scalars = dict(mode_max=int(mode == "max"), modifier=_cabi.GDBA_MODIFIERS[modifier],
+                   violation=_cabi.GDBA_VIOLATIONS[violation], increase_mode=_cabi.GDBA_INCREASE_MODES[increase_mode],
+                   mod_size=g["mod_size"], stop_cycle=int(stop_cycle or 0), seed=_seed(seed))
+    _set_psets(inputs, scalars, pset, psets, _cabi.FgGdbaPset,
+               lambda p: dict(modifier=_cabi.GDBA_MODIFIERS[p["modifier"]],
+                              violation=_cabi.GDBA_VIOLATIONS[p["violation"]]))
+    return inputs, state, scalars
+
+
+def _gdba_viol_ref(layout, pset, violations):
+    """viol_ref of a union whose variables have parameter sets (pset: internal order, violations: each set's mode):
+    per internal factor, the min (NM) or max (MX) of its base table by the set of its first variable (every variable of
+    a factor is of one problem, so of one set); None when every set is NZ."""
+    L = layout
+    code = np.array([_cabi.GDBA_VIOLATIONS[v] for v in violations])
+    if not L.n_factors or not code.any():
+        return None
+    out = np.zeros(L.n_factors, dtype=np.float64)
+    for c in L.classes:
+        t = L.tables[c.table_base:c.table_base + c.n_factors * c.table_size].reshape(c.n_factors, c.table_size)
+        first = L.edge_var[c.first_edge + np.arange(c.n_factors, dtype=np.int64) * c.arity]
+        mx = code[pset[first]] == _cabi.GDBA_VIOLATIONS["MX"]
+        out[c.first_factor:c.first_factor + c.n_factors] = np.where(mx, t.max(1), t.min(1))
+    return out
 
 
 class GdbaEngine(_LocalSearchEngine):
@@ -1122,12 +1189,14 @@ class GdbaEngine(_LocalSearchEngine):
                    default: argopt of the own cost with ties broken on the value index
     var_global_id  canonical order: the Philox counter of each variable (default: the canonical index), as MgmEngine
     var_seed       canonical order: the Philox key of each variable (default: `seed` for every variable), as MgmEngine
+    var_pset, psets  the parameter set of each variable (canonical order) and the sets, as DsaEngine; `modifiers()`
+                   reads with the scalar modifier's base
     """
     FAMILY = "gdba"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", modifier="A",
                  violation="NZ", increase_mode="E", stop_cycle=0, seed=0, var_rank=None, isolated_value=None,
-                 var_global_id=None, var_seed=None):
+                 var_global_id=None, var_seed=None, var_pset=None, psets=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -1139,7 +1208,7 @@ class GdbaEngine(_LocalSearchEngine):
                 raise ValueError(f"invalid {name} {v!r}: expected one of {sorted(ok)}")
         self.modifier, self.violation, self.increase_mode = modifier, violation, increase_mode
         inputs, state, scalars = gdba_plan(L, precision, mode, modifier, violation, increase_mode, stop_cycle, seed,
-                                           var_rank, isolated_value, var_global_id, var_seed)
+                                           var_rank, isolated_value, var_global_id, var_seed, var_pset, psets)
         self.nbr_ptr_host = inputs["nbr_ptr"]
         self.has_nbr_host = np.diff(self.nbr_ptr_host) > 0
         self.modifier_bytes = scalars["mod_size"] * 4
@@ -1325,10 +1394,12 @@ def mixeddsa_slots(layout: FactorGraphLayout, hard):
 
 
 def mixeddsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", proba_hard=0.7, proba_soft=0.5, variant="B",
-                  stop_cycle=0, seed=0, var_global_id=None, var_seed=None):
+                  stop_cycle=0, seed=0, var_global_id=None, var_seed=None, var_pset=None, psets=None):
     """MixedDsaEngine's host-array plan (inputs, state, scalar descriptor fields), as mgm_plan; `value` is the double
-    buffer, `slot_edge` the soft-then-hard slot order of mixeddsa_slots, `con_opt` written by fg_mixeddsa_init."""
+    buffer, `slot_edge` the soft-then-hard slot order of mixeddsa_slots, `con_opt` written by fg_mixeddsa_init.
+    var_pset / psets as dsa_plan (the kernels read each variable's probabilities and variant)."""
     L = layout
+    pset = _pset_index(L, var_pset, psets)
     dt = PRECISIONS[precision][2]
     with np.errstate(over="ignore"):     # an f64 entry above the f32 range becomes inf: hard in f32 (mixeddsa.py:219)
         tables = np.ascontiguousarray(L.tables, dt)
@@ -1346,9 +1417,12 @@ def mixeddsa_plan(layout: FactorGraphLayout, precision="f32", mode="min", proba_
     n = L.n_vars
     state = dict(con_opt=(L.n_factors, dt, 0), cost=(n, dt, 0), has_cost=(n, np.uint8, 0),
                  h_best=(n, np.int32, -1), branch=(n, np.uint8, 0))
-    return inputs, state, dict(proba_hard=float(proba_hard), proba_soft=float(proba_soft), mode_max=int(mode == "max"),
-                               variant=_cabi.MIXEDDSA_VARIANTS[variant], stop_cycle=int(stop_cycle or 0),
-                               seed=_seed(seed))
+    scalars = dict(proba_hard=float(proba_hard), proba_soft=float(proba_soft), mode_max=int(mode == "max"),
+                   variant=_cabi.MIXEDDSA_VARIANTS[variant], stop_cycle=int(stop_cycle or 0), seed=_seed(seed))
+    _set_psets(inputs, scalars, pset, psets, _cabi.FgMixedDsaPset,
+               lambda p: dict(proba_hard=float(p["proba_hard"]), proba_soft=float(p["proba_soft"]),
+                              variant=_cabi.MIXEDDSA_VARIANTS[p["variant"]]))
+    return inputs, state, scalars
 
 
 class MixedDsaEngine(_LocalSearchEngine):
@@ -1362,13 +1436,15 @@ class MixedDsaEngine(_LocalSearchEngine):
     stop_cycle  0 = run forever; else the run ends after stop_cycle rounds (dsa_gpu's convention, dsa.py:352)
     var_global_id  canonical order: the Philox counter of each variable (default: the canonical index), as MgmEngine
     var_seed    canonical order: the Philox key of each variable (default: `seed` for every variable), as MgmEngine
+    var_pset, psets  the parameter set of each variable (canonical order) and the sets, as DsaEngine
     `values()` reports the cost of the last move (inf while a hard constraint stays violated), NaN before the first
     one; `record()` the best H and the branch of the last round.
     """
     FAMILY = "mixeddsa"
 
     def __init__(self, layout: FactorGraphLayout, device=None, precision="f32", mode="min", proba_hard=0.7,
-                 proba_soft=0.5, variant="B", stop_cycle=0, seed=0, var_global_id=None, var_seed=None):
+                 proba_soft=0.5, variant="B", stop_cycle=0, seed=0, var_global_id=None, var_seed=None,
+                 var_pset=None, psets=None):
         L = layout
         self._open(layout, device, precision)
         if mode not in ("min", "max"):
@@ -1378,7 +1454,7 @@ class MixedDsaEngine(_LocalSearchEngine):
         if int(stop_cycle or 0) < 0:
             raise ValueError(f"invalid stop_cycle {stop_cycle!r}: must be >= 0")
         inputs, state, scalars = mixeddsa_plan(L, precision, mode, proba_hard, proba_soft, variant, stop_cycle, seed,
-                                               var_global_id, var_seed)
+                                               var_global_id, var_seed, var_pset, psets)
         t = self._upload(inputs, state)
         self.__dict__.update(t)
         self._classes = _class_array(L)
@@ -1667,17 +1743,22 @@ class SyncbbEngine(_EngineBase):
 
 
 def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precision="f32", device=None, seed=0,
-                var_rank=None, isolated_value=None, tree=None, var_global_id=None, var_seed=None):
+                var_rank=None, isolated_value=None, tree=None, var_global_id=None, var_seed=None, var_pset=None,
+                psets=None):
     """The single-GPU engine of algorithm `kind` (a value of solve.ALGOS) over `layout`.  `params`: its algorithm
     parameters, the missing ones taking solve.DEFAULTS; var_rank / isolated_value / var_global_id in canonical order
     as the engines take them (var_rank None: the canonical index; var_global_id None: the canonical index as every
     Philox counter, ignored by the families without draws: MaxSum, DPOP, SyncBB); var_seed in canonical order: the
     Philox key of every variable (None: `seed` for all; DBA, MaxSum, DPOP and SyncBB take none and refuse one);
+    var_pset / psets: the parameter set of every variable (canonical order) and the sets (checked parameter dicts)
+    for DSA, A-DSA, MGM-2, GDBA and MixedDSA (None: `params` for all; the other families refuse them).
     tree: DPOP's pseudo-tree.  MaxSum records no sent flags."""
     from .solve import DEFAULTS
     p = dict(DEFAULTS[kind], **params)
     if var_seed is not None and kind in ("syncbb", "dba", "dpop", "maxsum"):
         raise ValueError(f"{kind} takes no per-variable seeds")
+    if (var_pset is not None or psets is not None) and kind in ("syncbb", "dba", "dpop", "maxsum", "mgm"):
+        raise ValueError(f"{kind} takes no per-variable parameter sets")
     if kind == "syncbb":
         return SyncbbEngine(layout, device=device, precision=precision, mode=mode, var_rank=var_rank)
     if kind == "dba":
@@ -1688,16 +1769,16 @@ def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precisio
     if kind == "mixeddsa":
         return MixedDsaEngine(layout, device=device, precision=precision, mode=mode, proba_hard=p["proba_hard"],
                               proba_soft=p["proba_soft"], variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed,
-                              var_global_id=var_global_id, var_seed=var_seed)
+                              var_global_id=var_global_id, var_seed=var_seed, var_pset=var_pset, psets=psets)
     if kind == "gdba":
         return GdbaEngine(layout, device=device, precision=precision, mode=mode, modifier=p["modifier"],
                           violation=p["violation"], increase_mode=p["increase_mode"], stop_cycle=p["stop_cycle"],
                           seed=seed, var_rank=var_rank, isolated_value=isolated_value, var_global_id=var_global_id,
-                          var_seed=var_seed)
+                          var_seed=var_seed, var_pset=var_pset, psets=psets)
     if kind == "mgm2":
         return Mgm2Engine(layout, device=device, precision=precision, mode=mode, threshold=p["threshold"],
                           favor=p["favor"], stop_cycle=p["stop_cycle"], seed=seed, var_rank=var_rank,
-                          var_global_id=var_global_id, var_seed=var_seed)
+                          var_global_id=var_global_id, var_seed=var_seed, var_pset=var_pset, psets=psets)
     if kind == "mgm":
         return MgmEngine(layout, device=device, precision=precision, mode=mode, stop_cycle=p["stop_cycle"], seed=seed,
                          break_mode=p["break_mode"], var_rank=var_rank, isolated_value=isolated_value,
@@ -1709,4 +1790,4 @@ def make_engine(kind, layout: FactorGraphLayout, params, *, mode="min", precisio
     return DsaEngine(layout, device=device, precision=precision, mode=mode, probability=p["probability"],
                      p_mode=p.get("p_mode", "fixed"), variant=p["variant"], stop_cycle=p["stop_cycle"], seed=seed,
                      isolated_value=isolated_value, var_global_id=var_global_id, var_seed=var_seed,
-                     var_costs=(kind == "adsa"))   # A-DSA: candidates carry own costs
+                     var_costs=(kind == "adsa"), var_pset=var_pset, psets=psets)   # A-DSA: candidates carry own costs

@@ -424,12 +424,20 @@ class _Trace:
 
 
 BATCHED = ("maxsum", "dsa", "adsa", "mgm", "mgm2", "gdba", "mixeddsa")
+# the parameters problems of one engine may differ in: read per variable through a parameter set (DSA, A-DSA, MGM-2,
+# GDBA, MixedDSA), drawn per problem when the union is built (MaxSum's noise), or never read by the engine (A-DSA's
+# period, MGM's break_mode); every other parameter is one scalar per engine and splits groups
+IN_UNION = {"dsa": ("probability", "p_mode", "variant"), "adsa": ("period", "probability", "variant"),
+            "mgm": ("break_mode",), "mgm2": ("threshold", "favor"), "gdba": ("modifier", "violation"),
+            "mixeddsa": ("proba_hard", "proba_soft", "variant"), "maxsum": ("noise",)}
+ENGINE_PSETS = ("dsa", "adsa", "mgm2", "gdba", "mixeddsa")   # the families whose engines take parameter sets
 NOT_BATCHED = {"dba": "it stops per problem by itself, so each problem would need its own finish cycle",
                "dpop": "it computes over a pseudo-tree of the whole problem",
                "syncbb": "it searches over an order of the whole problem"}
 
 
-def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = None, timeout: Optional[float] = None,
+def solve_batch(problems, algo: str, algo_params: Union[None, Dict[str, Any], Sequence] = None,
+                timeout: Optional[float] = None,
                 precision: str = "f32", device=None, seed: Union[None, int, Sequence[int]] = None,
                 infinity: float = float("inf"),
                 chunk: int = 50, max_vars: int = batch.MAX_BATCH_VARS,
@@ -448,21 +456,34 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
               per problem: problem i's result is then solve(problems[i], ..., seed=seed[i])'s.  With it the same
               problem can appear many times, once per seed, to compare runs of a stochastic algorithm (pydcop
               batch's iterations); a DcopArrays entry is not re-parsed.
+    algo_params  None or a dict: one set of parameters for every problem; or a sequence with one dict (or None) per
+              problem: problem i's result is then solve(problems[i], algo, algo_params[i], ...)'s (pydcop batch's
+              parameter combinations).  The parameters IN_UNION names run in one engine, each variable reading its
+              problem's set; problems that differ in another parameter (stop_cycle, MaxSum's damping, GDBA's
+              increase_mode, ...) run in separate groups.
     `timeout` bounds the whole batch: a problem whose group has not reached stop_cycle when it expires reports
     TIMEOUT at the cycle its group reached (0 for groups that had not started).
     `time` and `ingest_time` are the whole batch's (loading, unions, layouts and engines for ingest_time);
     `h2d_bytes` is the problem's engine's.  `n_gpus` is 1: a batch runs on one device, never under torchrun.
     algo: maxsum | dsa | adsa | mgm | mgm2 | gdba | mixeddsa (the fixed-length families; dba, dpop and syncbb are
-    refused).  engine_factory(kind, layout, inst, params): as in solve(), `inst` with var_rank, var_global_id and
-    var_seed (None when the group's problems share one seed, params["seed"]).
+    refused).  engine_factory(kind, layout, inst, params): as in solve(), `inst` with var_rank, var_global_id,
+    var_seed (None when the group's problems share one seed, params["seed"]) and var_pset (None when they share one
+    parameter set; else the group's sets are params["psets"]).
     trace: every result gains solve()'s "trace", cut out of its group's per-problem record (its times are the
     group's); the trace of a problem whose group never started is empty.
     """
     kind = ALGOS.get(algo)
     if kind in NOT_BATCHED:
         raise ValueError(f"{kind} is not batched: {NOT_BATCHED[kind]}")
-    kind, params, stop_cycle = _algorithm(algo, algo_params, timeout)
     problems = list(problems)
+    if kind is None:
+        _algorithm(algo, None, timeout)   # unknown algorithm
+    if algo_params is None or isinstance(algo_params, dict):
+        kind, params, stop_cycle = _algorithm(algo, algo_params, timeout)
+        per_problem = None
+    else:
+        per_problem = _batch_params(algo, algo_params, timeout, len(problems))
+        kind, params, stop_cycle = per_problem[0] if per_problem else _algorithm(algo, None, timeout)
     if not problems:
         raise ValueError("solve_batch needs at least one problem")
     seeds = _batch_seeds(seed, len(problems))
@@ -479,28 +500,40 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
         batch.check_problem(i, dcops[-1])
     results: List[Optional[Dict[str, Any]]] = [None] * len(dcops)
     ingest_time = time.perf_counter() - t0
-    noise = params["noise"] if kind == "maxsum" else 0.0
-    for members in batch.groups(dcops, max_vars):
+    keys = sets = None
+    if per_problem is not None:
+        checked = [p for _, p, _ in per_problem]
+        keys = [batch.pset_key({k: v for k, v in p.items() if k not in IN_UNION[kind]}) for p in checked]
+        sets = [batch.pset_key(p) for p in checked]
+    for members in batch.groups(dcops, max_vars, keys, sets):
         t_group = time.perf_counter()
         mode = dcops[members[0]].objective
+        group_params = None if per_problem is None else [per_problem[i][1] for i in members]
+        if group_params is not None:
+            params, stop_cycle = group_params[0], per_problem[members[0]][2]
+        noise = ([p["noise"] for p in group_params] if group_params is not None else params["noise"]) \
+            if kind == "maxsum" else 0.0
         if engine_factory is not None:
             var_inputs = lambda d: (name_rank(d), None)  # noqa: E731
         else:
             var_inputs = lambda d: _var_inputs(kind, d, mode)  # noqa: E731
-        u = batch.build_union(dcops, members, var_inputs, noise, [seeds[i] for i in members])
+        u = batch.build_union(dcops, members, var_inputs, noise, [seeds[i] for i in members], group_params)
         layout = batch.union_layout(u, dcops)
         # one seed for the whole group: the scalar key, as solve() runs; else each variable's own (u.var_seed)
         group_seed = seeds[members[0]] or 0
         var_seed = None if kind == "maxsum" else u.var_seed   # MaxSum draws nothing on the device: its noise is in u
+        # one parameter set for the whole group: the scalars; else each variable's own set (u.var_pset)
+        var_pset = u.var_pset if kind in ENGINE_PSETS else None
+        psets = u.psets if var_pset is not None else None
         if engine_factory is not None:
             engine = engine_factory(kind, layout, dict(u.inst, var_rank=u.var_rank, var_global_id=u.var_global_id,
-                                                       var_seed=var_seed),
-                                    dict(params, mode=mode, seed=group_seed))
+                                                       var_seed=var_seed, var_pset=var_pset),
+                                    dict(params, mode=mode, seed=group_seed, **({"psets": psets} if psets else {})))
         else:
             from .engine import make_engine
             engine = make_engine(kind, layout, params, mode=mode, precision=precision, device=device, seed=group_seed,
                                  var_rank=u.var_rank, isolated_value=u.isolated_value, var_global_id=u.var_global_id,
-                                 var_seed=var_seed)
+                                 var_seed=var_seed, var_pset=var_pset, psets=psets)
         ingest_time += time.perf_counter() - t_group
         engine.init()
         tracer = None
@@ -531,6 +564,27 @@ def solve_batch(problems, algo: str, algo_params: Optional[Dict[str, Any]] = Non
     for r in results:
         r.update(time=total, ingest_time=ingest_time)
     return results
+
+
+def _batch_params(algo, algo_params, timeout, n: int) -> list:
+    """solve_batch's per-problem `algo_params`: (kind, checked parameters, stop_cycle) of every problem, each dict
+    through _algorithm, errors prefixed with the problem's index."""
+    try:
+        entries = list(algo_params)
+    except TypeError:
+        raise ValueError(f"algo_params must be a dict or a sequence of dicts, got {type(algo_params).__name__}") \
+            from None
+    if len(entries) != n:
+        raise ValueError(f"algo_params: {len(entries)} parameter dicts for {n} problems")
+    out = []
+    for i, p in enumerate(entries):
+        if p is not None and not isinstance(p, dict):
+            raise ValueError(f"problem {i}: algo_params must be a dict or None, got {type(p).__name__}")
+        try:
+            out.append(_algorithm(algo, p, timeout))
+        except ValueError as e:
+            raise ValueError(f"problem {i}: {e}") from e
+    return out
 
 
 def _batch_seeds(seed, n: int) -> list:
@@ -614,9 +668,16 @@ def main(argv=None):
                     help="with --batch: solve every file N times, with seeds --seed + r for r = 0..N-1 (--seed "
                          "defaults to 0 here), as `pydcop batch` iterations; the list is file-major and every entry "
                          "carries \"iteration\" and \"seed\"")
+    ap.add_argument("--sweep", action="append", default=[], metavar="name:v1,v2,...",
+                    help="with --batch: solve every file once per combination of the swept parameters' values, as "
+                         "`pydcop batch` expands its algo_params lists (names sorted, each value list sorted as "
+                         "strings); the list is file-major, then combination, then iteration, and every entry carries "
+                         "its checked \"algo_params\"")
     args = ap.parse_args(argv)
     if args.iterations is not None and not args.batch:
         ap.error("--iterations needs --batch")
+    if args.sweep and not args.batch:
+        ap.error("--sweep needs --batch")
     if args.iterations is not None and args.iterations < 1:
         ap.error("--iterations must be >= 1")
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -624,7 +685,7 @@ def main(argv=None):
     if args.batch:
         if args.run_metrics or args.save or world > 1:
             ap.error("--batch runs on one GPU and takes neither --run_metrics, --save nor torchrun")
-        return _main_batch(args, _algo_params(ap, args))
+        return _main_batch(args, _algo_params(ap, args), _sweeps(ap, args))
     trace = args.collect_on == "cycle_change"
     if world > 1:   # launched by torchrun: one process per GPU over NCCL
         import torch
@@ -677,7 +738,29 @@ def _algo_params(ap, args):
     return params
 
 
-def _main_batch(args, params):
+def _sweeps(ap, args):
+    """--sweep name:v1,v2,... as [(name, [values])], names sorted and every value list sorted as strings (pydcop
+    batch's parameters_configuration); a name also given to -p, twice, or without values is an argparse error."""
+    fixed = {p.split(":", 1)[0] for p in args.algo_params}
+    out = {}
+    for s in args.sweep:
+        if ":" not in s:
+            ap.error(f"--sweep must be name:v1,v2,..., got {s!r}")
+        k, vs = s.split(":", 1)
+        values = [v for v in vs.split(",") if v != ""]
+        if not values:
+            ap.error(f"--sweep {k}: no values")
+        if k in fixed:
+            ap.error(f"parameter {k} is given to both -p and --sweep")
+        if k in out:
+            ap.error(f"--sweep {k} is given twice")
+        out[k] = sorted(values)
+    return sorted(out.items())
+
+
+def _main_batch(args, params, sweeps=()):
+    if sweeps:
+        return _main_sweep(args, params, sweeps)
     if args.iterations is None:
         res = solve_batch(args.dcop_files, args.algo, params, args.timeout, args.precision, seed=args.seed,
                           infinity=args.infinity, trace=args.collect_on == "cycle_change")
@@ -695,6 +778,31 @@ def _main_batch(args, params):
     for r in res:
         if args.no_assignment:
             r.pop("assignment")
+    print(json.dumps(res, indent=2, sort_keys=True, default=str))
+    return 0
+
+
+def _main_sweep(args, params, sweeps):
+    """--batch --sweep: every file x every combination x every iteration (--iterations, default 1) in one
+    solve_batch call, each problem with its own parameters and seed."""
+    import itertools
+    names = [k for k, _ in sweeps]
+    combos = [dict(params, **dict(zip(names, vs))) for vs in itertools.product(*(v for _, v in sweeps))]
+    n = args.iterations or 1
+    base = (args.seed or 0) if args.iterations else args.seed
+    dcops = [load(path, base) for path in args.dcop_files]
+    entries = [(f, c, r) for f in range(len(dcops)) for c in range(len(combos)) for r in range(n)]
+    seeds = [base + r for _, _, r in entries] if args.iterations else args.seed
+    res = solve_batch([dcops[f] for f, _, _ in entries], args.algo, [combos[c] for _, c, _ in entries],
+                      args.timeout, args.precision, seed=seeds, infinity=args.infinity,
+                      trace=args.collect_on == "cycle_change")
+    checked = [check_params(ALGOS[args.algo], c) for c in combos]
+    for (f, c, r), out in zip(entries, res):
+        out.update(problem=args.dcop_files[f], algo_params=checked[c])
+        if args.iterations:
+            out.update(iteration=r, seed=base + r)
+        if args.no_assignment:
+            out.pop("assignment")
     print(json.dumps(res, indent=2, sort_keys=True, default=str))
     return 0
 

@@ -6,7 +6,7 @@ Workload: `--problems` (default 1000) random binary problems of pyDcop-benchmark
 with integer costs 0..9, no variable costs), `stop_cycle` 100, f32 by default.
 
     python tools/batch_throughput.py [--problems N] [--subset S] [--families maxsum,dsa,...] [--precision f32|f64]
-                                     [--seeds R]
+                                     [--seeds R] [--sweep P [--repeats K]]
 
 Per family, one JSON line: problems/s of sequential solve() calls, timed on the first `--subset` problems (default 50;
 the subset size is in the line), problems/s of solve_batch() over all N problems, the speed-up, and whether the batch's
@@ -18,6 +18,13 @@ there is no CPU path.
 With `--seeds R` the workload is a seed sweep instead (pydcop batch's iterations): the first generated problem run R
 times with seeds `--seed` + r, as R sequential solve() calls (timed on the first `--subset` seeds) against one
 solve_batch() with one seed per run; the line reports runs/s of each and whether the subset's results are equal.
+
+With `--sweep P` the workload is a parameter sweep (pydcop batch's parameter combinations): the N problems times P
+parameter sets of the family (SWEEPS), run three ways: one solve_batch() with one parameter dict per problem, P
+solve_batch() calls (one per set), and sequential solve() calls on the first `--subset` (problem, set) pairs.  The arms
+run in turn, rotated over `--repeats` rounds; the line reports every arm's problems/s (the best round), the speed-up of
+the one call over the P calls, and whether all three agree (the one call on every problem with the P calls, and on the
+subset with solve()).
 """
 import argparse
 import json
@@ -31,6 +38,19 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from gdba_throughput import power_limit_w  # noqa: E402
 
 FAMILIES = ("maxsum", "dsa", "adsa", "mgm", "mgm2", "gdba", "mixeddsa")
+
+
+def _spread(lo, hi, p):
+    return [round(lo + (hi - lo) * k / max(p - 1, 1), 6) for k in range(p)]
+
+
+# --sweep P: the parameter sets of each family, all inside one union
+SWEEPS = {"dsa": lambda p: [{"probability": x} for x in _spread(0.1, 0.9, p)],
+          "adsa": lambda p: [{"probability": x} for x in _spread(0.1, 0.9, p)],
+          "mgm2": lambda p: [{"threshold": x} for x in _spread(0.1, 0.9, p)],
+          "gdba": lambda p: [{"modifier": "AM"[k % 2], "violation": ("NZ", "NM", "MX")[k // 2 % 3]} for k in range(p)],
+          "mixeddsa": lambda p: [{"proba_hard": x} for x in _spread(0.1, 0.9, p)],
+          "maxsum": lambda p: [{"noise": x} for x in _spread(0.0, 0.05, p)]}
 
 
 def problems(n, seed=0):
@@ -54,6 +74,9 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=0, help="the problems' generator seed and the runs' seed")
     ap.add_argument("--seeds", type=int, default=0, metavar="R",
                     help="seed sweep: one problem solved with R seeds (--seed + r) instead of --problems problems")
+    ap.add_argument("--sweep", type=int, default=0, metavar="P",
+                    help="parameter sweep: every problem with P parameter sets, one call against P calls")
+    ap.add_argument("--repeats", type=int, default=2, help="--sweep: rounds of the three arms")
     args = ap.parse_args(argv)
     families = args.families.split(",")
     for f in families:
@@ -61,6 +84,11 @@ def main(argv=None):
             ap.error(f"unknown family {f!r}: expected some of {','.join(FAMILIES)}")
     if args.seeds > 0:
         return sweep(args, families)
+    if args.sweep > 0:
+        bad = [f for f in families if f not in SWEEPS]
+        if bad:
+            ap.error(f"--sweep: no parameter sweep for {','.join(bad)}")
+        return param_sweep(args, families)
     subset = min(args.subset, args.problems)
     dcops = problems(args.problems, args.seed)
 
@@ -128,6 +156,62 @@ def sweep(args, families):
                           "equal_on_subset": all(_same(r, s) for r, s in zip(res[:subset], seq)),
                           "distinct_assignments": len({tuple(sorted(r["assignment"].items())) for r in res}),
                           "device": card, "power_limit_w": watts}), flush=True)
+    return 0
+
+
+def param_sweep(args, families):
+    """The --sweep leg: N problems x P parameter sets, as one call, P calls and sequential solve() on a subset."""
+    dcops = problems(args.problems, args.seed)
+    import torch
+    if not torch.cuda.is_available():
+        print("batch_throughput: no CUDA device (the engines run on the GPU only)", file=sys.stderr)
+        return 2
+    from pydcop_b200.solve import solve, solve_batch
+
+    card, watts = torch.cuda.get_device_name(), power_limit_w()
+    n, P = len(dcops), args.sweep
+    subset = min(args.subset, n * P)
+    for kind in families:
+        sets = [dict(s, stop_cycle=args.stop_cycle) for s in SWEEPS[kind](P)]
+        probs = [d for d in dcops for _ in sets]           # problem-major, then set
+        params = [s for _ in dcops for s in sets]
+        kw = dict(precision=args.precision, seed=args.seed)
+        solve(dcops[0], kind, sets[0], **kw)               # warm-up: module loads, allocator
+        solve_batch(probs[:2 * P], kind, params[:2 * P], **kw)
+        best = {"one": float("inf"), "per_set": float("inf"), "sequential": float("inf")}
+        out = {}
+
+        def one():
+            out["one"] = solve_batch(probs, kind, params, **kw)
+
+        def per_set():
+            res = [None] * len(probs)
+            for j, s in enumerate(sets):
+                for i, r in enumerate(solve_batch(dcops, kind, s, **kw)):
+                    res[i * P + j] = r
+            out["per_set"] = res
+
+        def sequential():
+            out["sequential"] = [solve(d, kind, s, **kw) for d, s in zip(probs[:subset], params[:subset])]
+
+        arms = [("one", one), ("per_set", per_set), ("sequential", sequential)]
+        for k in range(max(1, args.repeats)):
+            for name, fn in arms[k % 3:] + arms[:k % 3]:   # rotated, so no arm always runs first
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                fn()
+                best[name] = min(best[name], time.perf_counter() - t0)
+        equal = (all(_same(r, s) for r, s in zip(out["one"], out["per_set"]))
+                 and all(_same(r, s) for r, s in zip(out["one"][:subset], out["sequential"])))
+        print(json.dumps({"workload": "random_factor_graph(100, 3, 150, 2, noise=0) x parameter sets", "family": kind,
+                          "precision": args.precision, "stop_cycle": args.stop_cycle, "problems": n, "sets": P,
+                          "sweep": [{k: v for k, v in s.items() if k != "stop_cycle"} for s in sets],
+                          "one_call_problems_per_s": n * P / best["one"],
+                          "per_set_calls_problems_per_s": n * P / best["per_set"],
+                          "sequential_subset": subset, "sequential_problems_per_s": subset / best["sequential"],
+                          "speedup_one_vs_per_set": best["per_set"] / best["one"],
+                          "one_call_ingest_s": out["one"][0]["ingest_time"], "repeats": args.repeats,
+                          "all_equal": equal, "device": card, "power_limit_w": watts}), flush=True)
     return 0
 
 
