@@ -993,6 +993,16 @@ const char *fg_trace_last_error(fg_trace_t tr);
 int fg_trace_start(fg_trace_t tr, void *stream);
 /* rows enqueued since fg_trace_start (a host count: no synchronisation) */
 int fg_trace_rows(fg_trace_t tr, int64_t *n_rows);
+/* Keep, per segment, the best row the trace records and the values of that cycle (the anytime result of a run):
+ * the first record sets it, a later row replaces it only when strictly better (fewer violations; at equal
+ * violations a cost < the best's in min mode, > in max mode; a NaN cost never beats a non-NaN one), so ties keep
+ * the earlier cycle.  dev_best: [n_seg * 2] doubles (cost, violations), the row's own; dev_best_cycle: [n_seg]
+ * int64, 0 = none yet, else the record number (1-based, counted since this call, NOT reset by fg_trace_start);
+ * dev_best_value: [n_vars] int32, internal order, the values the record summed.  Resets them on `stream`.  All three
+ * NULL: detach.  A record then adds at most one launch (the values of the segments it improved), counted by the
+ * trace; a full trace records, and so keeps, nothing. */
+int fg_trace_set_best(fg_trace_t tr, int32_t mode_max, double *dev_best, int64_t *dev_best_cycle,
+                      int32_t *dev_best_value, void *stream);
 /* Attach `tr` (NULL: detach) to a handle of the same device, precision and variable count.  Records the values of
  * MaxSum's dev_value, DSA's dev_value[cur], MGM's and MGM-2's dev_value, and GDBA's, DBA's and MixedDSA's
  * dev_value[cycle % 2]; the sharded step loops record nothing. */

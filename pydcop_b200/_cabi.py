@@ -368,6 +368,7 @@ SYMBOLS = {
     "fg_trace_last_error": (C.c_char_p, [P]),
     "fg_trace_start": (C.c_int, [P, P]),
     "fg_trace_rows": (C.c_int, [P, C.POINTER(C.c_int64)]),
+    "fg_trace_set_best": (C.c_int, [P, C.c_int32, P, P, P, P]),
     "fg_maxsum_set_trace": (C.c_int, [P, P]),
     "fg_dsa_set_trace": (C.c_int, [P, P]),
     "fg_mgm_set_trace": (C.c_int, [P, P]),

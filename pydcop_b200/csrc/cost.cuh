@@ -1,6 +1,6 @@
 // The per-factor and per-variable terms of the solution cost (dcop.py:319-367), shared by fg_solution_cost's kernels
-// and the trace record (engine.cu).  __host__ __device__, so tests/hostshim/cost_host.cpp runs the same code on the
-// CPU.  A term is (cost, violation): an entry equal to `infinity` (compared in the tables' precision) is one
+// and the trace record (engine.cu), and the rule that keeps a trace's best row.  __host__ __device__, so
+// tests/hostshim/cost_host.cpp and best_host.cpp run the same code on the CPU.  A term is (cost, violation): an entry equal to `infinity` (compared in the tables' precision) is one
 // violation, any other entry is summed.
 #pragma once
 #include <stdint.h>
@@ -32,6 +32,17 @@ __host__ __device__ inline int cost_factor_lane(const fg_class_t &c, int f, cons
   for (int i = c.arity - 1; i >= 0; --i) { idx += (int64_t)value[edge_var[e0 + i]] * stride; stride *= c.dom[i]; }
   cost_term<T>(tables[c.table_base + (int64_t)f * c.table_size + idx], infinity, cst, viol);
   return s;
+}
+
+// The anytime rule of fg_trace_set_best: a recorded (cost, violations) row replaces the best kept so far only when it
+// is strictly better, so ties keep the earlier cycle.  Fewer violations win; at equal violations the cost decides
+// (`<` in min mode, `>` in max mode), a NaN cost never beats a non-NaN one and any non-NaN cost beats a NaN best.
+__host__ __device__ inline bool best_better(double cost, double viol, double best_cost, double best_viol,
+                                            int32_t mode_max) {
+  if (viol != best_viol) return viol < best_viol;
+  if (cost != cost) return false;
+  if (best_cost != best_cost) return true;
+  return mode_max ? cost > best_cost : cost < best_cost;
 }
 
 // variable v (v >= n_vars: nothing): its own cost at its value, as cost_factor_lane

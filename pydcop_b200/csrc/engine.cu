@@ -936,23 +936,37 @@ extern "C" int fg_solution_cost_segmented(int32_t precision, int32_t n_classes, 
 // ---------------------------------------------------------------------------------------------
 constexpr int kTraceBlock = 128;
 
+// fg_trace_set_best's state, passed to the record by value; best == nullptr: no best is kept
+struct fg_trace_best {
+  double *best = nullptr;        // [n_seg * 2] (cost, violations) of each segment's best row
+  int64_t *cycle = nullptr;      // [n_seg] its record number, 0 = none yet
+  int32_t *value = nullptr;      // [n_vars] the values of that record
+  int32_t *improved = nullptr;   // [1 + n_seg]: [0] some segment improved in the last record, [1 + s] segment s did
+  int64_t record = 0;            // records since fg_trace_set_best (the number of the one being enqueued)
+  int32_t mode_max = 0;
+};
+
 struct fg_trace : fg_handle_base {
   fg_trace_desc_t d;
   int2 *dev_map = nullptr;       // per block: (class, first factor), or (-1, first variable)
   unsigned *dev_ticket = nullptr;
+  int32_t *dev_improved = nullptr;   // fg_trace_best::improved, allocated by the first fg_trace_set_best
   unsigned n_blocks = 0;
   int64_t rows = 0;              // records enqueued since fg_trace_start
+  fg_trace_best best;
 };
 
 // Every block covers kTraceBlock factors of one class or kTraceBlock variables (map[blockIdx.x]) and adds its warps'
 // runs into `row` as fg_solution_cost's kernels do; the last block to finish stamps the row and resets the ticket.
+// With a best kept, that block then compares the complete row with every segment's best (best_better) and flags the
+// segments it replaced for k_trace_best_values.
 template <typename T>
 __global__ void __launch_bounds__(kTraceBlock)
 k_trace_record(const fg_class_t *__restrict__ classes, const int2 *__restrict__ map, const T *__restrict__ tables,
                const int32_t *__restrict__ edge_var, const int32_t *__restrict__ value, const T *__restrict__ unary,
                const int64_t *__restrict__ unary_off, int n_vars, T infinity, const int32_t *__restrict__ factor_seg,
                const int32_t *__restrict__ var_seg, int32_t n_seg, double *__restrict__ row,
-               int64_t *__restrict__ stamp, unsigned *__restrict__ ticket) {
+               int64_t *__restrict__ stamp, unsigned *__restrict__ ticket, fg_trace_best kb) {
   const int2 b = map[blockIdx.x];
   double cst = 0.0, viol = 0.0;
   const int s = b.x >= 0 ? cost_factor_lane<T>(classes[b.x], b.y + (int)threadIdx.x, tables, edge_var, value, nullptr,
@@ -962,11 +976,42 @@ k_trace_record(const fg_class_t *__restrict__ classes, const int2 *__restrict__ 
   cost_warp_add(cst, viol, s, factor_seg != nullptr, row);
   __threadfence();   // this thread's adds are visible before its block takes a ticket
   __syncthreads();
-  if (threadIdx.x == 0 && atomicAdd(ticket, 1u) == gridDim.x - 1) {
-    __threadfence();
+  __shared__ bool last;
+  if (threadIdx.x == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  if (threadIdx.x == 0) {
     *stamp = (int64_t)global_timer_ns();
     *ticket = 0;
   }
+  if (!kb.best) return;
+  bool mine = false;
+  for (int k = threadIdx.x; k < n_seg; k += kTraceBlock) {
+    const double c = __ldcg(row + 2 * k), v = __ldcg(row + 2 * k + 1);   // the other blocks' adds, from L2
+    const bool up = kb.cycle[k] == 0 || best_better(c, v, kb.best[2 * k], kb.best[2 * k + 1], kb.mode_max);
+    if (up) {
+      kb.best[2 * k] = c;
+      kb.best[2 * k + 1] = v;
+      kb.cycle[k] = kb.record;
+    }
+    kb.improved[1 + k] = up;
+    mine |= up;
+  }
+  const int any = __syncthreads_or(mine);
+  if (threadIdx.x == 0) kb.improved[0] = any;
+}
+
+// the values of every variable whose segment the record just improved; after a record that improved nothing every
+// block returns at once
+__global__ void k_trace_best_values(const int32_t *__restrict__ value, const int32_t *__restrict__ var_seg,
+                                    int32_t n_seg, int n_vars, const int32_t *__restrict__ improved,
+                                    int32_t *__restrict__ best_value) {
+  if (!improved[0]) return;
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n_vars) return;
+  const int s = cost_seg(v, var_seg, n_seg);
+  if (s >= 0 && improved[1 + s]) best_value[v] = value[v];
 }
 
 __global__ void k_trace_stamp(int64_t *stamp) { *stamp = (int64_t)global_timer_ns(); }
@@ -1019,6 +1064,7 @@ extern "C" int fg_trace_destroy(fg_trace_t h) {
     fg_device_scope on(h);
     if (h->dev_map) cudaFree(h->dev_map);
     if (h->dev_ticket) cudaFree(h->dev_ticket);
+    if (h->dev_improved) cudaFree(h->dev_improved);
   }
   return fg_close(h);
 }
@@ -1044,6 +1090,37 @@ extern "C" int fg_trace_rows(fg_trace_t h, int64_t *n_rows) {
   return FG_OK;
 }
 
+extern "C" int fg_trace_set_best(fg_trace_t h, int32_t mode_max, double *dev_best, int64_t *dev_best_cycle,
+                                 int32_t *dev_best_value, void *stream) {
+  if (!h) return FG_ERR_ARG;
+  auto refuse = [&](const char *why) { snprintf(h->err, sizeof(h->err), "%s", why); return FG_ERR_ARG; };
+  if (mode_max != 0 && mode_max != 1) return refuse("mode_max must be 0 (min) or 1 (max)");
+  const int given = (dev_best != nullptr) + (dev_best_cycle != nullptr) + (dev_best_value != nullptr);
+  if (given != 0 && given != 3) return refuse("give dev_best, dev_best_cycle and dev_best_value together, or none");
+  FG_ON_DEVICE(h);
+  if (!given) {
+    h->best = fg_trace_best();
+    return FG_OK;
+  }
+  int rc = fg_check_resident(h, {fg_field{"dev_best", dev_best}, fg_field{"dev_best_cycle", dev_best_cycle},
+                                 fg_field{"dev_best_value", dev_best_value}});
+  if (rc != FG_OK) return rc;
+  const size_t n_seg = (size_t)h->d.n_seg;
+  if (!h->dev_improved) CUDA_TRY(h, cudaMalloc(&h->dev_improved, sizeof(int32_t) * (n_seg + 1)));
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_TRY(h, cudaMemsetAsync(dev_best, 0, sizeof(double) * 2 * n_seg, st));
+  CUDA_TRY(h, cudaMemsetAsync(dev_best_cycle, 0, sizeof(int64_t) * n_seg, st));
+  if (h->d.n_vars) CUDA_TRY(h, cudaMemsetAsync(dev_best_value, 0, sizeof(int32_t) * (size_t)h->d.n_vars, st));
+  CUDA_TRY(h, cudaMemsetAsync(h->dev_improved, 0, sizeof(int32_t) * (n_seg + 1), st));
+  h->best.best = dev_best;
+  h->best.cycle = dev_best_cycle;
+  h->best.value = dev_best_value;
+  h->best.improved = h->dev_improved;
+  h->best.record = 0;
+  h->best.mode_max = mode_max;
+  return FG_OK;
+}
+
 int fg_trace_check(const fg_trace *tr, int device, int32_t precision, int32_t n_vars, char *err, size_t n) {
   if (tr->device != device) { snprintf(err, n, "the trace belongs to device %d, the handle to %d", tr->device, device); return FG_ERR_ARG; }
   if (tr->d.precision != precision) { snprintf(err, n, "trace precision differs from the handle's"); return FG_ERR_ARG; }
@@ -1057,17 +1134,24 @@ static void trace_record_t(fg_trace *h, const int32_t *value, cudaStream_t st) {
   k_trace_record<T><<<h->n_blocks, kTraceBlock, 0, st>>>(
       h->dev_classes, h->dev_map, (const T *)d.dev_tables, d.dev_edge_var, value, (const T *)d.dev_unary,
       d.dev_unary_off, d.n_vars, (T)d.infinity, d.dev_factor_seg, d.dev_var_seg, d.n_seg,
-      d.dev_rows + 2 * (int64_t)d.n_seg * h->rows, d.dev_stamp + h->rows + 1, h->dev_ticket);
+      d.dev_rows + 2 * (int64_t)d.n_seg * h->rows, d.dev_stamp + h->rows + 1, h->dev_ticket, h->best);
 }
 
-// runs on the trace's device, which fg_trace_check made sure is the calling handle's
+// runs on the trace's device, which fg_trace_check made sure is the calling handle's.  The best values are copied
+// right behind the record on the same stream, before the step loop can overwrite `value` (a double buffer).
 int fg_trace_record(fg_trace *h, const int32_t *value, cudaStream_t st) {
   if (h->rows >= h->d.capacity) return FG_OK;   // full: the caller attaches a fresh trace
+  if (h->best.best) ++h->best.record;
   if (h->d.precision == FG_F64) trace_record_t<double>(h, value, st);
   else trace_record_t<float>(h, value, st);
+  ++h->launches;
+  if (h->best.best && h->d.n_vars) {
+    k_trace_best_values<<<blocks_for(h->d.n_vars, 256), 256, 0, st>>>(value, h->d.dev_var_seg, h->d.n_seg,
+                                                                      h->d.n_vars, h->best.improved, h->best.value);
+    ++h->launches;
+  }
   CUDA_TRY(h, cudaGetLastError());
   ++h->rows;
-  ++h->launches;
   return FG_OK;
 }
 

@@ -216,11 +216,14 @@ class _EngineBase:
         v_int = _per_var(L, np.asarray(seg_var, dtype=np.int32)[L.var_order], np.int32)
         return self._dev(f_int, torch.int32), self._dev(v_int, torch.int32), int(n_seg)
 
-    def start_trace(self, capacity, infinity=float("inf"), unary=None, seg=None):
+    def start_trace(self, capacity, infinity=float("inf"), unary=None, seg=None, best=False, rows=True):
         """Record (cost, violations) of the current values after every cycle step() runs from now on, on the device
         and without synchronising (fg_trace_*): solution_cost's sums, or with seg = (seg_factor, seg_var, n_seg) as
         in solution_costs_segmented, solution_costs_segmented's.  `capacity`: rows per trace block; a full block is
-        moved aside on the device and the trace goes on, so any number of cycles is recorded."""
+        moved aside on the device and the trace goes on, so any number of cycles is recorded.
+        best: also keep each segment's best recorded cycle and its values on the device (fg_trace_set_best, in the
+        engine's mode), read by best().  rows=False (with best): the rows are only scratch for the best; a full
+        block is restarted without a copy and trace() has nothing to give."""
         self.stop_trace()
         L = self.layout
         with torch.cuda.device(self.device):
@@ -228,6 +231,7 @@ class _EngineBase:
             segd = None if seg is None else self._segments(*seg)
             n_seg = 1 if seg is None else segd[2]
             capacity = max(1, int(capacity))
+            rows_kept = rows or not best
             rows = torch.zeros(capacity * n_seg * 2, dtype=torch.float64, device=self.device)
             stamp = torch.zeros(capacity + 1, dtype=torch.int64, device=self.device)
             un = self._unary_dev(unary)
@@ -246,8 +250,16 @@ class _EngineBase:
                 self.lib.fg_trace_destroy(h)
                 raise EngineError(f"fg_trace_create failed (rc={rc}): {msg}")
             self._trace = {"h": h, "capacity": capacity, "n_seg": n_seg, "rows": rows, "stamp": stamp,
-                           "keep": (un, segd), "done": []}
+                           "keep": (un, segd), "done": [], "keep_rows": bool(rows_kept), "best": None}
             self._trace_check(self.lib.fg_trace_start(h, self._stream()), "fg_trace_start")
+            if best:
+                b = (torch.zeros(2 * n_seg, dtype=torch.float64, device=self.device),
+                     torch.zeros(n_seg, dtype=torch.int64, device=self.device),
+                     torch.zeros(max(L.n_vars, 1), dtype=torch.int32, device=self.device))
+                self._trace_check(self.lib.fg_trace_set_best(h, int(getattr(self._desc, "mode_max", 0)), _ptr(b[0]),
+                                                             _ptr(b[1]), _ptr(b[2]), self._stream()),
+                                  "fg_trace_set_best")
+                self._trace["best"] = b
             self._check(self._fn("set_trace")(self._h, h), f"fg_{self.FAMILY}_set_trace")
         return self
 
@@ -264,9 +276,11 @@ class _EngineBase:
         return n.value
 
     def _trace_rotate(self):
-        """A full block: its rows and stamps copied aside on the stream, the trace restarted behind them."""
+        """A full block: its rows and stamps copied aside on the stream (not when the rows are only the best's
+        scratch), the trace restarted behind them; the best is kept outside the rows and survives."""
         tr = self._trace
-        tr["done"].append((tr["rows"].clone(), tr["stamp"].clone(), self._trace_rows()))
+        if tr["keep_rows"]:
+            tr["done"].append((tr["rows"].clone(), tr["stamp"].clone(), self._trace_rows()))
         self._trace_check(self.lib.fg_trace_start(tr["h"], self._stream()), "fg_trace_start")
 
     def trace(self):
@@ -276,6 +290,8 @@ class _EngineBase:
         tr = self._trace
         if tr is None:
             raise EngineError("no trace started")
+        if not tr["keep_rows"]:
+            raise EngineError("the trace keeps no rows: it was started with rows=False")
         with torch.cuda.device(self.device):
             blocks = tr["done"] + [(tr["rows"], tr["stamp"], self._trace_rows())]
             t0 = int(blocks[0][1][0].item())
@@ -284,6 +300,21 @@ class _EngineBase:
         out = np.concatenate(rows) if rows else np.zeros((0, tr["n_seg"], 2))
         return {"cost": out[:, :, 0].copy(), "violation": out[:, :, 1].astype(np.int64),
                 "time": (np.concatenate(stamps).astype(np.int64) - t0) * 1e-9}
+
+    def best(self):
+        """The best cycle of each segment since start_trace(best=True) (fg_trace_set_best's rule: fewer violations,
+        then a strictly better cost in the engine's mode, ties to the earlier cycle): cycle int64[n_seg] (the trace's
+        numbering, 1 = the first cycle recorded; 0 = none), cost float64[n_seg] and violation int64[n_seg] (that
+        row's), and value, the values after that cycle in canonical variable order (each variable's from its own
+        segment's best cycle).  Synchronises; still readable after stop_trace."""
+        tr = self._trace
+        if tr is None or tr["best"] is None:
+            raise EngineError("no best kept: start_trace(best=True) first")
+        with torch.cuda.device(self.device):
+            b, cycle, value = (t.cpu().numpy() for t in tr["best"])
+        b = b.reshape(-1, 2)
+        return {"cycle": cycle.astype(np.int64), "cost": b[:, 0].copy(), "violation": b[:, 1].astype(np.int64),
+                "value": self.layout.vars_to_canonical(value[:self.layout.n_vars])}
 
     def stop_trace(self):
         """Detach the trace: the step loop is the plain one again.  trace() still reads what was recorded."""

@@ -226,7 +226,7 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
           on_cycle: Optional[Callable[[int, np.ndarray], None]] = None,
           engine_factory: Optional[Callable] = None, distributed: Optional[bool] = None,
           partition="auto", halo: str = "auto", sharded_kwargs: Optional[Dict[str, Any]] = None,
-          trace: bool = False) -> Dict[str, Any]:
+          trace: bool = False, best: bool = False) -> Dict[str, Any]:
     """Run `algo` on `problem` and return pyDcop's result dict.
 
     Under `torchrun` (torch.distributed initialised, world size > 1; `distributed` None = detect)
@@ -250,6 +250,11 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
                  the step loop, without a host round trip; "time" is seconds on the device timer since the first
                  cycle was enqueued.  The last entry's cost and violation are the result's.  Single-GPU iterative
                  algorithms only (not dpop, syncbb or torchrun).
+    best         the result gains "best": {"cycle", "cost", "violation", "assignment"}, the run's best cycle (the
+                 anytime result): of the cycles the trace numbers, the first with the fewest violations and, among
+                 those, the strictly best cost in the problem's objective; later ties do not replace it.  Kept on the
+                 device inside the step loop with or without `trace`; None when no cycle ran.  The same algorithms
+                 as `trace`.
     SyncBB has no cycles to chunk: it ignores `chunk` and never calls `on_cycle` (a variable may have no value
     until the search ends).
     """
@@ -258,6 +263,8 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
         distributed = _under_torchrun()
     if trace:
         _check_trace(kind, distributed)
+    if best:
+        _check_trace(kind, distributed, "best")
     if distributed and seed is None:
         seed = 0
     t0 = time.perf_counter()
@@ -294,7 +301,7 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
     if kind == "syncbb":
         return _finish_syncbb(engine, dcop, deadline, infinity, precision, t0, t_packed)
     tracer = _Trace(engine, stop_cycle, infinity, dcop.arrays["unary"], None,
-                    lambda idx: [solution_cost(dcop, idx, infinity)]) if trace else None
+                    lambda idx: [solution_cost(dcop, idx, infinity)], best, trace, mode) if trace or best else None
     cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline, distributed, on_cycle, kind == "dba",
                                 tracer.after_cycle if tracer else None)
     if kind == "dba":                      # the rounds that changed the state
@@ -313,7 +320,11 @@ def solve(problem, algo: str = "maxsum", algo_params: Optional[Dict[str, Any]] =
            "h2d_bytes": int(getattr(getattr(engine, "engine", engine), "h2d_bytes", 0)),
            "d2h_bytes": int(len(idx) * 12 + 16)}
     if tracer is not None:
-        out["trace"] = tracer.result(cycle if kind == "dba" else None)[0]
+        traces, kept = tracer.finish(cycle if kind == "dba" else None)
+        if trace:
+            out["trace"] = traces[0]
+        if best:
+            out["best"] = _best_entry(dcop, kept[0][0], kept[1])
     return out
 
 
@@ -375,27 +386,46 @@ def _run_cycles(engine, stop_cycle, chunk, deadline, distributed=False, on_cycle
 TRACE_BYTES = 64 << 20   # device rows of one trace block, at most: a block of n_seg problems holds fewer cycles
 
 
-def _check_trace(kind, distributed):
+def _check_trace(kind, distributed, what="trace"):
     if kind in ("dpop", "syncbb"):
-        raise ValueError(f"trace: {kind} has no cycles to trace")
+        raise ValueError(f"{what}: {kind} has no cycles to trace")
     if distributed:
-        raise ValueError("trace: traces are recorded on one GPU: start the run without torchrun")
+        raise ValueError(f"{what}: traces are recorded on one GPU: start the run without torchrun")
+
+
+def best_better(cost, viol, best_cost, best_viol, mode_max):
+    """csrc/cost.cuh's best_better, the rule the device keeps a trace's best row by, for the host trace of the
+    engine seam: strictly fewer violations, or equal ones and a strictly better cost (a NaN cost never better)."""
+    if viol != best_viol:
+        return viol < best_viol
+    if cost != cost:
+        return False
+    if best_cost != best_cost:
+        return True
+    return cost > best_cost if mode_max else cost < best_cost
 
 
 class _Trace:
     """The cost of every cycle of one engine run: recorded on the device (engine.start_trace), or for an engine
     without one (the CPU tests' engine seam) on the host after every single cycle: host_costs(value_index) ->
-    [(violation, cost)] per segment, with solution_cost."""
+    [(violation, cost)] per segment, with solution_cost.  best: each segment's best cycle and its values are kept too
+    (var_start: the segments' variable ranges, canonical order); rows=False: the rows serve the best only."""
 
-    def __init__(self, engine, stop_cycle, infinity, unary, seg, host_costs):
+    def __init__(self, engine, stop_cycle, infinity, unary, seg, host_costs, best=False, rows=True, mode="min",
+                 var_start=None):
         self.engine, self.rows, self.t0 = engine, [], time.perf_counter()
         self.n_seg = 1 if seg is None else seg[2]
+        self.keep_best, self.keep_rows = best, rows
         self.device = hasattr(engine, "start_trace")
         if self.device:
             want = stop_cycle or 1024
-            engine.start_trace(max(1, min(want, TRACE_BYTES // (16 * self.n_seg))), infinity, unary, seg)
+            engine.start_trace(max(1, min(want, TRACE_BYTES // (16 * self.n_seg))), infinity, unary, seg, best=best,
+                               rows=rows)
         else:
             self.host_costs, self.cycle = host_costs, getattr(engine, "cycle", 0)
+            self.mode_max, self.var_start = mode == "max", var_start
+            self.best_row = [(0, 0.0, 0)] * self.n_seg   # (cycle, cost, violation); cycle 0 = none
+            self.best_value = None
         # what _run_cycles calls after every single cycle: nothing when the device records inside the step loop
         self.after_cycle = None if self.device else self._host_row
 
@@ -405,13 +435,33 @@ class _Trace:
             return
         self.cycle = c
         t = time.perf_counter() - self.t0
-        self.rows.append((t, self.host_costs(_indices(self.engine))))
+        idx = _indices(self.engine)
+        costs = self.host_costs(idx)
+        self.rows.append((t, costs))
+        if not self.keep_best:
+            return
+        n = len(self.rows)
+        if self.best_value is None:
+            self.best_value = np.zeros_like(idx)
+        for k, (v, cost) in enumerate(costs):
+            b = self.best_row[k]
+            if b[0] == 0 or best_better(float(cost), float(v), b[1], float(b[2]), self.mode_max):
+                self.best_row[k] = (n, float(cost), int(v))
+                lo, hi = (0, len(idx)) if self.var_start is None else (self.var_start[k], self.var_start[k + 1])
+                self.best_value[lo:hi] = idx[lo:hi]
+
+    def best(self):
+        """(cycle, cost, violation) of every segment's best cycle (cycle 0: none ran) and the values of the best
+        cycles, canonical order."""
+        if self.device:
+            b = self.engine.best()
+            return [(int(c), float(x), int(v)) for c, x, v in zip(b["cycle"], b["cost"], b["violation"])], b["value"]
+        return self.best_row, _indices(self.engine) if self.best_value is None else self.best_value
 
     def result(self, n_cycles=None):
         """One trace dict per segment; `n_cycles`: keep the first n (DBA: the rounds that changed the state)."""
         if self.device:
             tr = self.engine.trace()
-            self.engine.stop_trace()
             t, cost, viol = tr["time"], tr["cost"], tr["violation"]
         else:
             t = np.array([r[0] for r in self.rows], dtype=np.float64)
@@ -421,6 +471,22 @@ class _Trace:
         return [{"cycle": list(range(1, n + 1)), "time": [float(x) for x in t[:n]],
                  "cost": [float(x) for x in cost[:n, k]], "violation": [int(x) for x in viol[:n, k]]}
                 for k in range(self.n_seg)]
+
+    def finish(self, n_cycles=None):
+        """(result(n_cycles) or None without rows, best() or None without a best), the device trace stopped."""
+        out = (self.result(n_cycles) if self.keep_rows else None, self.best() if self.keep_best else None)
+        if self.device:
+            self.engine.stop_trace()
+        return out
+
+
+def _best_entry(dcop, row, value):
+    """A result's "best": its cycle, cost, violation and assignment (value: the problem's slice); None when no cycle
+    ran."""
+    cycle, cost, violation = row
+    if not cycle:
+        return None
+    return {"cycle": cycle, "cost": cost, "violation": violation, "assignment": dcop.assignment(value)}
 
 
 BATCHED = ("maxsum", "dsa", "adsa", "mgm", "mgm2", "gdba", "mixeddsa")
@@ -441,7 +507,8 @@ def solve_batch(problems, algo: str, algo_params: Union[None, Dict[str, Any], Se
                 precision: str = "f32", device=None, seed: Union[None, int, Sequence[int]] = None,
                 infinity: float = float("inf"),
                 chunk: int = 50, max_vars: int = batch.MAX_BATCH_VARS,
-                engine_factory: Optional[Callable] = None, trace: bool = False) -> List[Dict[str, Any]]:
+                engine_factory: Optional[Callable] = None, trace: bool = False,
+                best: bool = False) -> List[Dict[str, Any]]:
     """Run `algo` on every problem of `problems` and return one result dict per problem, in input order, with
     solve()'s keys.
 
@@ -471,6 +538,8 @@ def solve_batch(problems, algo: str, algo_params: Union[None, Dict[str, Any], Se
     parameter set; else the group's sets are params["psets"]).
     trace: every result gains solve()'s "trace", cut out of its group's per-problem record (its times are the
     group's); the trace of a problem whose group never started is empty.
+    best: every result gains solve()'s "best", kept per problem on the device (its cycle in the trace's numbering);
+    None for a problem whose group never started.
     """
     kind = ALGOS.get(algo)
     if kind in NOT_BATCHED:
@@ -537,13 +606,13 @@ def solve_batch(problems, algo: str, algo_params: Union[None, Dict[str, Any], Se
         ingest_time += time.perf_counter() - t_group
         engine.init()
         tracer = None
-        if trace:
+        if trace or best:
             tracer = _Trace(engine, stop_cycle, infinity, u.unary, (u.seg_factor, u.seg_var, len(members)),
                             lambda idx: [solution_cost(dcops[i], idx[u.var_start[k]:u.var_start[k + 1]], infinity)
-                                         for k, i in enumerate(members)])
+                                         for k, i in enumerate(members)], best, trace, mode, u.var_start)
         cycle, status = _run_cycles(engine, stop_cycle, chunk, deadline,
                                     after_cycle=tracer.after_cycle if tracer else None)
-        traces = tracer.result() if tracer is not None else None
+        traces, kept = tracer.finish() if tracer is not None else (None, None)
         idx = _indices(engine)
         if hasattr(engine, "solution_costs_segmented"):   # reduced per problem on the device
             costs, violations = engine.solution_costs_segmented(u.seg_factor, u.seg_var, len(members), infinity,
@@ -560,6 +629,8 @@ def solve_batch(problems, algo: str, algo_params: Union[None, Dict[str, Any], Se
                           "d2h_bytes": int(len(v) * 12 + 16)}
             if traces is not None:
                 results[i]["trace"] = traces[k]
+            if kept is not None:
+                results[i]["best"] = _best_entry(dcops[i], kept[0][k], kept[1][u.var_start[k]:u.var_start[k + 1]])
     total = time.perf_counter() - t0
     for r in results:
         r.update(time=total, ingest_time=ingest_time)
@@ -659,6 +730,9 @@ def main(argv=None):
     ap.add_argument("--collect_on", choices=["cycle_change"], default=None,
                     help="cycle_change: the solution cost of EVERY cycle, recorded on the device inside the step loop "
                          "(solve(trace=True)): --run_metrics gets one row per cycle, --batch entries a \"trace\"")
+    ap.add_argument("--best", action="store_true",
+                    help="add the run's best cycle (solve(best=True)): \"best\" with its cycle, cost, violation and "
+                         "assignment, kept on the device; in every --batch entry too")
     ap.add_argument("--partition", default="auto", choices=["auto", "blocks", "multilevel"],
                     help="under torchrun: how the variables are split over the GPUs")
     ap.add_argument("--batch", action="store_true",
@@ -707,7 +781,7 @@ def main(argv=None):
     res = solve(dcop, args.algo, params, args.timeout, args.precision, seed=args.seed,
                 infinity=args.infinity, partition=args.partition,
                 chunk=max(1, args.metrics_every) if host_rows else 50,
-                on_cycle=collect if host_rows else None, trace=trace)
+                on_cycle=collect if host_rows else None, trace=trace, best=args.best)
     if trace and args.run_metrics:
         tr = res.pop("trace")
         rows = [(c, t, cost, v, 0, 0, "RUNNING")
@@ -720,12 +794,19 @@ def main(argv=None):
             w.writerows(rows)
             w.writerow([res["cycle"], res["time"], res["cost"], res["violation"], 0, 0, res["status"]])
     if args.no_assignment:
-        res.pop("assignment")
+        _drop_assignment(res)
     if rank == 0:
         print(json.dumps(res, indent=2, sort_keys=True, default=str))
     if world > 1:
         dist.destroy_process_group()
     return 0
+
+
+def _drop_assignment(res):
+    """--no-assignment: the result without its assignments, the best cycle's included."""
+    res.pop("assignment")
+    if res.get("best"):
+        res["best"].pop("assignment")
 
 
 def _algo_params(ap, args):
@@ -763,7 +844,7 @@ def _main_batch(args, params, sweeps=()):
         return _main_sweep(args, params, sweeps)
     if args.iterations is None:
         res = solve_batch(args.dcop_files, args.algo, params, args.timeout, args.precision, seed=args.seed,
-                          infinity=args.infinity, trace=args.collect_on == "cycle_change")
+                          infinity=args.infinity, trace=args.collect_on == "cycle_change", best=args.best)
         for path, r in zip(args.dcop_files, res):
             r["problem"] = path
     else:
@@ -772,12 +853,12 @@ def _main_batch(args, params, sweeps=()):
         dcops = [load(path, base) for path in args.dcop_files]
         res = solve_batch([d for d in dcops for _ in range(n)], args.algo, params, args.timeout, args.precision,
                           seed=[base + r for _ in dcops for r in range(n)], infinity=args.infinity,
-                          trace=args.collect_on == "cycle_change")
+                          trace=args.collect_on == "cycle_change", best=args.best)
         for k, r in enumerate(res):
             r.update(problem=args.dcop_files[k // n], iteration=k % n, seed=base + k % n)
     for r in res:
         if args.no_assignment:
-            r.pop("assignment")
+            _drop_assignment(r)
     print(json.dumps(res, indent=2, sort_keys=True, default=str))
     return 0
 
@@ -795,14 +876,14 @@ def _main_sweep(args, params, sweeps):
     seeds = [base + r for _, _, r in entries] if args.iterations else args.seed
     res = solve_batch([dcops[f] for f, _, _ in entries], args.algo, [combos[c] for _, c, _ in entries],
                       args.timeout, args.precision, seed=seeds, infinity=args.infinity,
-                      trace=args.collect_on == "cycle_change")
+                      trace=args.collect_on == "cycle_change", best=args.best)
     checked = [check_params(ALGOS[args.algo], c) for c in combos]
     for (f, c, r), out in zip(entries, res):
         out.update(problem=args.dcop_files[f], algo_params=checked[c])
         if args.iterations:
             out.update(iteration=r, seed=base + r)
         if args.no_assignment:
-            out.pop("assignment")
+            _drop_assignment(out)
     print(json.dumps(res, indent=2, sort_keys=True, default=str))
     return 0
 

@@ -1,16 +1,18 @@
 #!/usr/bin/env python
-"""What the device cost trace (engine start_trace, solve(trace=True)) costs per cycle.
+"""What the device cost trace (engine start_trace, solve(trace=True)) and the best cycle kept with it
+(start_trace(best=True), solve(best=True)) cost per cycle.
 
-Three parts, each one JSON line with the card's name and power limit:
+Three parts, each one JSON line with the card's name, power limit and SM clock:
 
-1. `engines`: device time per cycle of the same engine stepped with and without a trace attached, CUDA events around
-   `--cycles` cycles after `--warmup`, the two arms alternating `--repeats` times (median and spread of each arm).
-   MaxSum on BASELINE.json's single-GPU configs (C2: 100k vars d=10 deg=4; C5: 50k arity-3 factors d=8) and DSA on C2
-   and C4's graph (1M vars d=20 deg=6) run on one GPU.
+1. `engines`: device time per cycle of the same engine stepped plain, with a trace attached, and with a trace that
+   also keeps the best cycle, CUDA events around `--cycles` cycles after `--warmup`, the three arms alternating
+   `--repeats` times (median and spread of each arm).  MaxSum on BASELINE.json's single-GPU configs (C2: 100k vars
+   d=10 deg=4; C5: 50k arity-3 factors d=8) and DSA on C2 and C4's graph (1M vars d=20 deg=6) run on one GPU
+   (`--cases` picks some of them).
 2. `batch`: tools/batch_throughput.py's workload (`--problems` x random_factor_graph(100, 3, 150, 2), stop_cycle 100)
-   through solve_batch with and without trace=True, per batched family: wall time of each (median of `--repeats`,
-   alternating), whether the results (assignment, status, cycle, cost, violation) are identical, and the per-cycle
-   device cost of one union engine with and without a trace as in part 1.
+   through solve_batch plain, with trace=True and with trace=True and best=True, per batched family: wall time of each
+   (median of `--repeats`, alternating), whether the results (assignment, status, cycle, cost, violation) are
+   identical in all three, and the per-cycle device cost of one union engine in the three arms as in part 1.
 3. `metrics_every_1`: wall time of the CLI's host-side metrics at every cycle (solve(chunk=1, on_cycle=...) with the
    numpy solution_cost, what `--run_metrics --metrics_every 1` does) against solve(trace=True), on C2 with MaxSum.
 
@@ -29,41 +31,60 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from gdba_throughput import power_limit_w  # noqa: E402
 
 
+def sm_clock_mhz():
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm,clocks.max.sm", "--format=csv,noheader,nounits",
+                            "-i", os.environ.get("CUDA_VISIBLE_DEVICES", "0").split(",")[0]],
+                           capture_output=True, text=True, timeout=30)
+        cur, top = (float(x) for x in r.stdout.strip().splitlines()[0].split(","))
+        return {"sm_clock_mhz": cur, "sm_clock_max_mhz": top}
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        return {"sm_clock_mhz": None, "sm_clock_max_mhz": None}
+
+
 def card():
     import torch
-    return {"gpu": torch.cuda.get_device_name(), "power_limit_w": power_limit_w()}
+    return {"gpu": torch.cuda.get_device_name(), "power_limit_w": power_limit_w(), **sm_clock_mhz()}
 
 
-def per_cycle_us(engine, cycles, warmup, traced, unary, seg=None):
+ARMS = ("plain", "traced", "best")   # no trace; a trace; a trace that also keeps the best cycle
+
+
+def per_cycle_us(engine, cycles, warmup, arm, unary, seg=None):
     """Device microseconds per cycle of `cycles` engine.step(1) calls (the solve() loop steps in chunks; one call per
-    cycle is the worst case for the host side and the same for both arms)."""
+    cycle is the worst case for the host side and the same for every arm)."""
     import torch
-    if traced:
-        engine.start_trace(cycles + warmup, float("inf"), unary, seg)
+    if arm != "plain":
+        engine.start_trace(cycles + warmup, float("inf"), unary, seg, best=arm == "best")
     engine.step(warmup)
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
     engine.step(cycles)
     b.record()
     b.synchronize()
-    if traced:
+    if arm != "plain":
         assert len(engine.trace()["time"]) == cycles + warmup
+        if arm == "best":
+            assert (engine.best()["cycle"] >= 1).all()
         engine.stop_trace()
     return a.elapsed_time(b) * 1e3 / cycles
 
 
 def engine_arms(make, unary, cycles, warmup, repeats, seg=None):
-    """Alternating plain / traced runs of fresh engines from make(); median and range of each arm, in us/cycle."""
-    arms = {"plain": [], "traced": []}
+    """Alternating plain / traced / best runs of fresh engines from make(); median and range of each arm, in
+    us/cycle."""
+    arms = {arm: [] for arm in ARMS}
     for _ in range(repeats):
-        for arm in ("plain", "traced"):
+        for arm in ARMS:
             e = make()
-            arms[arm].append(per_cycle_us(e, cycles, warmup, arm == "traced", unary, seg))
+            arms[arm].append(per_cycle_us(e, cycles, warmup, arm, unary, seg))
             e.close()
     out = {f"{k}_us_per_cycle": round(statistics.median(v), 2) for k, v in arms.items()}
     out.update({f"{k}_range_us": [round(min(v), 2), round(max(v), 2)] for k, v in arms.items()})
     out["overhead_us_per_cycle"] = round(out["traced_us_per_cycle"] - out["plain_us_per_cycle"], 2)
     out["overhead_pct"] = round(100 * out["overhead_us_per_cycle"] / out["plain_us_per_cycle"], 1)
+    out["best_over_trace_us_per_cycle"] = round(out["best_us_per_cycle"] - out["traced_us_per_cycle"], 2)
     return out
 
 
@@ -76,6 +97,8 @@ def part_engines(args):
              ("maxsum", "C5 50k arity-3 factors d=8", lambda: G.config_c5(0)),
              ("dsa", "C2 100k vars d=10 deg=4", lambda: G.config_c2(0)),
              ("dsa", "C4 1M vars d=20 deg=6 on one GPU", lambda: G.config_c4(0))]
+    if args.cases:
+        cases = [cases[int(i)] for i in args.cases.split(",")]
     for kind, name, gen in cases:
         inst = gen()
         L = build_layout(**inst)
@@ -90,26 +113,34 @@ def part_batch(args):
     from batch_throughput import problems
     from pydcop_b200 import batch
     from pydcop_b200.engine import make_engine
-    from pydcop_b200.solve import _var_inputs, solve_batch
+    from pydcop_b200.solve import _var_inputs, best_better, solve_batch
     dcops = problems(args.problems)
     families = args.families.split(",")
     keys = ("assignment", "status", "cycle", "cost", "violation")
     for kind in families:
         p = {"stop_cycle": 100}
         solve_batch(dcops[:20], kind, p, precision=args.precision, seed=1)     # warm-up, both arms
-        solve_batch(dcops[:20], kind, p, precision=args.precision, seed=1, trace=True)
-        times = {"plain": [], "traced": []}
+        solve_batch(dcops[:20], kind, p, precision=args.precision, seed=1, trace=True, best=True)
+        times = {arm: [] for arm in ARMS}
         same = True
         for _ in range(args.repeats):
-            for arm in ("plain", "traced"):
+            for arm in ARMS:
                 t = time.perf_counter()
-                res = solve_batch(dcops, kind, p, precision=args.precision, seed=1, trace=arm == "traced")
+                res = solve_batch(dcops, kind, p, precision=args.precision, seed=1, trace=arm != "plain",
+                                  best=arm == "best")
                 times[arm].append(time.perf_counter() - t)
                 if arm == "plain":
                     want = [{k: r[k] for k in keys} for r in res]
                 else:
                     same &= want == [{k: r[k] for k in keys} for r in res]
                     same &= all(len(r["trace"]["cycle"]) == len(res[0]["trace"]["cycle"]) > 0 for r in res)
+                if arm == "best":
+                    same &= all(r["best"] is not None and 1 <= r["best"]["cycle"] <= r["cycle"] for r in res)
+                    # problems whose best cycle beats the last one, both as the trace recorded them (the result's
+                    # own cost is summed in another order)
+                    gains = sum(best_better(r["best"]["cost"], r["best"]["violation"], r["trace"]["cost"][-1],
+                                            r["trace"]["violation"][-1], d.objective == "max")
+                                for d, r in zip(dcops, res))
         members = list(range(len(dcops)))
         u = batch.build_union(dcops, members, lambda d: _var_inputs(kind, d, "min"), 0.0, 1)
         L = batch.union_layout(u, dcops)
@@ -120,7 +151,9 @@ def part_batch(args):
         print(json.dumps(dict(part="batch", algo=kind, problems=len(dcops), precision=args.precision,
                               plain_s=round(statistics.median(times["plain"]), 4),
                               traced_s=round(statistics.median(times["traced"]), 4),
-                              results_identical=bool(same), union_engine=dev, **card())), flush=True)
+                              best_s=round(statistics.median(times["best"]), 4),
+                              results_identical=bool(same), problems_best_before_last=int(gains),
+                              union_engine=dev, **card())), flush=True)
 
 
 def part_metrics_every_1(args):
@@ -160,6 +193,7 @@ def main(argv=None):
     ap.add_argument("--cycles", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--repeats", type=int, default=5)
+    ap.add_argument("--cases", default="", help="engines part: comma-separated indices into its cases (default all)")
     ap.add_argument("--problems", type=int, default=1000)
     ap.add_argument("--families", default="maxsum,dsa,adsa,mgm,mgm2,gdba,mixeddsa")
     ap.add_argument("--metric-cycles", type=int, default=100)
